@@ -8,12 +8,12 @@ composite + MSE against the target images, and back-propagate to every leaf para
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload dtu|bmvs|stress]     our arm (torchrun launches N ranks)
   python bench.py --impl reference ...                            the reference's algorithm on the host cores (oracle port)
+  python bench.py ... --dump-outputs DIR                          also write the last timed step's loss and gradients as .npy
 
 Workloads = BASELINE.json configs: dtu = configs[1]/[2] (the metric's configuration and the default), bmvs = configs[3],
 stress = configs[4].  N > 1 is STRONG scaling: the step's views are split over the ranks at (view, 16-row band) granularity.
 """
 import argparse
-import hashlib
 import json
 import os
 import subprocess
@@ -23,6 +23,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 WORKLOADS = {
@@ -36,7 +37,10 @@ WORKLOADS = {
                                            '800x800, K=25, 128^2 block textures, 256^2 env textures'),
 }
 SEED = 227391          # configs/dtu/default.yml:42
-PASS_BYTES = 30e9      # views of a step are processed in passes of at most this much workspace (gradients accumulate)
+# views of a step are processed in passes of at most this much workspace (gradients accumulate); the two captured graphs
+# of the pipelined step and the eager warm-up each hold one pass's workspace, which must fit an 80 GB H100 together
+PASS_BYTES = 16e9
+DUMP_BYTES = 64 << 20  # --dump-outputs writes at most this much (a fixed, seeded sample of the larger arrays beyond it)
 
 
 def model_cfg(w):
@@ -59,34 +63,11 @@ def peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
-
-
-def kernel_fingerprint():
-    """sha256 over the sources of the raster kernels (dbw_render.cu and the headers it includes): ties a committed ncu capture
-    (profiles/ncu_traffic.json) to the build that is benched"""
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, 'differentiable-blocksworld_b200', 'csrc')
-    for fn in ('dbw_render.cu', 'dbw_math.cuh', 'dbw_fraglist.cuh', 'dbw_clip.cuh'):
-        h.update(open(os.path.join(d, fn), 'rb').read())
-    return h.hexdigest()[:16]
-
-
-def ncu_traffic(kernel_label, workload, world):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel_label` from the committed `ncu --set full` capture
-    (profiles/ncu_traffic.json, written by scripts/summarize_profile.py) -- only if it was taken on THIS build of the kernels,
-    this workload and one GPU; else None"""
-    path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    if world != 1 or not os.path.exists(path):
-        return None, 'no capture'
-    d = json.load(open(path))
-    if d.get('kernel_fingerprint') != kernel_fingerprint() or d.get('workload') != workload:
-        return None, f'profiles/ncu_traffic.json is from another build ({d.get("kernel_fingerprint")}) or workload: not used'
-    return d['bytes_per_launch'].get(kernel_label), f'{d.get("source", "profiles/ncu_traffic.json")} (same kernel sources: {d["kernel_fingerprint"]})'
+    return 3350.0, 'H100 SXM data sheet (HBM3)'
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line): one background
+    """nvidia-smi clocks / throttle reasons DURING the timed region: one background
     `nvidia-smi -lms 100` process, started before the region and stopped after it."""
     QUERY = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
             'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
@@ -186,7 +167,7 @@ def run_ours(args):
     n_pass, views_per_pass = len(passes), len(passes[0]['imgs'])
     local_px = int(sum(int((p['rows'][:, 1] - p['rows'][:, 0]).sum()) for p in passes)) * W
     dev_passes = [{k: v.to(dev) for k, v in p.items()} for p in passes]
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)       # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)       # > 50 MB L2
     acc = torch.zeros_like(vp.bucket.flat) if n_pass > 1 else None
     if n_pass > 1:
         vp.gather_grads = True          # the passes' gradients are accumulated through the flat bucket
@@ -194,16 +175,19 @@ def run_ours(args):
     # vertices, opacities, decimated texture cells -- one small all-reduce per pass, no leaf all-reduce), else at the leaves
     # (one all-reduce of the parameter-gradient bucket per step)
     inside = vp.reduces_inside_backward(dev_passes[0])
+    last = {}          # the losses of each pass of the latest step (what --dump-outputs writes with the gradients)
 
     def step_eager(collective=True):
+        losses = []
         for i, p in enumerate(dev_passes):
-            vp.forward_backward(p, None, already_sharded=True, n_total_views=B, all_reduce=collective and inside)
+            losses.append(vp.forward_backward(p, None, already_sharded=True, n_total_views=B, all_reduce=collective and inside))
             if acc is not None:
                 acc.copy_(vp.bucket.flat) if i == 0 else acc.add_(vp.bucket.flat)
         if acc is not None:
             vp.bucket.flat.copy_(acc)
         if collective and not inside:
             vp.bucket.all_reduce(vp.group)
+        last['losses'] = losses
 
     graphed = piped = None
     nocoll = None
@@ -219,14 +203,18 @@ def run_ours(args):
         if graphed is None:
             return step_eager(collective)
         g = graphed if collective else nocoll
+        losses = []
         for i, p in enumerate(dev_passes):
-            g.run(p if n_pass > 1 else None, all_reduce=False)          # a collective captured in the graph runs regardless
+            out = g.run(p if n_pass > 1 else None, all_reduce=False)     # a collective captured in the graph runs regardless
+            # the graph's loss tensors are static: the next pass's replay overwrites them, so keep a copy of each pass's
+            losses.append({k: v.clone() if torch.is_tensor(v) else v for k, v in out.items()} if n_pass > 1 else out)
             if acc is not None:
                 acc.copy_(vp.bucket.flat) if i == 0 else acc.add_(vp.bucket.flat)
         if acc is not None:
             vp.bucket.flat.copy_(acc)
         if collective and not g.capture_all_reduce and not inside:
             vp.bucket.all_reduce(vp.group)
+        last['losses'] = losses
 
     def step_e2e():
         """the public API with HOST buffers: every pass's inputs are copied H2D from pinned memory (the next pass's while
@@ -284,6 +272,8 @@ def run_ours(args):
         sampler.start()
     ms_local = timed(step_resident, args.steps)
     clocks = sampler.summary() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step_outputs(model, last['losses']))
     # the same steps without the gradient collective: what the all-reduce adds to a step when it is exposed
     ms_nocoll_local = timed(lambda: step_resident(False), args.steps) if world > 1 else ms_local
 
@@ -330,9 +320,8 @@ def run_ours(args):
             launches of one step cover local_px pixels"""
             ms = kt[key][0] / args.steps                       # all launches of this kernel in one step (one per pass)
             alg = local_px * (16 + 4 * key[1])
-            traffic, src = ncu_traffic(names[key], args.workload, world)
             return {'bound': 'hbm', 'kernel': names[key], 'achieved': alg / (ms / 1e3) / 1e9, 'peak': peak, 'unit': 'GB/s',
-                    'frac': alg / (ms / 1e3) / 1e9 / peak, 'traffic': traffic, 'traffic_source': src, 'peak_source': peak_src,
+                    'frac': alg / (ms / 1e3) / 1e9 / peak, 'traffic': None, 'traffic_source': 'not measured', 'peak_source': peak_src,
                     'algorithmic_bytes_per_step': alg, 'kernel_ms_per_step': ms, 'launches_per_step': kt[key][1] / args.steps}
 
         dom = max(kt, key=lambda k: kt[k][0])                  # the raster kernel with the largest summed duration
@@ -372,6 +361,27 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def step_outputs(model, losses):
+    """what a caller of the timed step receives: each pass's loss terms and the gradient of every leaf parameter"""
+    out = {f'loss_{k}': torch.stack([torch.as_tensor(l[k]).detach().float().reshape(()).cpu() for l in losses])
+           for k in losses[0]}
+    out.update({f'grad_{n}': p.grad.detach().float().cpu() for n, p in model.named_parameters() if p.grad is not None})
+    return out
+
+
+def dump_outputs(directory, arrays):
+    """<directory>/<name>.npy in float32; beyond DUMP_BYTES in all, the larger arrays are replaced by a fixed, seeded sample
+    of their flattened elements (the same sample in every run with the same arguments)"""
+    os.makedirs(directory, exist_ok=True)
+    total = sum(a.numel() * 4 for a in arrays.values())
+    share = DUMP_BYTES // 4 // len(arrays)
+    g = torch.Generator().manual_seed(SEED)
+    for name, a in sorted(arrays.items()):
+        if total > DUMP_BYTES and a.numel() > share:
+            a = a.reshape(-1)[torch.randperm(a.numel(), generator=g)[:share].sort().values]
+        np.save(os.path.join(directory, f'{name}.npy'), a.numpy().astype(np.float32))
+
+
 # ------------------------------------------------------------------------------------------------ CPU legs (oracle port)
 def sample_views(n_views, n):
     """n view indices spread evenly over the ring: the CPU legs render a subset of the very views the GPU arm renders"""
@@ -398,7 +408,7 @@ def oracle_step(workload, views):
 
 def cpu_threads():
     """threads for the CPU legs: all host cores up to 32 (beyond that the small torch ops of the path get slower, not
-    faster; measured on the 128-core GPU box)"""
+    faster)"""
     return min(os.cpu_count(), 32)
 
 
@@ -446,7 +456,8 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=100)
+    ap.add_argument('--steps', type=int, default=None,
+                    help='timed steps (default: 100 for dtu, 10 for the larger workloads, 5 for --impl reference)')
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--workload', default='dtu', choices=sorted(WORKLOADS))
@@ -457,12 +468,18 @@ def main():
                          'step is split over 4 or more GPUs (short launches whose tails then overlap)')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='submit the step eagerly instead of replaying a CUDA graph')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="after the timed steps, write the last one's loss terms and leaf-parameter gradients as DIR/<name>.npy")
     args = ap.parse_args()
-    if args.workload != 'dtu' and args.steps == 100:
-        args.steps = 10              # the larger workloads take 10-100x longer per step: keep the default run within minutes
+    if args.steps is None:
+        # the larger workloads take 10-100x longer per step, a reference step is a bounded CPU sample: keep the default run
+        # within minutes
+        args.steps = 5 if args.impl == 'reference' else 100 if args.workload == 'dtu' else 10
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes what the GPU arm computes')
     if args.impl == 'reference':
-        if args.steps > 5:
-            args.steps = 5          # each step is a bounded CPU sample; keep the whole run within minutes
         run_reference(args)
     else:
         run_ours(args)

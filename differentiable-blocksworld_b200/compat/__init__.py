@@ -1,6 +1,6 @@
 """Import shims that let the reference's UNMODIFIED `src/trainer.py`, `src/optimizer.py`, `src/scheduler.py` and
 `src/utils/*` load on a machine without PyTorch3D / toolz / lpips / seaborn / matplotlib / imageio / trimesh / open3d /
-iopath (SURVEY.md 8b "Caveat", 8f rank 3) -- the B200 image is one.
+iopath (SURVEY.md 8b "Caveat", 8f rank 3).
 
     import dbw_b200.compat as compat
     compat.install()                                   # registers stand-ins ONLY for modules that are not importable

@@ -1,6 +1,6 @@
-// dbw_comm.cu -- the step's ONE gradient exchange (SURVEY.md 8e) as a hand-written all-reduce over NVLink 5 / NVSwitch
+// dbw_comm.cu -- the step's ONE gradient exchange (SURVEY.md 8e) as a hand-written all-reduce over NVLink / NVSwitch
 // peer memory: a plain kernel (no NCCL, no host synchronisation), so that it is captured INSIDE the step's CUDA graph --
-// round 1 had to issue an ncclAllReduce after the graph replay (capturing it hung) and paid ~0.13 ms per step for it.
+// an ncclAllReduce has to be issued after the graph replay instead (capturing it hung).
 //
 // One process per GPU.  Every rank owns an arena (cudaMalloc, exported with cudaIpcGetMemHandle, opened by its peers):
 //     control:  flagsA[world], flagsB[world] (written BY the peers), epoch, grid-barrier counters

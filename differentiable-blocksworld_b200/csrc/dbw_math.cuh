@@ -60,7 +60,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #endif  // __CUDACC__
 
 // reciprocal of the CONTINUOUS normalisations (perspective correction, barycentric clipping): the 1-ulp MUFU
-// approximation -- together with -prec-div=false (Makefile) worth 3.5 % of the step on B200.  Everything a discrete decision
+// approximation, as -prec-div=false (Makefile) makes the plain divisions.  Everything a discrete decision
 // depends on (edge functions, pixel coordinates) uses the explicitly rounded intrinsics (__fmul_rn, __fdiv_rn, ...) and is
 // not affected by either.  -DDBW_PRECISE_RCP restores the correctly rounded reciprocal.
 #ifdef DBW_PRECISE_RCP

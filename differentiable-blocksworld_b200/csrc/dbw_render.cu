@@ -1,4 +1,4 @@
-// dbw_render.cu -- sm_100a kernels + C-ABI of the differentiable primitive renderer (see include/dbw_render.h).
+// dbw_render.cu -- sm_90a kernels + C-ABI of the differentiable primitive renderer (see include/dbw_render.h).
 //
 // Replaces, for the reference's render hot path (src/model/renderer.py:84-98, 219-273):
 //   PerspectiveCameras/MeshRasterizer.transform, clip_faces, _C.rasterize_meshes{,_backward},
@@ -44,6 +44,16 @@ int dbw_fail_(const char* what, cudaError_t e) { return fail(what, e); }
 void dbw_count_launch_(void) { ++g_launches; }
 #define CK(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) return fail(#call, _e); } while (0)
 #define LAUNCH_CK(name) do { ++g_launches; cudaError_t _e = cudaGetLastError(); if (_e != cudaSuccess) return fail(name, _e); } while (0)
+
+// CTAs of 256 threads for a grid-stride kernel over n items: at most `per_sm` per SM of the current device; -1 if the
+// device cannot be queried
+static int stride_grid(long long n, int per_sm) {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return -1;
+  const long long blocks = (n + 255) / 256, cap = (long long)sms * per_sm;
+  return (int)(blocks < cap ? blocks : cap);
+}
 
 static int g_no_hard_kernel = 0;
 // test hook: 1 routes hard single-layer renders through the generic kernel (the two must agree bit for bit)
@@ -399,9 +409,9 @@ struct RasterParams {
   float ep_inv_count; int ep_part_mask;
 };
 
-// Raster CTAs: the 8x4-pixel patches of a CTA's warps tile a 16 x (NT / 16) pixel tile.  Measured on B200 (cfg 2): the
-// backward kernels and the K > 4 forward are fastest with 128 threads (finer scheduling granularity, less waiting on the
-// slowest warp of a tile), the K <= 4 forward with 256 (the bin scan is amortised over more pixels).
+// Raster CTAs: the 8x4-pixel patches of a CTA's warps tile a 16 x (NT / 16) pixel tile.  The backward kernels and the
+// K > 4 forward use 128 threads (finer scheduling granularity, less waiting on the slowest warp of a tile), the K <= 4
+// forward 256 (the bin scan is amortised over more pixels).
 #ifndef DBW_FWD_NT_SMALLK
 #define DBW_FWD_NT_SMALLK 256
 #endif
@@ -478,11 +488,11 @@ __device__ __forceinline__ void shade_geometry(const RasterParams& P, int view, 
 
 // Resident CTAs per SM each raster kernel is compiled for (register cap = 65536 / (threads * CTAs)).
 #ifndef DBW_FWD_SMALLK_MINB
-#define DBW_FWD_SMALLK_MINB 5     // CTAs of DBW_FWD_NT_SMALLK threads (51 registers; 4 was slower on B200)
+#define DBW_FWD_SMALLK_MINB 5     // CTAs of DBW_FWD_NT_SMALLK threads (51 registers)
 #endif
 #ifndef DBW_FWD_MINB
-#define DBW_FWD_MINB 7            // CTAs of DBW_FWD_NT threads: shared memory (25.6 KB of lists at K = 10 + 5 KB tile list) allows 7;
-                                  // measured on B200: 7 CTAs x 72 registers beats 6 x 80 by 7 %
+#define DBW_FWD_MINB 7            // CTAs of DBW_FWD_NT threads: shared memory (25.6 KB of lists at K = 10 + 5 KB tile list) allows 7
+                                  // of the 227 KB an H100 SM gives its CTAs (72 registers)
 #endif
 #ifndef DBW_BWD_DETACH_MINB
 #define DBW_BWD_DETACH_MINB 7     // backward without the barycentric path, CTAs of DBW_BWD_NT threads (72 registers)
@@ -1114,8 +1124,8 @@ __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int
 // helpers run converged.
 #define DBW_ALPHA_SMEM_MAX 512      // opacity entries per view that a CTA may pre-accumulate in shared memory
 // 16 x 8 tiles a backward CTA walks (each warp its own patch of every tile, no barrier between, the next patch's first-level
-// loads in flight).  Measured on B200 (cfg 2): a single-layer pass is a chain of DRAM latencies per pixel and gains from 8
-// (0.449 -> 0.410 ms); the K = 10 blocks pass LOSES (0.95 / 1.03 / 1.11 / 1.18 ms at 1 / 2 / 4 / 8: longer CTAs, worse tails)
+// loads in flight).  A single-layer pass is a chain of DRAM latencies per pixel and gains from 8 tiles; the K = 10 blocks
+// pass walks one (more tiles make longer CTAs and worse tails)
 #define DBW_BWD_TILES_K1 8
 #define DBW_BWD_TILES_KN 1
 
@@ -1593,7 +1603,8 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   LAUNCH_CK("face_setup_kernel");
   if (!s->maps_are_texels4) {
     const int n_texels = s->n_map_floats / 3;
-    int blocks = (n_texels + 255) / 256; if (blocks > 148 * 8) blocks = 148 * 8;
+    const int blocks = stride_grid(n_texels, 8);
+    if (blocks < 0) return fail("maps_to_float4_kernel: SM count", cudaGetLastError());
     maps_to_float4_kernel<<<blocks, 256, 0, st>>>(maps, w.maps4, n_texels);
     LAUNCH_CK("maps_to_float4_kernel");
   }
@@ -1683,7 +1694,8 @@ extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const floa
   LAUNCH_CK("raster_backward_kernel");
   if (g_maps && !s->maps_are_texels4) {
     const int n_texels = s->n_map_floats / 3;
-    int blocks = (n_texels + 255) / 256; if (blocks > 148 * 8) blocks = 148 * 8;
+    const int blocks = stride_grid(n_texels, 8);
+    if (blocks < 0) return fail("fold_gmaps_kernel: SM count", cudaGetLastError());
     fold_gmaps_kernel<<<blocks, 256, 0, st>>>(g.g_maps4, g_maps, n_texels);
     LAUNCH_CK("fold_gmaps_kernel");
   }
@@ -1711,8 +1723,8 @@ extern "C" int dbw_composite_mse(int32_t n_views, int32_t height, int32_t width,
   const int plane = height * width;
   const long long total = (long long)n_views * plane;
   if (total > 0x7fffffffLL) return fail("dbw_composite_mse: too many pixels for one call");
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  const int blocks = stride_grid(total, 16);
+  if (blocks < 0) return fail("composite_mse_kernel: SM count", cudaGetLastError());
   composite_mse_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((int)total, plane, fg, env, imgs, inv_count, rec, loss_sum, g_fg, g_env);
   LAUNCH_CK("composite_mse_kernel");
   return 0;
@@ -1726,8 +1738,8 @@ extern "C" int dbw_composite_mse_backward(int32_t n_views, int32_t height, int32
   const int plane = height * width;
   const long long total = (long long)n_views * plane;
   if (total > 0x7fffffffLL) return fail("dbw_composite_mse_backward: too many pixels for one call");
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  const int blocks = stride_grid(total, 16);
+  if (blocks < 0) return fail("composite_backward_kernel: SM count", cudaGetLastError());
   composite_backward_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((int)total, plane, fg, env, imgs, inv_count, g_loss, g_rec, g_fg, g_env);
   LAUNCH_CK("composite_backward_kernel");
   return 0;

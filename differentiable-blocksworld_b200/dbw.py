@@ -1,5 +1,5 @@
 """Scene model of the render hot path: a drop-in for the reference's `DifferentiableBlocksWorld`
-(/root/reference src/model/dbw.py:38-462) as far as src/trainer.py, src/optimizer.py and configs/*.yml see it --
+(the reference's src/model/dbw.py:38-462) as far as src/trainer.py, src/optimizer.py and configs/*.yml see it --
 same constructor kwargs, same parameter / buffer names (checkpoints, the `texture*` Adam group), same
 `forward(inp, labels) -> {loss name: tensor}` / `predict(...)` / `build_*` / `get_opacities` surface.
 

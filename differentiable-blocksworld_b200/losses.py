@@ -1,4 +1,4 @@
-"""Parameter-only regularisers of the DBW objective (what /root/reference src/model/dbw.py:373-405 adds to the pixel
+"""Parameter-only regularisers of the DBW objective (what the reference's src/model/dbw.py:373-405 adds to the pixel
 terms) as standalone functions: they never touch an image, so they stay plain PyTorch on the leaf parameters -- tiny,
 view-independent, and (in a multi-GPU step) identical on every rank (parallel.py divides them by the world size)."""
 import torch

@@ -3,7 +3,7 @@ that runs, SURVEY.md section 0 item 5 and section 8e).
 
 Views of a step are independent given the replicated scene parameters, so they shard with NO data-path collective:
 rank r renders a contiguous range of the B views (or of their 16-row bands) and back-propagates into its own gradients;
-ONE all-reduce(SUM) per step over NVLink 5 / NVSwitch then gives every rank the full gradient -- either of a single flat
+ONE all-reduce(SUM) per step over NVLink / NVSwitch then gives every rank the full gradient -- either of a single flat
 fp32 bucket of the parameter gradients after the backward (about 9.4 MB for 10 blocks with 256^2 textures), or, while the
 textures are box-decimated, of the scene tensors' gradients inside the backward (GradSumPoint: about 0.16 MB).
 Correctness conditions handled here:

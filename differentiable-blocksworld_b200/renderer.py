@@ -1,7 +1,7 @@
 """Drop-in for the reference's `Renderer` (src/model/renderer.py:24-132): same constructor kwargs, same
 `forward(meshes, R, T, viz_purpose=False, **kwargs) -> (B,4,H,W)`, same `update_cameras(device=, K=)` /
 `.cameras.K` probe (src/model/dbw.py:204-208) -- but the whole MeshRasterizer + LayeredShader + layered_rgb_blend
-stack behind it is ONE pair of hand-written sm_100a kernels reached through the C-ABI of include/dbw_render.h.
+stack behind it is ONE pair of hand-written sm_90a kernels reached through the C-ABI of include/dbw_render.h.
 There is no CPU / PyTorch fallback: a missing library or a non-CUDA tensor raises."""
 import ctypes
 from copy import deepcopy
@@ -61,7 +61,7 @@ class _RenderFn(torch.autograd.Function):
     def forward(ctx, verts, maps, faces_alpha, R, T, faces, faces_uvs, face_map, map_table, cfg, face_shade=None, want_dists=False,
                 want_ids=False):
         if not verts.is_cuda:
-            raise DbwError('the B200 renderer needs CUDA tensors (there is no CPU fallback)')
+            raise DbwError('the CUDA renderer needs CUDA tensors (there is no CPU fallback)')
         s = cfg
         B, H, W, K = s.n_views, s.height, s.width, s.faces_per_pixel
         L = _lib.lib()

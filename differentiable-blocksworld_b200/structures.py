@@ -1,6 +1,6 @@
 """Host-side stand-ins for the PyTorch3D containers the reference passes through its render seam
-(`Meshes`, `TexturesUV`, `join_meshes_as_scene`, `join_meshes_as_batch`; used at /root/reference
-src/model/dbw.py:74-96, 214-220, 260-265, 280, 295, 342-346).  They carry exactly what the B200 kernels consume:
+(`Meshes`, `TexturesUV`, `join_meshes_as_scene`, `join_meshes_as_batch`; used at the reference's
+src/model/dbw.py:74-96, 214-220, 260-265, 280, 295, 342-346).  They carry exactly what the CUDA kernels consume:
 one vertex buffer, one int32 face buffer, per-face-vertex UVs, a per-face map index and the texture maps; nothing is
 replicated per view (`extend(B)` only records B, it does not copy -- the reference's Meshes.extend + TexturesUV
 replication is what forced its batch size down, SURVEY.md section 8 row a9)."""

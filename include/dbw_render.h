@@ -1,5 +1,5 @@
 /*
- * include/dbw_render.h -- C-ABI of the B200-native differentiable primitive renderer.
+ * include/dbw_render.h -- C-ABI of the H100-native (sm_90a) differentiable primitive renderer.
  *
  * The reference (monniert/differentiable-blocksworld) has no FFI: its render hot path is a Python-level seam,
  *     Renderer.forward(meshes, R, T, viz_purpose=False, **kwargs) -> (B,4,H,W)      src/model/renderer.py:84-98

@@ -15,8 +15,8 @@ reference itself owns, composed with the PyTorch3D restatement in oracle/pt3d.py
     _init_blocks / build_* / predict <- src/model/dbw.py:55-119, 202-239, 267-352
     rgb loss                         <- src/model/dbw.py:366-367 (nn.MSELoss via src/model/loss.py:15)
 
-tests/test_oracle_vs_reference.py extracts the reference's own pure-torch functions with `ast` (when
-/root/reference is present) and checks these restatements against them; tests/golden/ holds the vectors.
+tests/golden/make_golden.py extracts the reference's own pure-torch functions with `ast` from a reference checkout and
+stores their outputs under tests/golden/; tests/test_oracle_golden.py checks these restatements against them.
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import this.
 """
 import math

@@ -1,8 +1,8 @@
 """oracle/pt3d.py -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.  **PARITY UNPINNED** (see oracle/README.md).
 
 CPU restatement (torch fp32 / fp64 + the C rasterizer in raster_oracle.c) of the PyTorch3D 0.7.1 pieces the
-reference's render hot path calls.  PyTorch3D (pinned at /root/reference/environment.yml:21) is an un-vendored
-dependency that is absent from /root/reference and from this image; what is restated here is its published
+reference's render hot path calls.  PyTorch3D (pinned at the reference's environment.yml:21) is an un-vendored
+dependency that is absent from the reference's tree; what is restated here is its published
 algorithm as recorded in SURVEY.md Appendix A, anchored on the reference's call sites:
 
     PerspectiveCameras + MeshRasterizer.transform      <- src/model/renderer.py:53,62-67,94   (Appendix A1)

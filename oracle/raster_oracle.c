@@ -2,10 +2,10 @@
  * oracle/raster_oracle.c -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * CPU restatement of the mesh rasterizer the reference's render hot path delegates to:
- * PyTorch3D 0.7.1 (pinned by /root/reference/environment.yml:21), reached from the reference at
+ * PyTorch3D 0.7.1 (pinned by the reference's environment.yml:21), reached from the reference at
  *   src/model/renderer.py:50-54  (RasterizationSettings + MeshRasterizer)
  *   src/model/renderer.py:94     (self.renderer(meshes, R=R, T=T, eps=EPS, **kwargs))
- * PyTorch3D is an un-vendored third-party dependency: its sources are NOT under /root/reference and
+ * PyTorch3D is an un-vendored third-party dependency: its sources are NOT in the reference's tree and
  * it is not installed in this image, so this file restates the *published algorithm* of
  *   pytorch3d/csrc/rasterize_meshes/rasterize_meshes_cpu.cpp  (RasterizeMeshesNaiveCpu, RasterizeMeshesBackwardCpu)
  *   pytorch3d/csrc/utils/geometry_utils.h                     (edge function, barycentrics, perspective

@@ -1,5 +1,5 @@
 """Per-CUDA-source-line stall samples (where warps WAIT) for one kernel of an .ncu-rep, plus the stall-reason totals:
-   python scripts/ncu_stalls.py gpurun_out/prof.ncu-rep <kernel index 1..> [topn]"""
+   python scripts/ncu_stalls.py prof.ncu-rep <kernel index 1..> [topn]"""
 import csv, subprocess, sys, collections
 rep, kid = sys.argv[1], sys.argv[2]
 topn = int(sys.argv[3]) if len(sys.argv) > 3 else 25

@@ -1,18 +1,19 @@
-"""AST-extraction of the reference's own pure-torch functions (only possible where /root/reference exists).
+"""AST-extraction of the reference's own pure-torch functions from a checkout of monniert/differentiable-blocksworld
+named by the DBW_REFERENCE environment variable (tests/golden/make_golden.py uses it to regenerate the vectors).
 
-Nothing is copied into the repo: the function source is read from the reference checkout at test time, compiled
-in a scratch namespace and called, so the comparison is against the reference's code itself."""
+Nothing is copied into the repo: the function source is read from the reference checkout, compiled in a scratch
+namespace and called, so the golden vectors are the output of the reference's code itself."""
 import ast
 import os
 
 import numpy as np
 import torch
 
-REF = '/root/reference'
+REF = os.environ.get('DBW_REFERENCE', '')
 
 
 def have_reference():
-    return os.path.isdir(os.path.join(REF, 'src'))
+    return bool(REF) and os.path.isdir(os.path.join(REF, 'src'))
 
 
 def extract(relpath, names, extra_ns=None):

@@ -11,7 +11,7 @@ import torch.multiprocessing as mp
 
 from oracle import dbw_path as D, pt3d
 
-REF_CFG = '/root/reference/configs'
+REF_CFG = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_configs')   # the reference's configs/
 
 DTU_DEFAULT_MODEL = {          # restated values of configs/dtu/default.yml:1-26
     'name': 'dbw',
@@ -116,7 +116,6 @@ def test_model_constructs_with_reference_parameter_names():
     assert torch.allclose(model.state_dict()['sq_eps'], sd['spq_eps'])
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_CFG), reason='needs the reference checkout (/root/reference)')
 def test_every_reference_config_parses_unmodified():
     import yaml
     from dbw_b200.dbw import create_model

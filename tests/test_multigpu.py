@@ -1,4 +1,4 @@
-"""Multi-GPU (skipped on a 1-GPU box; run with `gpurun --gpus 2`): the hand-written NVLink peer-memory all-reduce
+"""Multi-GPU (skipped with fewer than 2 GPUs): the hand-written NVLink peer-memory all-reduce
 (csrc/dbw_comm.cu) against ncclAllReduce, eagerly and captured inside a CUDA graph, and a row-band-sharded 2-rank step
 against the single-GPU step."""
 import os
