@@ -130,7 +130,8 @@ static Workspace carve(const DbwRenderSettings& s, void* base) {
   w.nfrag = (unsigned char*)(p + off); off += s.save_fragment_state ? align_up(npx) : 0;
   w.total = off; return w;
 }
-struct BwdScratch { float* g_tri; float* g_conv; float* g_verts_ndc; float4* g_maps4; size_t total; };
+struct BwdScratch { float* g_tri; float* g_conv; float* g_verts_ndc; float4* g_maps4; int* bary_flags; size_t total; };
+static size_t bary_flag_count(const DbwRenderSettings& s);
 static BwdScratch carve_bwd(const DbwRenderSettings& s, void* base) {
   BwdScratch w; char* p = (char*)base; size_t off = 0;
   const size_t B = s.n_views, V = s.n_verts, S = 2 * (size_t)s.n_faces;
@@ -138,6 +139,7 @@ static BwdScratch carve_bwd(const DbwRenderSettings& s, void* base) {
   w.g_conv = (float*)(p + off);       off += align_up(B * S * 9 * sizeof(float));
   w.g_verts_ndc = (float*)(p + off);  off += align_up(B * V * 3 * sizeof(float));
   w.g_maps4 = (float4*)(p + off);     off += s.maps_are_texels4 ? 0 : align_up((size_t)(s.n_map_floats / 3) * sizeof(float4));
+  w.bary_flags = (int*)(p + off);     off += align_up(bary_flag_count(s) * sizeof(int));
   w.total = off; return w;
 }
 
@@ -404,6 +406,7 @@ struct RasterParams {
   // backward only
   const float* grad_rgba; float* g_tri; float* g_conv; float* g_faces_alpha; float4* g_maps4;
   const float* grad_scale;   // device scalar multiplied into grad_rgba (the upstream gradient of a fused loss) or NULL
+  int* bary_flags;           // (B, tile columns, strips) of a non-detached single-layer pass: strip needs the barycentric path
   // fused compositing + MSE epilogue of the forward (DbwLossEpilogue); ep_target == NULL: plain render
   const float* ep_env; const float* ep_target; float* ep_g_env; float* ep_rec; float* ep_partials;
   float ep_inv_count; int ep_part_mask;
@@ -499,6 +502,9 @@ __device__ __forceinline__ void shade_geometry(const RasterParams& P, int view, 
 #endif
 #ifndef DBW_BWD_BARY_MINB
 #define DBW_BWD_BARY_MINB 4       // backward with the barycentric path: more live state (128 registers)
+#endif
+#ifndef DBW_BWD_GEOM_MINB
+#define DBW_BWD_GEOM_MINB 5       // barycentric path of a single-layer pass alone (raster_bary_backward_kernel, 92 registers)
 #endif
 
 // CTA -> (view, tile) mapping of the raster kernels.  CTAs are dispatched in linear grid order, so the grid is laid out as
@@ -939,8 +945,11 @@ __device__ __forceinline__ float warp_sum_spread(float (&x)[NP], int lane) {
     if (l < L) {
       const int c = NP >> (l + 1);
       const bool upper = (lane & o) != 0;
+      // constant trip count: the inner loop is unrolled before the outer one, and a bound that depends on l would leave
+      // it a loop with run-time indices into x -- which puts x in local memory
 #pragma unroll
-      for (int j = 0; j < c; ++j) {
+      for (int j = 0; j < NP / 2; ++j) {
+        if (j >= c) break;
         const float send = upper ? x[j] : x[j + c];
         const float keep = upper ? x[j + c] : x[j];
         x[j] = keep + __shfl_xor_sync(0xffffffffu, send, o);
@@ -1017,24 +1026,29 @@ __device__ __forceinline__ void warp_agg_add(float* __restrict__ dst, int stride
   }
 }
 
-// Texture-gradient scatter of one fragment: 4 bilinear taps x RGB.  Under magnification (the environment maps seen
-// through a narrow field of view: hundreds of pixels per texel) whole warps hit the same 2x2 texel footprint, so
-// lanes that share the footprint with >= 8 others are reduced (16-wide spread reduction: total i lands in lane 2i and
-// is added to channel i % 3 of tap i / 3); the rest issue plain vector reds.
-// Coherence is probed from the first pending lane only (no match.any): an incoherent warp pays two ballots.
+// Texture-gradient scatter of one fragment: 4 bilinear taps x RGB, i.e. the colour gradient g times the tap weights w.
+// Only those 7 floats are carried; the 12 products are formed where they are consumed, so the scatter keeps no
+// 12-float array live across the fragment loop (which spilled to local memory).  Under magnification (the environment
+// maps: several pixels per texel) the lanes of a warp fall into a few groups that share a 2x2 texel footprint.
+// Groups of >= DBW_TEX_AGG_MIN lanes (found with one match.any) are reduced (16-wide spread reduction: total i lands in
+// lane 2i and is added to channel i % 3 of tap i / 3); the other lanes issue plain vector reds.  On an H100 SXM, 4 lanes
+// beat 8: 0.495 vs 0.504 ms for the dtu environment backward, 1.19 vs 1.25 ms for the blocks backward (per step).
+#ifndef DBW_TEX_AGG_MIN
+#define DBW_TEX_AGG_MIN 4
+#endif
 __device__ __forceinline__ void warp_tex_scatter(float4* __restrict__ gm, int key, int i01, int i10, int i11,
-                                                 const float (&v)[12], int lane) {
-  unsigned todo = __ballot_sync(0xffffffffu, key >= 0);
-  bool done = key < 0;
+                                                 const float (&g)[3], const float (&w)[4], int lane) {
+  const unsigned grp_mine = __match_any_sync(0xffffffffu, key);
+  const bool big = key >= 0 && __popc(grp_mine) >= DBW_TEX_AGG_MIN;
+  // one bit per group to reduce: its lowest lane
+  unsigned todo = __ballot_sync(0xffffffffu, big && (__ffs(grp_mine) - 1) == lane);
   while (todo) {
     const int leader = __ffs(todo) - 1;
     const int lk = __shfl_sync(0xffffffffu, key, leader);
-    const bool mine = !done && key == lk;
-    const unsigned grp = __ballot_sync(0xffffffffu, mine);
-    if (__popc(grp) < 8) break;
+    const bool mine = big && key == lk;
     float x[16];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) x[i] = (i < 12 && mine) ? v[i] : 0.f;
+    for (int i = 0; i < 16; ++i) x[i] = (i < 12 && mine) ? g[i % 3] * w[i / 3] : 0.f;
     const float r = warp_sum_spread<16>(x, lane);
     // the footprint (i00 = key, i01, i10, i11) is the same for every lane of the group: fetch it from the leader
     const int l01 = __shfl_sync(0xffffffffu, i01, leader), l10 = __shfl_sync(0xffffffffu, i10, leader);
@@ -1042,14 +1056,13 @@ __device__ __forceinline__ void warp_tex_scatter(float4* __restrict__ gm, int ke
     const int idx = lane >> 1, tap = idx / 3, ch = idx - tap * 3;
     const int texel = tap == 0 ? lk : (tap == 1 ? l01 : (tap == 2 ? l10 : l11));
     if ((lane & 1) == 0 && idx < 12 && texel >= 0 && r != 0.f) atomicAdd(reinterpret_cast<float*>(gm + texel) + ch, r);
-    done = done || mine;
-    todo &= ~grp;
+    todo &= todo - 1;
   }
-  if (!done) {
-    red_add_v4(gm + key, v[0], v[1], v[2]);
-    if (i01 >= 0) red_add_v4(gm + i01, v[3], v[4], v[5]);
-    if (i10 >= 0) red_add_v4(gm + i10, v[6], v[7], v[8]);
-    if (i11 >= 0) red_add_v4(gm + i11, v[9], v[10], v[11]);
+  if (key >= 0 && !big) {
+    red_add_v4(gm + key, g[0] * w[0], g[1] * w[0], g[2] * w[0]);
+    if (i01 >= 0) red_add_v4(gm + i01, g[0] * w[1], g[1] * w[1], g[2] * w[1]);
+    if (i10 >= 0) red_add_v4(gm + i10, g[0] * w[2], g[1] * w[2], g[2] * w[2]);
+    if (i11 >= 0) red_add_v4(gm + i11, g[0] * w[3], g[1] * w[3], g[2] * w[3]);
   }
 }
 
@@ -1116,17 +1129,56 @@ __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int
   }
 }
 
+// Barycentric-path gradient of one fragment with colour gradient (gcx, gcy, gcz): colour -> (ix, iy) -> (u, v) ->
+// barycentrics -> vertices (grid_sample backward + A6).  Writes the slot's 9 vertex gradients; returns true when the face
+// is z-clipped and gc9 holds the gradient of its conversion matrix too.
+__device__ __forceinline__ bool bary_frag_backward(const RasterParams& P, size_t gsl, f2 p, const Shade& s, const Texel4& tx,
+                                                   float gcx, float gcy, float gcz, float (&gv9)[9], float (&gc9)[9]) {
+  const float fx0 = (float)tx.tap.x0, fy0 = (float)tx.tap.y0;
+  const float ex = fx0 + 1.f - tx.tap.ix, wx = tx.tap.ix - fx0, ey = fy0 + 1.f - tx.tap.iy, wy = tx.tap.iy - fy0;
+  const float d00 = tx.c00.x * gcx + tx.c00.y * gcy + tx.c00.z * gcz, d01 = tx.c01.x * gcx + tx.c01.y * gcy + tx.c01.z * gcz;
+  const float d10 = tx.c10.x * gcx + tx.c10.y * gcy + tx.c10.z * gcz, d11 = tx.c11.x * gcx + tx.c11.y * gcy + tx.c11.z * gcz;
+  const float gix = (d01 - d00) * ey + (d11 - d10) * wy;
+  const float giy = (d10 - d00) * ex + (d11 - d01) * wx;
+  const float gu = gix * tx.tap.mx, gv = giy * tx.tap.my;
+  f3 gbu = {gu * s.uv01.x + gv * s.uv01.y, gu * s.uv01.z + gv * s.uv01.w, gu * s.u2 + gv * s.v2};
+  f3 gbc = gbu;
+  const bool clipped = s.t.flags & 1;
+  if (clipped) {
+    // z-clipped face (the ground plane under the camera is one): bu = bc @ conv, so the conversion matrix gets
+    // gradient too; it is accumulated per slot with the same warp aggregation as the vertex gradient
+    const float* cv = P.conv + gsl * 9;
+    gbc.x = cv[0] * gbu.x + cv[1] * gbu.y + cv[2] * gbu.z;
+    gbc.y = cv[3] * gbu.x + cv[4] * gbu.y + cv[5] * gbu.z;
+    gbc.z = cv[6] * gbu.x + cv[7] * gbu.y + cv[8] * gbu.z;
+    gc9[0] = s.b.bc.x * gbu.x; gc9[1] = s.b.bc.x * gbu.y; gc9[2] = s.b.bc.x * gbu.z;
+    gc9[3] = s.b.bc.y * gbu.x; gc9[4] = s.b.bc.y * gbu.y; gc9[5] = s.b.bc.y * gbu.z;
+    gc9[6] = s.b.bc.z * gbu.x; gc9[7] = s.b.bc.z * gbu.y; gc9[8] = s.b.bc.z * gbu.z;
+  }
+  float gz0 = 0.f, gz1 = 0.f, gz2 = 0.f;
+  f3 gb_ = gbc;
+  if (P.clipb) gb_ = clip_backward(s.b.bp, gb_);
+  if (P.persp) gb_ = persp_backward(s.b.b0, s.t.z0, s.t.z1, s.t.z2, gb_, gz0, gz1, gz2);
+  f2 g0 = {0.f, 0.f}, g1 = {0.f, 0.f}, g2 = {0.f, 0.f};
+  bary_backward(p, s.t, gb_, g0, g1, g2);
+  gv9[0] = g0.x; gv9[1] = g0.y; gv9[2] = gz0; gv9[3] = g1.x; gv9[4] = g1.y; gv9[5] = gz1; gv9[6] = g2.x; gv9[7] = g2.y; gv9[8] = gz2;
+  return clipped;
+}
+
 // One thread per pixel.  Pass 1 streams the pixel's saved fragment records {slot, u, v, signed distance} front to back,
 // re-fetches the four texels of each (the float4 atlas is L2-resident), scatters the texture gradient and -- unless
 // detach_bary -- re-derives the geometry for the barycentric-path vertex gradient (skipped for faces whose vertices are
-// constants); pass 2 walks back to front with the division-free suffix recurrence of SURVEY Appendix B for d/d(alpha_k)
+// constants; a single-layer pass leaves it to raster_bary_backward_kernel); pass 2 walks back to front with the division-free suffix recurrence of SURVEY Appendix B for d/d(alpha_k)
 // -> opacity and distance -> vertex gradients.  Loops are warp-uniform (trip count = warp max) so that the aggregation
 // helpers run converged.
 #define DBW_ALPHA_SMEM_MAX 512      // opacity entries per view that a CTA may pre-accumulate in shared memory
 // 16 x 8 tiles a backward CTA walks (each warp its own patch of every tile, no barrier between, the next patch's first-level
-// loads in flight).  A single-layer pass is a chain of DRAM latencies per pixel and gains from 8 tiles; the K = 10 blocks
-// pass walks one (more tiles make longer CTAs and worse tails)
+// loads in flight).  A single-layer pass is a chain of DRAM latencies per pixel and gains from 8 tiles (on an H100 SXM,
+// 4 tiles: 0.51 ms instead of 0.50 ms for the dtu environment backward); the K = 10 blocks pass walks one (more tiles
+// make longer CTAs and worse tails)
+#ifndef DBW_BWD_TILES_K1
 #define DBW_BWD_TILES_K1 8
+#endif
 #define DBW_BWD_TILES_KN 1
 
 // K1: faces_per_pixel == 1 (the environment pass): no record prefetch registers, at most one trip through the loops
@@ -1174,6 +1226,7 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
   };
   First first_next;
   load_first(0, first_next);
+  bool need_bary = false;       // K1 && DETACH: this thread saw a fragment that raster_bary_backward_kernel must visit
   for (int t = 0; t < DBW_BWD_TILES; ++t) {
   const First first = first_next;
   load_first(t + 1, first_next);
@@ -1206,7 +1259,7 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
     int key = -1, ckey = -1, tkey = -1, t01 = -1, t10 = -1, t11 = -1;
     float gv9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float gc9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    float tv[12] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float tg[3] = {0.f, 0.f, 0.f}, tw[4] = {0.f, 0.f, 0.f, 0.f};      // texture gradient = tg x tw (colour x tap weights)
     if (have) {
       n = k + 1;
       const int bits = __float_as_int(fr.x), slot = bits & DBW_FRAG_SLOT_MASK;
@@ -1234,48 +1287,18 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
         const float gcx = w * gr, gcy = w * gg, gcz = w * gb;
         if (P.g_maps4) {
           tkey = tx.tap.i00; t01 = tx.tap.i01; t10 = tx.tap.i10; t11 = tx.tap.i11;
-          tv[0] = gcx * tx.tap.w00; tv[1] = gcy * tx.tap.w00; tv[2] = gcz * tx.tap.w00;
-          tv[3] = gcx * tx.tap.w01; tv[4] = gcy * tx.tap.w01; tv[5] = gcz * tx.tap.w01;
-          tv[6] = gcx * tx.tap.w10; tv[7] = gcy * tx.tap.w10; tv[8] = gcz * tx.tap.w10;
-          tv[9] = gcx * tx.tap.w11; tv[10] = gcy * tx.tap.w11; tv[11] = gcz * tx.tap.w11;
+          tg[0] = gcx; tg[1] = gcy; tg[2] = gcz;
+          tw[0] = tx.tap.w00; tw[1] = tx.tap.w01; tw[2] = tx.tap.w10; tw[3] = tx.tap.w11;
         }
         if (bary_path && P.g_tri) {
-          // colour -> (ix, iy) -> (u, v) -> barycentrics -> vertices  (grid_sample backward + A6)
-          const float fx0 = (float)tx.tap.x0, fy0 = (float)tx.tap.y0;
-          const float ex = fx0 + 1.f - tx.tap.ix, wx = tx.tap.ix - fx0, ey = fy0 + 1.f - tx.tap.iy, wy = tx.tap.iy - fy0;
-          const float d00 = tx.c00.x * gcx + tx.c00.y * gcy + tx.c00.z * gcz, d01 = tx.c01.x * gcx + tx.c01.y * gcy + tx.c01.z * gcz;
-          const float d10 = tx.c10.x * gcx + tx.c10.y * gcy + tx.c10.z * gcz, d11 = tx.c11.x * gcx + tx.c11.y * gcy + tx.c11.z * gcz;
-          const float gix = (d01 - d00) * ey + (d11 - d10) * wy;
-          const float giy = (d10 - d00) * ex + (d11 - d01) * wx;
-          const float gu = gix * tx.tap.mx, gv = giy * tx.tap.my;
-          f3 gbu = {gu * s.uv01.x + gv * s.uv01.y, gu * s.uv01.z + gv * s.uv01.w, gu * s.u2 + gv * s.v2};
-          const size_t gsl = slot_base + slot;
-          f3 gbc = gbu;
-          if (s.t.flags & 1) {
-            // z-clipped face (the ground plane under the camera is one): bu = bc @ conv, so the conversion matrix gets
-            // gradient too; it is accumulated per slot with the same warp aggregation as the vertex gradient below
-            const float* cv = P.conv + gsl * 9;
-            gbc.x = cv[0] * gbu.x + cv[1] * gbu.y + cv[2] * gbu.z;
-            gbc.y = cv[3] * gbu.x + cv[4] * gbu.y + cv[5] * gbu.z;
-            gbc.z = cv[6] * gbu.x + cv[7] * gbu.y + cv[8] * gbu.z;
-            ckey = slot;
-            gc9[0] = s.b.bc.x * gbu.x; gc9[1] = s.b.bc.x * gbu.y; gc9[2] = s.b.bc.x * gbu.z;
-            gc9[3] = s.b.bc.y * gbu.x; gc9[4] = s.b.bc.y * gbu.y; gc9[5] = s.b.bc.y * gbu.z;
-            gc9[6] = s.b.bc.z * gbu.x; gc9[7] = s.b.bc.z * gbu.y; gc9[8] = s.b.bc.z * gbu.z;
-          }
-          float gz0 = 0.f, gz1 = 0.f, gz2 = 0.f;
-          f3 gb_ = gbc;
-          if (P.clipb) gb_ = clip_backward(s.b.bp, gb_);
-          if (P.persp) gb_ = persp_backward(s.b.b0, s.t.z0, s.t.z1, s.t.z2, gb_, gz0, gz1, gz2);
-          f2 g0 = {0.f, 0.f}, g1 = {0.f, 0.f}, g2 = {0.f, 0.f};
-          bary_backward(p, s.t, gb_, g0, g1, g2);
           key = slot;
-          gv9[0] = g0.x; gv9[1] = g0.y; gv9[2] = gz0; gv9[3] = g1.x; gv9[4] = g1.y; gv9[5] = gz1; gv9[6] = g2.x; gv9[7] = g2.y; gv9[8] = gz2;
+          if (bary_frag_backward(P, slot_base + slot, p, s, tx, gcx, gcy, gcz, gv9, gc9)) ckey = slot;
         }
       }
+      if (K1 && DETACH && face >= P.n_static_faces && w != 0.f) need_bary = true;
       occ *= (1.f - a);
     }
-    if (P.g_maps4) warp_tex_scatter(P.g_maps4, tkey, t01, t10, t11, tv, lane);
+    if (P.g_maps4) warp_tex_scatter(P.g_maps4, tkey, t01, t10, t11, tg, tw, lane);
     if (!DETACH) {
       if (__ballot_sync(0xffffffffu, key >= 0)) warp_agg_add<9>(P.g_tri + slot_base * 9, 9, key, gv9, lane);
       if (__ballot_sync(0xffffffffu, ckey >= 0)) warp_agg_add<9>(P.g_conv + slot_base * 9, 9, ckey, gc9, lane);
@@ -1343,6 +1366,64 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
       const float v = s_galpha[i];
       if (v != 0.f) atomicAdd(&P.g_faces_alpha[(size_t)view * P.alpha_stride + i], v);
     }
+  }
+  if (K1 && DETACH && P.bary_flags) {
+    if (__syncthreads_or(need_bary) && tid == 0) P.bary_flags[((size_t)view * gridDim.y + blockIdx.y) * gridDim.z + strip] = 1;
+  }
+}
+
+// Barycentric-path vertex gradient of a single-layer pass that is not detached (the environment pass: the ground's pose
+// gets gradient only through its barycentrics).  It runs after raster_backward_kernel<true, *, true>, which scatters the
+// texture gradients and the opacity / distance gradients of every pixel and flags the strips holding a fragment of a face
+// >= n_static_faces; this kernel has the same grid and leaves the unflagged strips at once.  Per pixel it re-derives the
+// fragment's geometry and its four texels for d(colour)/d(uv), and aggregates the slot gradients -- no texture scatter,
+// so the geometry has the register file to itself.
+template <bool ALPHA>
+__global__ void __launch_bounds__(DBW_BWD_NT, DBW_BWD_GEOM_MINB) raster_bary_backward_kernel(const RasterParams P) {
+  extern __shared__ int4 s_desc[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int view = blockIdx.x;
+  const int strip = centre_out(blockIdx.z, gridDim.z);
+  const int xi = blockIdx.y * TILE_W + (warp & 1) * 8 + (lane & 7);
+  int row_lo = 0, row_hi = P.H;
+  if (P.view_rows) { row_lo = P.view_rows[view * 2]; row_hi = P.view_rows[view * 2 + 1]; }
+  constexpr int TH = DBW_BWD_NT / 16;
+  if (strip * DBW_BWD_TILES_K1 * TH >= row_hi || (strip + 1) * DBW_BWD_TILES_K1 * TH <= row_lo) return;
+  if (!P.bary_flags[((size_t)view * gridDim.y + blockIdx.y) * gridDim.z + strip]) return;
+  stage_map_table(P, s_desc, tid, DBW_BWD_NT);
+  const size_t plane = (size_t)P.H * P.W;
+  const float gs = P.grad_scale ? __ldg(P.grad_scale) : 1.f;
+  const size_t slot_base = (size_t)view * 2 * P.F;
+  __syncthreads();
+  for (int t = 0; t < DBW_BWD_TILES_K1; ++t) {
+    const int yi = (strip * DBW_BWD_TILES_K1 + t) * TH + (warp >> 1) * 4 + (lane >> 3);
+    const bool live = xi < P.W && yi < P.H && yi >= row_lo && yi < row_hi;
+    const size_t pix = live ? (size_t)yi * P.W + xi : 0;
+    int key = -1, ckey = -1;
+    float gv9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float gc9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (live && P.nfrag[(size_t)view * plane + pix]) {
+      const float4 fr = P.frag[(size_t)view * plane + pix];
+      const int bits = __float_as_int(fr.x), slot = bits & DBW_FRAG_SLOT_MASK;
+      const int face = slot >= P.F ? slot - P.F : slot;
+      if (face >= P.n_static_faces) {
+        const float* go = P.grad_rgba + (size_t)view * 4 * plane + pix;
+        const float gr = go[0] * gs, gg = go[plane] * gs, gb = go[2 * plane] * gs;
+        const float fa = ALPHA ? __ldg(&P.faces_alpha[alpha_index(P, view, face)]) : 1.f;
+        const float w = frag_alpha(fr.w, P.sigma, P.clip_inside) * fa;        // the only layer: occlusion 1
+        if (w != 0.f && (gr != 0.f || gg != 0.f || gb != 0.f)) {
+          const f2 p = {pix_to_ndc(P.W - 1 - xi, P.W, P.H), pix_to_ndc(P.H - 1 - yi, P.H, P.W)};
+          Shade s;
+          Texel4 tx;
+          shade_geometry(P, view, slot, p, s);
+          fetch_color(P, s.u, s.v, s_desc[(unsigned)bits >> DBW_FRAG_MAP_SHIFT], tx);
+          key = slot;
+          if (bary_frag_backward(P, slot_base + slot, p, s, tx, w * gr, w * gg, w * gb, gv9, gc9)) ckey = slot;
+        }
+      }
+    }
+    if (__ballot_sync(0xffffffffu, key >= 0)) warp_agg_add<9>(P.g_tri + slot_base * 9, 9, key, gv9, lane);
+    if (__ballot_sync(0xffffffffu, ckey >= 0)) warp_agg_add<9>(P.g_conv + slot_base * 9, 9, ckey, gc9, lane);
   }
 }
 
@@ -1520,6 +1601,18 @@ static RasterParams make_params(const DbwRenderSettings& s, const Workspace& w, 
   return P;
 }
 
+// backward grid: (view, 16-px tile column, strip of DBW_BWD_TILES_K1 / _KN tiles)
+static dim3 bwd_grid(const DbwRenderSettings& s) {
+  const int strip_rows = (s.faces_per_pixel == 1 ? DBW_BWD_TILES_K1 : DBW_BWD_TILES_KN) * (DBW_BWD_NT / 16);
+  return dim3(s.n_views, (s.width + TILE_W - 1) / TILE_W, (s.height + strip_rows - 1) / strip_rows);
+}
+// one flag per backward CTA of a single-layer pass that is not detached (see raster_bary_backward_kernel)
+static size_t bary_flag_count(const DbwRenderSettings& s) {
+  if (s.faces_per_pixel != 1 || s.detach_bary) return 0;
+  const dim3 g = bwd_grid(s);
+  return (size_t)g.x * g.y * g.z;
+}
+
 // dynamic shared memory of the raster kernels: K list entries (forward) / K saved scalars (backward) of 20 B per thread
 static size_t frag_smem_bytes(int K, int NT, int M, int n_alpha = 0) {
   return (size_t)K * NT * (sizeof(float4) + sizeof(float)) + (size_t)M * sizeof(int4) + (n_alpha <= 512 ? (size_t)n_alpha * sizeof(float) : 0);
@@ -1674,24 +1767,37 @@ extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const floa
   P.map_table = map_table;
   P.grad_rgba = grad_rgba; P.grad_scale = grad_scale; P.g_tri = need_geom ? g.g_tri : nullptr; P.g_conv = g.g_conv;
   P.g_faces_alpha = g_faces_alpha; P.g_maps4 = g_maps ? (s->maps_are_texels4 ? (float4*)g_maps : g.g_maps4) : nullptr;
-  const int strip_rows = (s->faces_per_pixel == 1 ? DBW_BWD_TILES_K1 : DBW_BWD_TILES_KN) * (DBW_BWD_NT / 16);
-  dim3 grid(B, (s->width + TILE_W - 1) / TILE_W, (s->height + strip_rows - 1) / strip_rows);       // see centre_out()
+  const dim3 grid = bwd_grid(*s);        // see centre_out()
   const size_t smem = frag_smem_bytes(s->faces_per_pixel, DBW_BWD_NT, s->n_maps, P.n_alpha);
   {
+    ScopedTimer timer(1, s->faces_per_pixel, st);       // both launches of a split single-layer pass
     auto launch = [&](auto kern) -> cudaError_t {
       if (smem > 40 * 1024) { cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); if (e != cudaSuccess) return e; }
-      ScopedTimer timer(1, s->faces_per_pixel, st);
       kern<<<grid, DBW_BWD_NT, smem, st>>>(P);
       return cudaSuccess;
     };
     const bool det = s->detach_bary != 0, al = faces_alpha != nullptr, k1 = s->faces_per_pixel == 1;
-    cudaError_t e = k1  ? (det ? (al ? launch(raster_backward_kernel<true, true, true>) : launch(raster_backward_kernel<true, false, true>))
-                               : (al ? launch(raster_backward_kernel<false, true, true>) : launch(raster_backward_kernel<false, false, true>)))
+    // A single-layer pass that is not detached runs as the detached kernel (texture, opacity and distance gradients of
+    // every pixel) plus raster_bary_backward_kernel over the strips that hold faces with vertex gradients
+    const bool split = k1 && !det && need_geom;
+    if (split) P.bary_flags = g.bary_flags;
+    cudaError_t e = k1  ? (al ? launch(raster_backward_kernel<true, true, true>) : launch(raster_backward_kernel<true, false, true>))
                   : det ? (al ? launch(raster_backward_kernel<true, true, false>) : launch(raster_backward_kernel<true, false, false>))
                         : (al ? launch(raster_backward_kernel<false, true, false>) : launch(raster_backward_kernel<false, false, false>));
     if (e != cudaSuccess) return fail("raster_backward_kernel attribute", e);
+    LAUNCH_CK("raster_backward_kernel");
+    if (split) {
+      const size_t gsmem = (size_t)s->n_maps * sizeof(int4);
+      auto launch_bary = [&](auto kern) -> cudaError_t {
+        if (gsmem > 40 * 1024) { cudaError_t e2 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem); if (e2 != cudaSuccess) return e2; }
+        kern<<<grid, DBW_BWD_NT, gsmem, st>>>(P);
+        return cudaSuccess;
+      };
+      e = al ? launch_bary(raster_bary_backward_kernel<true>) : launch_bary(raster_bary_backward_kernel<false>);
+      if (e != cudaSuccess) return fail("raster_bary_backward_kernel attribute", e);
+      LAUNCH_CK("raster_bary_backward_kernel");
+    }
   }
-  LAUNCH_CK("raster_backward_kernel");
   if (g_maps && !s->maps_are_texels4) {
     const int n_texels = s->n_map_floats / 3;
     const int blocks = stride_grid(n_texels, 8);
