@@ -283,6 +283,29 @@ __device__ __forceinline__ TexTap tex_tap(float u, float v, int off, int H, int 
   return t;
 }
 
+// Cell maps (DbwMapDesc.reserved = DBW_MAP_CELLS(f, p_left), include/dbw_render.h): a box-decimated map stored as its
+// (TS/f) x (TS/f) cells instead of the TS x (p_left + TS + p_right) atlas that repeats each cell over f x f texels (and over
+// the circular padding).  tex_tap runs on the logical atlas as before; the taps' texel indices are then replaced by cell
+// indices (`off`: first cell of the map): atlas row H-1-y holds source row H-1-y, i.e. cell row (H-1-y)/f; atlas column x
+// holds source column (x - p_left) mod TS, i.e. cell column ((x - p_left) mod TS)/f -- the padded columns wrap exactly as
+// DBW_TEX_STAGE_EXPAND writes them.  Absent (border) taps stay -1.  TS = H: the textures are square.  f is a power of two
+// (2 .. 128), so the divisions are shifts.
+__device__ __forceinline__ void tap_to_cells(TexTap& t, int off, int H, int cells) {
+  const int f = cells & 0xff, p_left = cells >> 8, TS = H;
+  const int sh = ((f & 0xaa) != 0) | (((f & 0xcc) != 0) << 1) | (((f & 0xf0) != 0) << 2);      // log2(f)
+  const int CS = TS >> sh;
+  int sx0 = t.x0 - p_left;
+  sx0 = sx0 < 0 ? sx0 + TS : (sx0 >= TS ? sx0 - TS : sx0);
+  const int sx1 = sx0 + 1 >= TS ? 0 : sx0 + 1;
+  const int r0 = H - 1 - t.y0;                      // r0 - 1 is used only when the row below exists (r0 >= 1)
+  const int row0 = off + (r0 >> sh) * CS, row1 = off + ((r0 - 1) >> sh) * CS;
+  const int c0 = sx0 >> sh, c1 = sx1 >> sh;
+  t.i00 = row0 + c0;
+  t.i01 = t.i01 >= 0 ? row0 + c1 : -1;
+  t.i10 = t.i10 >= 0 ? row1 + c0 : -1;
+  t.i11 = t.i11 >= 0 ? row1 + c1 : -1;
+}
+
 __device__ __forceinline__ f3 ld_texel(const float4* __restrict__ m, int i) {
   if (i < 0) return {0.f, 0.f, 0.f};
   const float4 t = __ldg(m + i);          // one 128-bit load per tap (RGB + pad)

@@ -130,7 +130,7 @@ static Workspace carve(const DbwRenderSettings& s, void* base) {
   w.nfrag = (unsigned char*)(p + off); off += s.save_fragment_state ? align_up(npx) : 0;
   w.total = off; return w;
 }
-struct BwdScratch { float* g_tri; float* g_conv; float* g_verts_ndc; float4* g_maps4; int* bary_flags; size_t total; };
+struct BwdScratch { float* g_tri; float* g_conv; float* g_verts_ndc; float4* g_maps4; float4* g_cells; int* bary_flags; size_t total; };
 static size_t bary_flag_count(const DbwRenderSettings& s);
 static BwdScratch carve_bwd(const DbwRenderSettings& s, void* base) {
   BwdScratch w; char* p = (char*)base; size_t off = 0;
@@ -139,6 +139,8 @@ static BwdScratch carve_bwd(const DbwRenderSettings& s, void* base) {
   w.g_conv = (float*)(p + off);       off += align_up(B * S * 9 * sizeof(float));
   w.g_verts_ndc = (float*)(p + off);  off += align_up(B * V * 3 * sizeof(float));
   w.g_maps4 = (float4*)(p + off);     off += s.maps_are_texels4 ? 0 : align_up((size_t)(s.n_map_floats / 3) * sizeof(float4));
+  // cell-map gradients: DBW_CELL_GRAD_COPIES copies of the whole map array (a CTA adds into one of them)
+  w.g_cells = (float4*)(p + off);     off += s.maps_are_texels4 == 2 ? align_up((size_t)DBW_CELL_GRAD_COPIES * (s.n_map_floats / 3) * sizeof(float4)) : 0;
   w.bary_flags = (int*)(p + off);     off += align_up(bary_flag_count(s) * sizeof(int));
   w.total = off; return w;
 }
@@ -163,6 +165,7 @@ static int validate(const DbwRenderSettings* s) {
   if (s->n_maps > DBW_FRAG_MAX_MAPS) return fail("too many texture maps: a fragment's map is stored in 9 bits");
   if (s->sigma < 0.f || s->blur_radius < 0.f) return fail("sigma and blur_radius must be >= 0");
   if (s->n_map_floats <= 0 || s->n_map_floats % 3 != 0) return fail("n_map_floats must be a positive multiple of 3");
+  if (s->maps_are_texels4 < 0 || s->maps_are_texels4 > 2) return fail("maps_are_texels4 must be 0, 1 or 2");
   return 0;
 }
 
@@ -170,6 +173,18 @@ static int validate(const DbwRenderSettings* s) {
 __global__ void maps_to_float4_kernel(const float* __restrict__ maps, float4* __restrict__ maps4, int n_texels) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_texels; i += gridDim.x * blockDim.x)
     maps4[i] = make_float4(maps[3 * i], maps[3 * i + 1], maps[3 * i + 2], 0.f);
+}
+// g_maps += the sum of the DBW_CELL_GRAD_COPIES cell-gradient copies (maps_are_texels4 = 2)
+__global__ void fold_gcells_kernel(const float4* __restrict__ gc, float4* __restrict__ g_maps, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float4 a = g_maps[i];
+#pragma unroll
+    for (int r = 0; r < DBW_CELL_GRAD_COPIES; ++r) {
+      const float4 c = gc[(size_t)r * n + i];
+      a.x += c.x; a.y += c.y; a.z += c.z;
+    }
+    g_maps[i] = a;
+  }
 }
 __global__ void fold_gmaps_kernel(const float4* __restrict__ g4, float* __restrict__ g_maps, int n_texels) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_texels; i += gridDim.x * blockDim.x) {
@@ -405,6 +420,7 @@ struct RasterParams {
   float* out_dists;          // (B,K,H,W) signed squared distances of the kept fragments (-1 = empty) or NULL
   // backward only
   const float* grad_rgba; float* g_tri; float* g_conv; float* g_faces_alpha; float4* g_maps4;
+  float4* g_cells; int n_cells;   // cell-map gradient copies (DBW_CELL_GRAD_COPIES x n_cells) or NULL: cell taps go to g_maps4
   const float* grad_scale;   // device scalar multiplied into grad_rgba (the upstream gradient of a fused loss) or NULL
   int* bary_flags;           // (B, tile columns, strips) of a non-detached single-layer pass: strip needs the barycentric path
   // fused compositing + MSE epilogue of the forward (DbwLossEpilogue); ep_target == NULL: plain render
@@ -444,19 +460,31 @@ __device__ __forceinline__ int alpha_index(const RasterParams& P, int view, int 
 
 // bilinear colour of a fragment from its UV (shared by forward shading and the detach_bary backward)
 struct Texel4 { TexTap tap; f3 c00, c01, c10, c11, color; };
-// the map table in shared memory: (first texel, H, W, -) per map, staged once per CTA -- a fragment's tap addresses then
+// the map table in shared memory: (first texel, H, W, DBW_MAP_CELLS or 0) per map, staged once per CTA -- a fragment's tap addresses then
 // depend on no global load
 __device__ __forceinline__ void stage_map_table(const RasterParams& P, int4* s_desc, int tid, int nthreads) {
   for (int m = tid; m < P.M; m += nthreads) {
     const DbwMapDesc d = P.map_table[m];
-    s_desc[m] = make_int4(d.offset / 3, d.height, d.width, 0);
+    s_desc[m] = make_int4(d.offset / 3, d.height, d.width, d.reserved);
   }
 }
-__device__ __forceinline__ void tap_only(float u, float v, int4 d, Texel4& s) { s.tap = tex_tap(u, v, d.x, d.y, d.z); }
+// taps of (u, v) in map d: texel indices, or cell indices for a cell map (d.w != 0)
+__device__ __forceinline__ TexTap map_tap(float u, float v, int4 d) {
+  TexTap t = tex_tap(u, v, d.x, d.y, d.z);
+  if (d.w) tap_to_cells(t, d.x, d.y, d.w);
+  return t;
+}
+__device__ __forceinline__ void tap_only(float u, float v, int4 d, Texel4& s) { s.tap = map_tap(u, v, d); }
 __device__ __forceinline__ void fetch_color(const RasterParams& P, float u, float v, int4 d, Texel4& s) {
-  s.tap = tex_tap(u, v, d.x, d.y, d.z);
-  s.c00 = ld_texel(P.maps4, s.tap.i00); s.c01 = ld_texel(P.maps4, s.tap.i01);
-  s.c10 = ld_texel(P.maps4, s.tap.i10); s.c11 = ld_texel(P.maps4, s.tap.i11);
+  s.tap = map_tap(u, v, d);
+  s.c00 = ld_texel(P.maps4, s.tap.i00);
+  if (d.w) {          // cell map: the four taps usually share one cell (49 of 64 footprints at f = 8); each distinct cell is loaded once
+    s.c01 = s.tap.i01 == s.tap.i00 ? s.c00 : ld_texel(P.maps4, s.tap.i01);
+    s.c10 = s.tap.i10 == s.tap.i00 ? s.c00 : ld_texel(P.maps4, s.tap.i10);
+    s.c11 = s.tap.i11 == s.tap.i01 ? s.c01 : (s.tap.i11 == s.tap.i10 ? s.c10 : ld_texel(P.maps4, s.tap.i11));
+  } else {
+    s.c01 = ld_texel(P.maps4, s.tap.i01); s.c10 = ld_texel(P.maps4, s.tap.i10); s.c11 = ld_texel(P.maps4, s.tap.i11);
+  }
   s.color.x = s.c00.x * s.tap.w00 + s.c01.x * s.tap.w01 + s.c10.x * s.tap.w10 + s.c11.x * s.tap.w11;
   s.color.y = s.c00.y * s.tap.w00 + s.c01.y * s.tap.w01 + s.c10.y * s.tap.w10 + s.c11.y * s.tap.w11;
   s.color.z = s.c00.z * s.tap.w00 + s.c01.z * s.tap.w01 + s.c10.z * s.tap.w10 + s.c11.z * s.tap.w11;
@@ -671,8 +699,8 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
       if (hit && pos < CAP) { s_slot[pos] = sl; s_bbox[pos] = bb[q]; }
     }
   }
-  if (tid < P.M) s_desc[tid] = make_int4(my_desc.offset / 3, my_desc.height, my_desc.width, 0);
-  for (int m = tid + NT; m < P.M; m += NT) { const DbwMapDesc d = P.map_table[m]; s_desc[m] = make_int4(d.offset / 3, d.height, d.width, 0); }
+  if (tid < P.M) s_desc[tid] = make_int4(my_desc.offset / 3, my_desc.height, my_desc.width, my_desc.reserved);
+  for (int m = tid + NT; m < P.M; m += NT) { const DbwMapDesc d = P.map_table[m]; s_desc[m] = make_int4(d.offset / 3, d.height, d.width, d.reserved); }
   __syncthreads();
   const int total = s_count;
   if (total <= CAP) {
@@ -825,7 +853,7 @@ __global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const R
   const int nvis = __ldg(P.view_nvis + view);
   const size_t slot_base = (size_t)view * 2 * P.F;
   const int* vis = P.vis_list + slot_base;
-  for (int m = tid; m < P.M; m += HARD_NT) { const DbwMapDesc d = P.map_table[m]; s_desc[m] = make_int4(d.offset / 3, d.height, d.width, 0); }
+  for (int m = tid; m < P.M; m += HARD_NT) { const DbwMapDesc d = P.map_table[m]; s_desc[m] = make_int4(d.offset / 3, d.height, d.width, d.reserved); }
   __syncthreads();
   const f2 p = {s_ndc[xi - tx0], s_ndc[16 + yi - ty0]};
   const int tx1 = min(tx0 + 16, P.W) - 1, ty1 = min(ty0 + 16, P.H) - 1;
@@ -1036,8 +1064,74 @@ __device__ __forceinline__ void warp_agg_add(float* __restrict__ dst, int stride
 #ifndef DBW_TEX_AGG_MIN
 #define DBW_TEX_AGG_MIN 4
 #endif
-__device__ __forceinline__ void warp_tex_scatter(float4* __restrict__ gm, int key, int i01, int i10, int i11,
-                                                 const float (&g)[3], const float (&w)[4], int lane) {
+// Cell maps (DbwMapDesc.reserved != 0): a lane first merges its taps that share a cell (one cell carries all four weights
+// for 49 of 64 footprints at f = 8) and issues one red.v4 per distinct cell instead of four, one tap slot per round, into
+// one of DBW_CELL_GRAD_COPIES copies of the cell gradients (cell_grad_copy): a cell collects what 64 texels did, and with a
+// single copy the reds of all the warps that cover it serialise at the L2.
+//  - MATCH (single-layer passes: the environment maps, magnified, a warp often inside one cell): the lanes of every group of
+//    >= DBW_CELL_AGG_MIN lanes found by match.any are warp-reduced first and their leader issues one red.v4.
+//  - otherwise (the blocks pass): no warp reduction.  On an H100 at 400 W (dtu, blocks backward): 1.12 ms, against 1.27 ms
+//    with the groups found in lane order and reduced, and 1.25 ms for the texel-space scatter of atlas maps.
+#ifndef DBW_CELL_AGG_MIN
+#define DBW_CELL_AGG_MIN 4
+#endif
+template <bool MATCH>
+__device__ __forceinline__ void warp_cell_scatter(float4* __restrict__ gm, int k00, int k01, int k10, int k11,
+                                                  const float (&g)[3], const float (&w)[4], int lane) {
+  // merge this lane's taps that share a cell (kept in the first of them; k = -1: no tap)
+  float m00 = w[0], m01 = w[1], m10 = w[2], m11 = w[3];
+  if (k01 >= 0 && k01 == k00) { m00 += m01; k01 = -1; }
+  if (k10 >= 0 && k10 == k00) { m00 += m10; k10 = -1; }
+  if (k11 >= 0 && k11 == k00) { m00 += m11; k11 = -1; }
+  else if (k11 >= 0 && k11 == k01) { m01 += m11; k11 = -1; }
+  else if (k11 >= 0 && k11 == k10) { m10 += m11; k11 = -1; }
+  // one tap slot per round, the slots rotated through registers (a rolled loop: the scatter stays small)
+#pragma unroll 1
+  while (__any_sync(0xffffffffu, (k00 & k01 & k10 & k11) != -1)) {
+    const int key = k00;
+    const float v0 = g[0] * m00, v1 = g[1] * m00, v2 = g[2] * m00;
+    // groups to reduce: one bit per group, its leader; `big`: this lane's value goes into a group sum
+    unsigned todo = 0;
+    bool big = false;
+    if (MATCH) {
+      const unsigned grp = __match_any_sync(0xffffffffu, key);
+      big = key >= 0 && __popc(grp) >= DBW_CELL_AGG_MIN;
+      todo = __ballot_sync(0xffffffffu, big && (__ffs(grp) - 1) == lane);
+    }
+    while (todo) {
+      const int leader = __ffs(todo) - 1;
+      const int lk = __shfl_sync(0xffffffffu, key, leader);
+      const bool mine = big && key == lk;
+      float x[4] = {mine ? v0 : 0.f, mine ? v1 : 0.f, mine ? v2 : 0.f, 0.f};
+      const float r = warp_sum_spread<4>(x, lane);          // total c in lanes 8c .. 8c + 7
+      const float r0 = __shfl_sync(0xffffffffu, r, 0), r1 = __shfl_sync(0xffffffffu, r, 8), r2 = __shfl_sync(0xffffffffu, r, 16);
+      if (lane == leader) red_add_v4(gm + lk, r0, r1, r2);
+      todo &= todo - 1;
+    }
+    if (key >= 0 && !big) red_add_v4(gm + key, v0, v1, v2);
+    k00 = k01; k01 = k10; k10 = k11; k11 = -1;
+    m00 = m01; m01 = m10; m10 = m11;
+  }
+}
+
+// cells: this lane's map is a cell map (the taps are cell indices).  A warp with any such lane takes the cell path for all
+// its lanes: it is correct for texel taps too (a lane's four texels are distinct, so nothing merges), and only one of the two
+// paths is live at a time.
+// the copy of the cell-map gradients a warp adds into (re-derived where it is used: no register held across the loops).
+// Neighbouring CTAs and the warps of a CTA cover neighbouring pixels, i.e. mostly the same cells, and spread over the copies.
+__device__ __forceinline__ float4* cell_grad_copy(const RasterParams& P, int warp) {
+  if (!P.g_cells) return P.g_maps4;
+  const unsigned c = (blockIdx.y + 3 * blockIdx.z + 5 * blockIdx.x + 2 * warp) & (DBW_CELL_GRAD_COPIES - 1);
+  return P.g_cells + (size_t)c * P.n_cells;
+}
+template <bool K1>
+__device__ __forceinline__ void warp_tex_scatter(const RasterParams& P, int key, int i01, int i10, int i11, bool cells,
+                                                 const float (&g)[3], const float (&w)[4], int lane, int warp) {
+  float4* const gm = P.g_maps4;
+  if (__any_sync(0xffffffffu, key >= 0 && cells)) {
+    warp_cell_scatter<K1>(cell_grad_copy(P, warp), key, i01, i10, i11, g, w, lane);
+    return;
+  }
   const unsigned grp_mine = __match_any_sync(0xffffffffu, key);
   const bool big = key >= 0 && __popc(grp_mine) >= DBW_TEX_AGG_MIN;
   // one bit per group to reduce: its lowest lane
@@ -1257,6 +1351,7 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
     }
     const bool have = k < n_px && occ != 0.f;      // everything behind a fully opaque fragment has zero weight and zero gradient
     int key = -1, ckey = -1, tkey = -1, t01 = -1, t10 = -1, t11 = -1;
+    bool tcells = false;
     float gv9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float gc9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float tg[3] = {0.f, 0.f, 0.f}, tw[4] = {0.f, 0.f, 0.f, 0.f};      // texture gradient = tg x tw (colour x tap weights)
@@ -1286,7 +1381,7 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
       if (w != 0.f) {
         const float gcx = w * gr, gcy = w * gg, gcz = w * gb;
         if (P.g_maps4) {
-          tkey = tx.tap.i00; t01 = tx.tap.i01; t10 = tx.tap.i10; t11 = tx.tap.i11;
+          tkey = tx.tap.i00; t01 = tx.tap.i01; t10 = tx.tap.i10; t11 = tx.tap.i11; tcells = desc.w != 0;
           tg[0] = gcx; tg[1] = gcy; tg[2] = gcz;
           tw[0] = tx.tap.w00; tw[1] = tx.tap.w01; tw[2] = tx.tap.w10; tw[3] = tx.tap.w11;
         }
@@ -1298,7 +1393,7 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
       if (K1 && DETACH && face >= P.n_static_faces && w != 0.f) need_bary = true;
       occ *= (1.f - a);
     }
-    if (P.g_maps4) warp_tex_scatter(P.g_maps4, tkey, t01, t10, t11, tg, tw, lane);
+    if (P.g_maps4) warp_tex_scatter<K1>(P, tkey, t01, t10, t11, tcells, tg, tw, lane, warp);
     if (!DETACH) {
       if (__ballot_sync(0xffffffffu, key >= 0)) warp_agg_add<9>(P.g_tri + slot_base * 9, 9, key, gv9, lane);
       if (__ballot_sync(0xffffffffu, ckey >= 0)) warp_agg_add<9>(P.g_conv + slot_base * 9, 9, ckey, gc9, lane);
@@ -1767,6 +1862,8 @@ extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const floa
   P.map_table = map_table;
   P.grad_rgba = grad_rgba; P.grad_scale = grad_scale; P.g_tri = need_geom ? g.g_tri : nullptr; P.g_conv = g.g_conv;
   P.g_faces_alpha = g_faces_alpha; P.g_maps4 = g_maps ? (s->maps_are_texels4 ? (float4*)g_maps : g.g_maps4) : nullptr;
+  const int n_entries = s->n_map_floats / 3;
+  if (g_maps && s->maps_are_texels4 == 2) { P.g_cells = g.g_cells; P.n_cells = n_entries; }
   const dim3 grid = bwd_grid(*s);        // see centre_out()
   const size_t smem = frag_smem_bytes(s->faces_per_pixel, DBW_BWD_NT, s->n_maps, P.n_alpha);
   {
@@ -1797,6 +1894,12 @@ extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const floa
       if (e != cudaSuccess) return fail("raster_bary_backward_kernel attribute", e);
       LAUNCH_CK("raster_bary_backward_kernel");
     }
+  }
+  if (P.g_cells) {
+    const int blocks = stride_grid(n_entries, 8);
+    if (blocks < 0) return fail("fold_gcells_kernel: SM count", cudaGetLastError());
+    fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries);
+    LAUNCH_CK("fold_gcells_kernel");
   }
   if (g_maps && !s->maps_are_texels4) {
     const int n_texels = s->n_map_floats / 3;

@@ -297,6 +297,10 @@ __global__ void texture_prep_forward_kernel(const TexJobs J) {
     }
     return;
   }
+  if (stage == DBW_TEX_STAGE_CELLS4) {                                           // (n_maps, CS, CS) float4 cells
+    if (x % f == 0 && y % f == 0) atlas[cell / 3] = make_float4(s[0], s[1], s[2], 0.f);
+    return;
+  }
   const int Wp = TS + p_left + p_right;
   float4* row = atlas + ((size_t)m * TS + y) * Wp;
   const float4 val = make_float4(s[0], s[1], s[2], 0.f);
@@ -320,10 +324,11 @@ __global__ void texture_prep_backward_kernel(const TexJobs J) {
   const int CS = TS / f;
   const size_t cell = (((size_t)m * CS + y / f) * CS + x / f) * 3;
   float g[3] = {0.f, 0.f, 0.f};
-  if (stage == DBW_TEX_STAGE_CELLS) {
-    // `atlas` holds the CELL gradient (n_maps, CS, CS, 3), already summed over the cell's texels (and over ranks)
+  if (stage == DBW_TEX_STAGE_CELLS || stage == DBW_TEX_STAGE_CELLS4) {
+    // `atlas` holds the CELL gradient (n_maps, CS, CS, 3 or 4), already summed over the cell's texels (and over ranks); the
+    // float4 one is read a float at a time: it may be a view of a gradient bucket at any 4-byte offset
     if (ok) {
-      const float* gc = jb.atlas + cell;
+      const float* gc = jb.atlas + (stage == DBW_TEX_STAGE_CELLS4 ? cell / 3 * 4 : cell);
       const size_t o = (((size_t)m * TS + y) * TS + x) * 3;
       const float scale = f == 8 ? 1.f / 64.f : 1.f;
 #pragma unroll
@@ -388,7 +393,9 @@ static int launch_tex(const DbwTexJob* jobs, int n_jobs, bool backward, void* st
   for (int i = 0; i < n_jobs; ++i) {
     const DbwTexJob& j = jobs[i];
     if (!j.textures || !j.atlas || (backward && !j.g_textures)) return dbw_fail_("texture prep: null pointer argument", cudaSuccess);
-    if (j.stage < 0 || j.stage > 2) return dbw_fail_("texture prep: stage must be DBW_TEX_STAGE_FUSED, _CELLS or _EXPAND", cudaSuccess);
+    if (j.stage < 0 || j.stage > 3) return dbw_fail_("texture prep: stage must be DBW_TEX_STAGE_FUSED, _CELLS, _EXPAND or _CELLS4", cudaSuccess);
+    if (j.stage == DBW_TEX_STAGE_CELLS4 && !backward && (reinterpret_cast<uintptr_t>(j.atlas) & 15))
+      return dbw_fail_("texture prep: float4 cells must be 16-byte aligned", cudaSuccess);
     if (check_tex(who, j.n_maps, j.txt_size, j.p_left, j.p_right, j.decimate)) return -1;
     J.j[i] = j; J.zoff[i + 1] = J.zoff[i] + j.n_maps;
     ts_max = j.txt_size > ts_max ? j.txt_size : ts_max;

@@ -23,7 +23,8 @@ import torch.nn.functional as F
 from . import _lib, geometry as G, losses as L
 from .renderer import Renderer, render_scene, _c, _stream
 from .fused_loss import ScenePass, scene_mse
-from .scene_ops import scene_geometry_passes, block_opacities, scene_atlases, scene_texture_cells, atlases_from_cells
+from .scene_ops import (scene_geometry_passes, block_opacities, scene_atlases, scene_texture_cells, atlases_from_cells,
+                        cell_map_table)
 from .structures import Meshes, TexturesUV, join_meshes_as_scene
 
 # accepted keys and defaults of the config sub-dicts (configs/*/*.yml -> model.{mesh,rend_optim,loss}); unknown keys are
@@ -350,9 +351,12 @@ class DifferentiableBlocksWorld(nn.Module):
             return torch.randn(self.alpha_logit.shape, generator=self.noise_generator, device=self.alpha_logit.device)
         return torch.randn_like(self.alpha_logit)
 
-    def _scene_tensors(self, hard_filter):
+    def _scene_tensors(self, hard_filter, cells=False):
         """leaf parameters -> scene kernels -> raw tensors of the two passes:
-        (env verts, env atlas, env map table), (block verts, block atlas, block map table, face_map, per-face opacities)"""
+        (env verts, env atlas, env map table), (block verts, block atlas, block map table, face_map, per-face opacities).
+        cells: while both texture stacks are box-decimated 8x, the "atlases" are the float4 CELLS of scene_texture_cells and the
+        tables describe cell maps -- the passes sample and scatter at the cells (64x fewer texels, no atlas expansion either
+        way); the renders are bit for bit those of the atlases"""
         st = self._static_arrays()
         coarse_training = self.training and self.is_live('coarse_learning')
         decim_env = self.decim_factor if (self.training and self.is_live('decimate_txt')) else 1
@@ -362,25 +366,38 @@ class DifferentiableBlocksWorld(nn.Module):
                                                      st['geom'], st['bkg_world'])
         fmap = self._opacities(hard_filter, coarse_training)
         alpha = None if hard_filter else self._alpha          # one opacity per block: alpha_group = BNF faces share an entry
-        if self.grad_sum_point is not None and decim_env == 8 and decim_blocks == 8:
-            # data parallel: everything the two raster passes differentiate goes through ONE gradient-sum point, textures as
-            # their decimated cells (parallel.GradSumPoint); what lies before it turns summed gradients into leaf gradients
-            cells_env, cells_blk = scene_texture_cells(self.texture_bkg, self.texture_ground, self.textures, decim_env, decim_blocks)
-            summed = self.grad_sum_point(blk_verts, env_verts, cells_env, cells_blk, *([alpha] if alpha is not None else []))
-            blk_verts, env_verts, cells_env, cells_blk = summed[:4]
-            alpha = summed[4] if alpha is not None else None
+        side = self.texture_bkg.shape[1]
+        cells = cells and decim_env == 8 and decim_blocks == 8
+        if cells or (self.grad_sum_point is not None and decim_env == 8 and decim_blocks == 8):
+            cells_env, cells_blk = scene_texture_cells(self.texture_bkg, self.texture_ground, self.textures, decim_env, decim_blocks,
+                                                       texels4=cells)
+            if self.grad_sum_point is not None:
+                # data parallel: everything the two raster passes differentiate goes through ONE gradient-sum point, textures
+                # as their decimated cells (parallel.GradSumPoint); what lies before it turns summed gradients into leaf gradients
+                summed = self.grad_sum_point(blk_verts, env_verts, cells_env, cells_blk, *([alpha] if alpha is not None else []))
+                blk_verts, env_verts, cells_env, cells_blk = summed[:4]
+                alpha = summed[4] if alpha is not None else None
+            if cells:
+                env_atlas, atlas = cells_env, cells_blk
+                env_table = cell_map_table(2, side, decim_env)
+                table = cell_map_table(self.n_blocks, self.textures.shape[1], decim_blocks, *self.txt_padding)
+                self._reg_state_stale = True
+                return (env_verts, env_atlas.reshape(-1, 4), env_table), (blk_verts, atlas.reshape(-1, 4), table, fmap,
+                                                                         self._per_face_alpha(alpha))
             env_atlas, atlas = atlases_from_cells(cells_env, cells_blk, self.txt_padding, decim_env, decim_blocks)
         else:
             env_atlas, atlas = scene_atlases(self.texture_bkg, self.texture_ground, self.textures, self.txt_padding, decim_env, decim_blocks)
         env_atlas = env_atlas.reshape(-1, 4)
-        side = self.texture_bkg.shape[1]
         env_table = [(0, side, side), (side * side * 3, side, side)]
         rows, cols = atlas.shape[1], atlas.shape[2]
         table = [(i * rows * cols * 3, rows, cols) for i in range(self.n_blocks)]
+        self._reg_state_stale = True          # compute_losses() rebuilds what the regularisers read, if they are on
+        return (env_verts, env_atlas, env_table), (blk_verts, atlas.reshape(-1, 4), table, fmap, self._per_face_alpha(alpha))
+
+    def _per_face_alpha(self, alpha):
         if alpha is not None and self.alpha_group_faces == 1:
             alpha = alpha[:, None].expand(-1, self.BNF).reshape(-1)
-        self._reg_state_stale = True          # compute_losses() rebuilds what the regularisers read, if they are on
-        return (env_verts, env_atlas, env_table), (blk_verts, atlas.reshape(-1, 4), table, fmap, alpha)
+        return alpha
 
     def _render_decoupled_fused(self, R, T, hard_filter, renderer):
         """environment pass + blocks pass over the fused scene tensors -> (env RGBA, blocks RGBA)"""
@@ -403,7 +420,7 @@ class DifferentiableBlocksWorld(nn.Module):
         self._install_cameras(inp)
         _, hard_filter, renderer = self._phase()
         st = self._static_arrays()
-        (env_verts, env_atlas, env_table), (blk_verts, atlas, table, fmap, alpha) = self._scene_tensors(hard_filter)
+        (env_verts, env_atlas, env_table), (blk_verts, atlas, table, fmap, alpha) = self._scene_tensors(hard_filter, cells=True)
         key = (id(renderer), id(st['faces_b']), tuple(env_table), tuple(table))
         if self._passes is None or self._passes[0] != key:
             self._passes = (key, ScenePass(st['faces_e'], st['fvu_e'], st['fmap_e'], env_table, self.renderer_env,
@@ -423,7 +440,7 @@ class DifferentiableBlocksWorld(nn.Module):
         """floats a parallel.GradSumPoint moves per step (vertices of both passes, decimated cells of all maps, opacities)"""
         f = self.decim_factor
         ts, side = self.textures.shape[1], self.texture_bkg.shape[1]
-        cells = (self.n_blocks * (ts // f) ** 2 + 2 * (side // f) ** 2) * 3
+        cells = (self.n_blocks * (ts // f) ** 2 + 2 * (side // f) ** 2) * 4          # float4 cells (scene_texture_cells(texels4=True))
         verts = (self.n_blocks * self.sq_eta.shape[1] + self.bkg.verts_packed().shape[0] + self.ground.verts_packed().shape[0]) * 3
         return cells + verts + self.n_blocks + 8
 

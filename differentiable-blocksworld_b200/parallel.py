@@ -5,7 +5,7 @@ Views of a step are independent given the replicated scene parameters, so they s
 rank r renders a contiguous range of the B views (or of their 16-row bands) and back-propagates into its own gradients;
 ONE all-reduce(SUM) per step over NVLink / NVSwitch then gives every rank the full gradient -- either of a single flat
 fp32 bucket of the parameter gradients after the backward (about 9.4 MB for 10 blocks with 256^2 textures), or, while the
-textures are box-decimated, of the scene tensors' gradients inside the backward (GradSumPoint: about 0.16 MB).
+textures are box-decimated, of the scene tensors' gradients inside the backward (GradSumPoint: about 0.21 MB).
 Correctness conditions handled here:
   * the RGB loss is a MEAN over all B views (dbw.py:367): each rank divides by the GLOBAL pixel count
     (model.n_total_views), so the SUM of the per-rank gradients is the gradient of the global mean;
@@ -110,7 +110,7 @@ class GradSumPoint:
     box-decimated CELLS (scene_ops.scene_texture_cells) -- so what lies before the point (texture-cell / geometry / opacity
     backward kernels: deterministic, no atomics) turns GLOBAL gradients into leaf gradients, identically on every rank, and no
     leaf all-reduce follows.  While textures are decimated 8x (the first `decimate_txt` iterations, src/model/dbw.py:276-279,
-    331-334) the cells hold 64x fewer values than the texture parameters: ~0.15 MB per step instead of ~9.4 MB on the DTU shape."""
+    331-334) the cells hold 64x fewer values than the texture parameters: ~0.21 MB per step (float4 cells) instead of ~9.4 MB on the DTU shape."""
 
     def __init__(self, peer):
         self.peer = peer

@@ -122,10 +122,11 @@ _TABLE_CACHE = {}
 
 
 def _device_map_table(table_host, dev):
-    """(M) DbwMapDesc on the device, cached per (layout, device): built once, so that steady-state calls do no H2D."""
+    """(M) DbwMapDesc on the device, cached per (layout, device): built once, so that steady-state calls do no H2D.
+    Entries are (offset, H, W) or (offset, H, W, reserved) -- reserved != 0: a cell map (scene_ops.cell_map_table)."""
     key = (tuple(table_host), str(dev))
     if key not in _TABLE_CACHE:
-        table = (DbwMapDesc * len(table_host))(*[DbwMapDesc(int(o), int(h), int(w), 0) for o, h, w in table_host])
+        table = (DbwMapDesc * len(table_host))(*[DbwMapDesc(*(int(x) for x in e), *([0] if len(e) == 3 else [])) for e in table_host])
         _TABLE_CACHE[key] = torch.frombuffer(bytearray(bytes(table)), dtype=torch.int32).to(dev)
     return _TABLE_CACHE[key]
 
@@ -156,6 +157,19 @@ def make_settings(B, H, W, K, V, Fn, M, alpha_stride, intr, sigma, blur_radius, 
     return s
 
 
+def _check_cell_maps(table_host, maps, texels4):
+    """cell maps (DbwMapDesc.reserved != 0) lie within `maps`, counted in float4 cells (the library only sees the device table)"""
+    for e in table_host:
+        if len(e) < 4 or not e[3]:
+            continue
+        o, h, _, r = (int(x) for x in e[:4])
+        f, p_left = r & 0xff, r >> 8
+        if not texels4 or f not in (2, 4, 8, 16, 32, 64, 128) or h % f or p_left > h or o % 3:
+            raise DbwError(f'bad cell map {tuple(e)}: needs maps_are_texels4, a power-of-two f in [2, 128] dividing H, p_left <= H')
+        if o // 3 + (h // f) ** 2 > maps.numel() // 4:
+            raise DbwError(f'cell map {tuple(e)} reaches past the {maps.numel() // 4} cells of `maps`')
+
+
 def scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigma, faces_per_pixel, z_clip=None,
                    detach_bary=False, clip_inside=True, background=(0., 0., 0.), faces_alpha=None, perspective_correct=True,
                    verts_are_ndc=False, blur_radius=None, maps_are_texels4=False, alpha_group=1, n_static_faces=0, view_rows=None):
@@ -164,6 +178,7 @@ def scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigm
     n_static_faces: leading faces whose vertices are constants (no vertex gradient wanted)."""
     H, W = image_size
     V, Fn = verts.shape[-2], faces.shape[0]
+    _check_cell_maps(map_table_host, maps, maps_are_texels4)
     map_table = _device_map_table(map_table_host, verts.device)
     alpha_stride = 0
     if faces_alpha is not None:
@@ -177,7 +192,8 @@ def scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigm
     cfg = make_settings(B, H, W, faces_per_pixel, V, Fn, len(map_table_host), alpha_stride, intr, sigma, blur_radius,
                         z_clip, background, clip_inside, perspective_correct, True, detach_bary, verts_are_ndc,
                         n_map_floats=(maps.numel() // 4 * 3) if maps_are_texels4 else maps.numel(),
-                        maps_are_texels4=maps_are_texels4,
+                        # 2: float4 maps with cell maps among them (the backward then spreads their gradient over copies)
+                        maps_are_texels4=(2 if any(len(e) > 3 and e[3] for e in map_table_host) else 1) if maps_are_texels4 else 0,
                         # what a backward streams: one 16 B record per kept fragment, written only when one may follow
                         save_fragment_state=torch.is_grad_enabled(), alpha_group=alpha_group, n_static_faces=n_static_faces,
                         view_rows=view_rows)

@@ -207,7 +207,7 @@ class _SceneAtlasesFn(torch.autograd.Function):
         return gb, gg, gk, None, None, None
 
 
-STAGE_FUSED, STAGE_CELLS, STAGE_EXPAND = 0, 1, 2          # DBW_TEX_STAGE_* of include/dbw_render.h
+STAGE_FUSED, STAGE_CELLS, STAGE_EXPAND, STAGE_CELLS4 = 0, 1, 2, 3          # DBW_TEX_STAGE_* of include/dbw_render.h
 
 
 def _tex_launch(jobs, backward):
@@ -217,35 +217,37 @@ def _tex_launch(jobs, backward):
 
 class _SceneCellsFn(torch.autograd.Function):
     """first half of the texture preparation (DBW_TEX_STAGE_CELLS): the three texture stacks -> their CELL colours
-    box_mean(sigmoid(logits)): (2, se/f_env, se/f_env, 3) for background + ground, (N, TS/f_blk, TS/f_blk, 3) for the blocks"""
+    box_mean(sigmoid(logits)): (2, se/f_env, se/f_env, C) for background + ground, (N, TS/f_blk, TS/f_blk, C) for the blocks;
+    C = 3, or 4 (RGB + 0, DBW_TEX_STAGE_CELLS4: the float4 cells the raster passes sample as cell maps)"""
 
     @staticmethod
-    def forward(ctx, tex_bkg, tex_ground, tex_blocks, decim_env, decim_blocks):
+    def forward(ctx, tex_bkg, tex_ground, tex_blocks, decim_env, decim_blocks, texels4):
         tb, tg, tk = (t.detach().contiguous().float() for t in (tex_bkg, tex_ground, tex_blocks))
         se, N, TS = tb.shape[1], tk.shape[0], tk.shape[1]
         assert tb.shape == tg.shape and tb.shape[0] == 1
-        ce, ck = se // decim_env, TS // decim_blocks
-        env = torch.empty(2, ce, ce, 3, device=tb.device, dtype=torch.float32)
-        blk = torch.empty(N, ck, ck, 3, device=tb.device, dtype=torch.float32)
-        _tex_launch([DbwTexJob(tb.data_ptr(), env[0].data_ptr(), None, 1, se, 0, 0, decim_env, STAGE_CELLS),
-                     DbwTexJob(tg.data_ptr(), env[1].data_ptr(), None, 1, se, 0, 0, decim_env, STAGE_CELLS),
-                     DbwTexJob(tk.data_ptr(), blk.data_ptr(), None, N, TS, 0, 0, decim_blocks, STAGE_CELLS)], False)
+        ce, ck, C = se // decim_env, TS // decim_blocks, 4 if texels4 else 3
+        stage = STAGE_CELLS4 if texels4 else STAGE_CELLS
+        env = torch.empty(2, ce, ce, C, device=tb.device, dtype=torch.float32)
+        blk = torch.empty(N, ck, ck, C, device=tb.device, dtype=torch.float32)
+        _tex_launch([DbwTexJob(tb.data_ptr(), env[0].data_ptr(), None, 1, se, 0, 0, decim_env, stage),
+                     DbwTexJob(tg.data_ptr(), env[1].data_ptr(), None, 1, se, 0, 0, decim_env, stage),
+                     DbwTexJob(tk.data_ptr(), blk.data_ptr(), None, N, TS, 0, 0, decim_blocks, stage)], False)
         ctx.save_for_backward(tb, tg, tk)
-        ctx.cfg = (decim_env, decim_blocks)
+        ctx.cfg = (decim_env, decim_blocks, stage)
         return env, blk
 
     @staticmethod
     def backward(ctx, g_env, g_blk):
         tb, tg, tk = ctx.saved_tensors
-        decim_env, decim_blocks = ctx.cfg
+        decim_env, decim_blocks, stage = ctx.cfg
         se, N, TS = tb.shape[1], tk.shape[0], tk.shape[1]
         g_env, g_blk = g_env.contiguous().float(), g_blk.contiguous().float()
         flat = torch.empty(tb.numel() + tg.numel() + tk.numel(), device=tb.device, dtype=torch.float32)
         gb, gg, gk = flat[:tb.numel()].view_as(tb), flat[tb.numel():tb.numel() + tg.numel()].view_as(tg), flat[tb.numel() + tg.numel():].view_as(tk)
-        _tex_launch([DbwTexJob(tb.data_ptr(), g_env[0].data_ptr(), gb.data_ptr(), 1, se, 0, 0, decim_env, STAGE_CELLS),
-                     DbwTexJob(tg.data_ptr(), g_env[1].data_ptr(), gg.data_ptr(), 1, se, 0, 0, decim_env, STAGE_CELLS),
-                     DbwTexJob(tk.data_ptr(), g_blk.data_ptr(), gk.data_ptr(), N, TS, 0, 0, decim_blocks, STAGE_CELLS)], True)
-        return gb, gg, gk, None, None
+        _tex_launch([DbwTexJob(tb.data_ptr(), g_env[0].data_ptr(), gb.data_ptr(), 1, se, 0, 0, decim_env, stage),
+                     DbwTexJob(tg.data_ptr(), g_env[1].data_ptr(), gg.data_ptr(), 1, se, 0, 0, decim_env, stage),
+                     DbwTexJob(tk.data_ptr(), g_blk.data_ptr(), gk.data_ptr(), N, TS, 0, 0, decim_blocks, stage)], True)
+        return gb, gg, gk, None, None, None
 
 
 class _AtlasesFromCellsFn(torch.autograd.Function):
@@ -276,11 +278,20 @@ class _AtlasesFromCellsFn(torch.autograd.Function):
         return ge, gk, None, None, None
 
 
-def scene_texture_cells(texture_bkg, texture_ground, textures, decim_env=1, decim_blocks=1):
+def scene_texture_cells(texture_bkg, texture_ground, textures, decim_env=1, decim_blocks=1, texels4=False):
     """(environment cells (2, se/f, se/f, 3), block cells (N, TS/f, TS/f, 3)): sigmoid + box mean of the three texture stacks, one
     launch.  With atlases_from_cells() it equals scene_atlases() bit for bit; the cells are where a data-parallel step sums its
-    texture gradients (64x fewer values than the parameters while textures are decimated)."""
-    return _SceneCellsFn.apply(texture_bkg, texture_ground, textures, int(decim_env), int(decim_blocks))
+    texture gradients (64x fewer values than the parameters while textures are decimated).  texels4: float4 cells (last dim 4,
+    RGB + 0), which the raster passes sample directly through cell_map_table() -- no atlas in between."""
+    return _SceneCellsFn.apply(texture_bkg, texture_ground, textures, int(decim_env), int(decim_blocks), bool(texels4))
+
+
+def cell_map_table(n_maps, txt_size, decimate, p_left=0, p_right=0):
+    """map table [(offset, H, W, reserved)] of `n_maps` float4 cell maps stored back to back (scene_texture_cells(...,
+    texels4=True)): each samples as the (txt_size, p_left + txt_size + p_right) atlas that atlases_from_cells() would expand it
+    to (DbwMapDesc / DBW_MAP_CELLS in include/dbw_render.h)"""
+    cs = txt_size // decimate
+    return [(i * cs * cs * 3, txt_size, txt_size + p_left + p_right, (p_left << 8) | decimate) for i in range(n_maps)]
 
 
 def atlases_from_cells(cells_env, cells_blk, pad, decim_env=1, decim_blocks=1):

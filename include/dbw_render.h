@@ -55,7 +55,11 @@ typedef struct DbwRenderSettings {
   int32_t verts_are_ndc;      /* 1: `verts` is (B,V,3) = (x_ndc, y_ndc, z_view) and R/T/K are ignored                 */
   int32_t n_map_floats;       /* total floats in `maps` (= 3 * sum_m H_m*W_m): sizes the library's float4 texel scratch    */
   int32_t maps_are_texels4;   /* 1: `maps` (and `g_maps`) are already RGB+pad float4 texel atlases (dbw_texture_prep_*);
-                                 DbwMapDesc.offset keeps its meaning (3 * first texel index)                              */
+                                 DbwMapDesc.offset keeps its meaning (3 * first texel index).  2: the same, and the table
+                                 holds cell maps (DBW_MAP_CELLS): the backward spreads their gradient atomics over
+                                 DBW_CELL_GRAD_COPIES copies in its scratch and adds the copies into g_maps at the end (a
+                                 cell collects the gradient of f x f texels: one copy would serialise the atomics of
+                                 every warp that covers it)                                                               */
   int32_t save_fragment_state;/* 1: the forward also keeps one 16 B record {triangle slot | closest edge, u, v, signed squared
                                  distance} per kept fragment (+ a per-pixel count byte) in its workspace; dbw_render_backward*
                                  streams these instead of re-deriving geometry and REQUIRES them.  Costs
@@ -71,8 +75,18 @@ typedef struct DbwRenderSettings {
                                  over 8 ranks (SURVEY 8e)                                                                   */
 } DbwRenderSettings;
 
-/* Texture table entry: map m lives at maps[offset .. offset + height*width*3), row-major (H, W, 3). */
+/* Texture table entry: map m lives at maps[offset .. offset + height*width*3), row-major (H, W, 3).
+ * reserved = 0: that layout.  reserved = DBW_MAP_CELLS(f, p_left): a CELL map -- an f x f box-decimated square texture
+ * (DBW_TEX_STAGE_CELLS4 output, maps_are_texels4 = 2) stored as its (height/f) x (height/f) cells, row-major, one float4 per
+ * cell, from cell offset / 3 on.  height and width still describe the logical atlas the cells stand for (TS rows,
+ * p_left + TS + p_right columns of circular padding along u, as DBW_TEX_STAGE_EXPAND would write it), so sampling is
+ * unchanged: every bilinear tap reads (and its gradient goes to) the cell its atlas texel would repeat.  Renders are bit
+ * for bit those of the expanded atlas; texture gradients are the atlas gradients summed per cell (what
+ * DBW_TEX_STAGE_EXPAND's backward computes), up to summation order.  The caller keeps offset / 3 + (height/f)^2 within the
+ * n_map_floats / 3 cells of `maps`.  f is a power of two in [2, 128], height % f == 0, 0 <= p_left <= height. */
 typedef struct DbwMapDesc { int32_t offset, height, width, reserved; } DbwMapDesc;
+#define DBW_MAP_CELLS(f, p_left) (((p_left) << 8) | (f))
+#define DBW_CELL_GRAD_COPIES 8
 
 int dbw_abi_version(void);
 /* Test hook: 1 = hard single-layer renders (K = 1, sigma = 0) go through the generic raster kernel instead of their dedicated one. */
@@ -245,11 +259,15 @@ int dbw_opacity_backward(const float* alpha_logit, const float* noise, float noi
  *   DBW_TEX_STAGE_CELLS   logits -> cells, written to `atlas`                 (backward: `atlas` = CELL gradient -> logit gradient)
  *   DBW_TEX_STAGE_EXPAND  cells (passed as `textures`) -> atlas               (backward: atlas gradient -> cell gradient, written
  *                                                                              to `g_textures`; `textures` is not read)
+ *   DBW_TEX_STAGE_CELLS4  as CELLS, but the cells are float4 (RGB + 0, 16-byte aligned): the maps of DBW_MAP_CELLS map
+ *                         table entries, which the raster kernels sample without an atlas (backward: `atlas` = float4 cell
+ *                         gradient, read with 4-byte loads -> logit gradient)
  * CELLS then EXPAND equals FUSED bit for bit, forward and backward. */
 #define DBW_MAX_TEX_JOBS 4
 #define DBW_TEX_STAGE_FUSED 0
 #define DBW_TEX_STAGE_CELLS 1
 #define DBW_TEX_STAGE_EXPAND 2
+#define DBW_TEX_STAGE_CELLS4 3
 typedef struct DbwTexJob {
   const float* textures; float* atlas; float* g_textures;
   int32_t n_maps, txt_size, p_left, p_right, decimate, stage;
