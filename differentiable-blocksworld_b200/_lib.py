@@ -45,6 +45,11 @@ class DbwTexJob(ctypes.Structure):
                 ('decimate', ctypes.c_int32), ('stage', ctypes.c_int32)]
 
 
+class DbwEvalGrid(ctypes.Structure):
+    _fields_ = [('origin', ctypes.c_double * 3), ('cell', ctypes.c_double), ('dims', ctypes.c_int64 * 3),
+                ('block', ctypes.c_int32), ('reserved', ctypes.c_int32)]
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -57,7 +62,9 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_sizeof_setti
            'dbw_scene_geometry_backward', 'dbw_scene_geometry_forward_env', 'dbw_scene_geometry_backward_parts',
            'dbw_opacity_forward', 'dbw_opacity_backward', 'dbw_texture_prep_forward', 'dbw_texture_prep_backward',
            'dbw_texture_prep_forward_multi', 'dbw_texture_prep_backward_multi',
-           'dbw_comm_create', 'dbw_comm_buffer', 'dbw_comm_ipc_handle', 'dbw_comm_connect', 'dbw_comm_all_reduce', 'dbw_comm_error', 'dbw_comm_destroy']
+           'dbw_comm_create', 'dbw_comm_buffer', 'dbw_comm_ipc_handle', 'dbw_comm_connect', 'dbw_comm_all_reduce', 'dbw_comm_error', 'dbw_comm_destroy',
+           'dbw_eval_sample_setup', 'dbw_eval_sample_count', 'dbw_eval_sample_write', 'dbw_eval_cell_keys',
+           'dbw_eval_cell_ranges', 'dbw_eval_downsample_workspace_bytes', 'dbw_eval_radius_downsample', 'dbw_eval_nn_distance']
 
 _lib = None
 
@@ -110,6 +117,16 @@ def lib():
         L.dbw_timing_enable.restype = None
         L.dbw_timing_reset.restype = None
         L.dbw_timing_read.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_int)]
+        i64, gp = ctypes.c_int64, ctypes.POINTER(DbwEvalGrid)
+        L.dbw_eval_sample_setup.argtypes = [vp, vp, i64, vp, vp, vp]
+        L.dbw_eval_sample_count.argtypes = [vp, vp, i64, i64, vp, vp]
+        L.dbw_eval_sample_write.argtypes = [vp, vp, i64, i64, vp, vp, vp, vp]
+        L.dbw_eval_cell_keys.argtypes = [vp, i64, gp, vp, vp]
+        L.dbw_eval_cell_ranges.argtypes = [vp, vp, i64, gp, vp, vp, vp]
+        L.dbw_eval_downsample_workspace_bytes.argtypes = [i64, ctypes.POINTER(sz)]
+        L.dbw_eval_radius_downsample.argtypes = [vp] * 5 + [i64, ctypes.c_double, ctypes.c_int32, vp,
+                                                            ctypes.POINTER(ctypes.c_int32), vp, sz, vp]
+        L.dbw_eval_nn_distance.argtypes = [vp, i64, vp, vp, gp, ctypes.c_double, vp, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

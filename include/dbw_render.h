@@ -322,6 +322,63 @@ int dbw_comm_all_reduce(void* comm, float* buf, size_t n_floats, void* stream);
 int dbw_comm_error(void* comm, int32_t* out);
 int dbw_comm_destroy(void* comm);
 
+/*
+ * DTU chamfer evaluation (the reference's utils/dtu_eval.evaluate_mesh, run at the end of Trainer.evaluate() on a DTU
+ * scene): mesh point sampling, greedy radius downsampling and exact nearest-neighbour distances, all in fp64 with
+ * non-contracting arithmetic (bit-identical samples, distances sqrt((dx^2 + dy^2) + dz^2)).  Points are (N,3) double.
+ * The entry points are the per-point stages; scans and sorts between them are the caller's (dbw_b200/dtu_eval.py
+ * uses torch.cumsum / torch.sort).  Same conventions as above: device pointers, caller-owned buffers, `stream`, 0 = ok.
+ *
+ * Uniform grid of cells of edge `cell` from `origin`; dims are cell counts per axis.  block = 1: a point's key is its
+ * linear cell (x + nx * (y + ny * z)).  block = B > 1 (dims multiples of B): block-major keys, so that the B^3 cells of one
+ * block are consecutive and a block's occupancy is the difference of two cell offsets.  Cell coordinates are clamped into
+ * the grid.
+ */
+typedef struct DbwEvalGrid {
+  double origin[3];
+  double cell;
+  int64_t dims[3];
+  int32_t block, reserved;
+} DbwEvalGrid;
+
+/* Sampling, pass 1 (per triangle): tri (F,12) records (t0, v1, v2, n1, n2, -) and n_rows (F): the lattice rows of each
+ * triangle (0 for zero-area triangles and triangles with n1 == 0 or n2 == 0).  faces (F,3) int64 index verts (V,3). */
+int dbw_eval_sample_setup(const double* verts, const int64_t* faces, int64_t n_faces, double* tri, int64_t* n_rows, void* stream);
+/* Pass 2 (per row): row_begin (F+1) = exclusive scan of n_rows; row_count (n_rows_total) = samples of each row. */
+int dbw_eval_sample_count(const double* tri, const int64_t* row_begin, int64_t n_faces, int64_t n_rows_total,
+                          int64_t* row_count, void* stream);
+/* Pass 3 (one warp per row): sample_begin (n_rows_total) = exclusive scan of row_count; out (S,3) receives the samples
+ * in the reference's order (triangle, then row-major over (i, j)). */
+int dbw_eval_sample_write(const double* tri, const int64_t* row_begin, int64_t n_faces, int64_t n_rows_total,
+                          const int64_t* row_count, const int64_t* sample_begin, double* out, void* stream);
+
+/* keys (N) int64 of points (N,3) on `grid` (a HOST pointer). */
+int dbw_eval_cell_keys(const double* points, int64_t n, const DbwEvalGrid* grid, int64_t* keys, void* stream);
+
+/* Greedy radius downsample = the lexicographically-first maximal independent set of the graph dist <= radius, in ORDER
+ * (a point's rank is its position in the shuffled cloud).  Inputs, on a block = 1 grid whose cell is >= radius:
+ *   points   (N,3) sorted by cell key;  rank (N) int64 order position of each sorted point
+ *   cell_of  (N) int32 index of each sorted point's cell in the C occupied cells
+ *   nbr_begin, nbr_end (C,9) int32: sorted-point ranges of the 3x3x3 neighbourhood, one x-run per (dy, dz)
+ *            (dbw_eval_cell_ranges)
+ * Output keep (N) uint8 indexed by RANK.  Runs parallel rounds (keep a point once every earlier neighbour is removed,
+ * remove it once one is kept) until every point is decided, reading a device counter after each round: this call
+ * synchronises `stream`.  *rounds_out (host) = rounds run; more than max_rounds is an error, never a spin. */
+int dbw_eval_cell_ranges(const int64_t* cell_keys, const int64_t* cell_begin, int64_t n_cells, const DbwEvalGrid* grid,
+                         int32_t* nbr_begin, int32_t* nbr_end, void* stream);
+int dbw_eval_downsample_workspace_bytes(int64_t n, size_t* bytes);
+int dbw_eval_radius_downsample(const double* points, const int64_t* rank, const int32_t* cell_of, const int32_t* nbr_begin,
+                               const int32_t* nbr_end, int64_t n, double radius, int32_t max_rounds, uint8_t* keep,
+                               int32_t* rounds_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Exact 1-NN distance of each query to the targets, searched within max_dist: dist (n_queries) = the distance when one
+ * is < max_dist, +inf otherwise.  targets (n_targets,3) sorted by block-major key on `grid` (block > 1);
+ * cell_start (dims product + 1) int32 = first sorted target of each key.  The search walks rings of blocks around the
+ * query, skips empty blocks and blocks farther than the best distance so far, and stops once the next ring cannot hold
+ * anything closer.  Queries are best passed sorted by the same keys (coherent warps). */
+int dbw_eval_nn_distance(const double* queries, int64_t n_queries, const double* targets, const int32_t* cell_start,
+                         const DbwEvalGrid* grid, double max_dist, double* dist, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
