@@ -64,7 +64,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_sizeof_setti
            'dbw_texture_prep_forward_multi', 'dbw_texture_prep_backward_multi',
            'dbw_comm_create', 'dbw_comm_buffer', 'dbw_comm_ipc_handle', 'dbw_comm_connect', 'dbw_comm_all_reduce', 'dbw_comm_error', 'dbw_comm_destroy',
            'dbw_eval_sample_setup', 'dbw_eval_sample_count', 'dbw_eval_sample_write', 'dbw_eval_cell_keys',
-           'dbw_eval_cell_ranges', 'dbw_eval_downsample_workspace_bytes', 'dbw_eval_radius_downsample', 'dbw_eval_nn_distance']
+           'dbw_eval_cell_ranges', 'dbw_eval_downsample_workspace_bytes', 'dbw_eval_radius_downsample', 'dbw_eval_nn_distance',
+           'dbw_knn_forward', 'dbw_knn_backward']
 
 _lib = None
 
@@ -127,6 +128,8 @@ def lib():
         L.dbw_eval_radius_downsample.argtypes = [vp] * 5 + [i64, ctypes.c_double, ctypes.c_int32, vp,
                                                             ctypes.POINTER(ctypes.c_int32), vp, sz, vp]
         L.dbw_eval_nn_distance.argtypes = [vp, i64, vp, vp, gp, ctypes.c_double, vp, vp]
+        L.dbw_knn_forward.argtypes = [vp] * 4 + [i64] * 3 + [ctypes.c_int32] + [vp] * 3
+        L.dbw_knn_backward.argtypes = [vp] * 6 + [i64] * 3 + [ctypes.c_int32] + [vp] * 3
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

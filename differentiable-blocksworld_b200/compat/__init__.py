@@ -10,9 +10,11 @@ iopath (SURVEY.md 8b "Caveat", 8f rank 3).
 
 What is real: `toolz`'s five dict helpers, the PyTorch3D containers / constructors the model surface hands to the trainer
 (`Meshes`, `TexturesUV`, `join_meshes_as_*`, `ico_sphere`, `SubdivideMeshes`, the 6D-rotation transforms -- all this repo's
-own implementations), the two `seaborn` / `matplotlib.colors` calls behind the block colour map (`utils/plot.py:77-87`).
-Everything else the reference imports at module load but only calls on its export / evaluation paths (PLY / OBJ I/O, point
-sampling, ICP, chamfer, Open3D, video writing, plotting, LPIPS weights) is a named placeholder that raises
+own implementations), the point-cloud ops of the reference's 3-D evaluation (`knn_points` / `knn_gather` on the sm_90a
+k-NN kernels, the chamfer helpers and `chamfer_distance`, `sample_points_from_meshes`: dbw_b200/pointcloud.py), the two
+`seaborn` / `matplotlib.colors` calls behind the block colour map (`utils/plot.py:77-87`).
+Everything else the reference imports at module load but only calls on its export / evaluation paths (PLY / OBJ I/O, the
+SVD ICP, `Pointclouds`, Open3D, video writing, plotting, LPIPS weights) is a named placeholder that raises
 `NotImplementedError` when CALLED: the control plane stays out of scope (SURVEY 8), the import graph is satisfied."""
 import colorsys
 import importlib
@@ -25,6 +27,7 @@ import torch
 from torch import nn
 
 from .. import geometry as G
+from .. import pointcloud as PC
 from ..structures import Meshes, TexturesUV, join_meshes_as_batch, join_meshes_as_scene
 
 
@@ -104,16 +107,17 @@ def _pytorch3d():
     _module('pytorch3d.utils', ico_sphere=_ico_sphere)
     _module('pytorch3d.transforms', rotation_6d_to_matrix=G.rotation_6d_to_matrix, matrix_to_rotation_6d=G.matrix_to_rotation_6d,
             random_rotations=lambda n, dtype=None, device=None: G.random_rotations(n).to(device=device, dtype=dtype or torch.float32))
-    _module('pytorch3d.ops', SubdivideMeshes=SubdivideMeshes, sample_points_from_meshes=P('ops.sample_points_from_meshes'),
-            iterative_closest_point=P('ops.iterative_closest_point'), knn_points=P('ops.knn_points'), knn_gather=P('ops.knn_gather'))
+    _module('pytorch3d.ops', SubdivideMeshes=SubdivideMeshes, sample_points_from_meshes=PC.sample_points_from_meshes,
+            iterative_closest_point=P('ops.iterative_closest_point'), knn_points=PC.knn_points, knn_gather=PC.knn_gather)
     _module('pytorch3d.ops.subdivide_meshes', SubdivideMeshes=SubdivideMeshes)
-    _module('pytorch3d.ops.knn', knn_points=P('ops.knn.knn_points'), knn_gather=P('ops.knn.knn_gather'))
+    _module('pytorch3d.ops.knn', knn_points=PC.knn_points, knn_gather=PC.knn_gather)
     _module('pytorch3d.io', save_ply=P('io.save_ply'), load_ply=P('io.load_ply'), save_obj=P('io.save_obj'),
             load_obj=P('io.load_obj'), load_objs_as_meshes=P('io.load_objs_as_meshes'))
     _module('pytorch3d.io.utils', _open_file=P('io.utils._open_file'))
-    _module('pytorch3d.loss', mesh_normal_consistency=P('loss.mesh_normal_consistency'), chamfer_distance=P('loss.chamfer_distance'))
-    _module('pytorch3d.loss.chamfer', _validate_chamfer_reduction_inputs=P('loss.chamfer._validate_chamfer_reduction_inputs'),
-            _handle_pointcloud_input=P('loss.chamfer._handle_pointcloud_input'))
+    _module('pytorch3d.loss', mesh_normal_consistency=P('loss.mesh_normal_consistency'), chamfer_distance=PC.chamfer_distance)
+    _module('pytorch3d.loss.chamfer', chamfer_distance=PC.chamfer_distance,
+            _validate_chamfer_reduction_inputs=PC._validate_chamfer_reduction_inputs,
+            _handle_pointcloud_input=PC._handle_pointcloud_input)
     names = ['FoVPerspectiveCameras', 'PerspectiveCameras', 'RasterizationSettings', 'MeshRenderer', 'MeshRasterizer', 'BlendParams',
              'DirectionalLights', 'PointLights', 'AmbientLights', 'TexturesVertex', 'look_at_view_transform', 'look_at_rotation',
              'SoftPhongShader', 'HardPhongShader', 'SoftSilhouetteShader', 'Materials']

@@ -379,6 +379,30 @@ int dbw_eval_radius_downsample(const double* points, const int64_t* rank, const 
 int dbw_eval_nn_distance(const double* queries, int64_t n_queries, const double* targets, const int32_t* cell_start,
                          const DbwEvalGrid* grid, double max_dist, double* dist, void* stream);
 
+/*
+ * k-nearest neighbours (pytorch3d.ops.knn_points, D = 3, squared L2): the search under the reference's chamfer distance
+ * (src/utils/chamfer.py), hence ChamferLoss, gradient_icp and the chamfer legs of ems_eval.py / mbf_eval.py.  Exact brute
+ * force.  p1 (N,P1,3), p2 (N,P2,3) fp32; lengths1, lengths2 (N) int64 (clamped to [0, P]); N <= 65535, P < 2^31 - 1.
+ *
+ * dbw_knn_forward writes every element of dists (N,P1,K) fp32 and idx (N,P1,K) int64 (no zero-fill needed):
+ *  - per query i < lengths1[n], the K nearest of p2[n, :lengths2[n]] in ascending (distance, index) order: ties go to
+ *    the lower index;
+ *  - distance = (dx*dx + dy*dy) + dz*dz, dx = p1.x - p2.x, each operation rounded to nearest fp32 (no contraction);
+ *  - a target at a distance that is not below +inf (overflow, NaN) is never selected;
+ *  - padding as PyTorch3D 0.7.1 (as recalled): rows i >= lengths1[n] and slots beyond the points found are dist 0, idx 0.
+ * 1 <= K <= DBW_KNN_MAX_K.
+ *
+ * dbw_knn_backward: for i < lengths1[n] and k < min(K, lengths2[n]), with j = idx[n,i,k] (skipped outside
+ * [0, lengths2[n])) and g = grad_dists[n,i,k]:  grad_p1[n,i] += 2 g (p1[n,i] - p2[n,j]),  grad_p2[n,j] -= the same
+ * (fp32 atomics: the order of the additions into grad_p2 is not fixed).  The caller zero-fills both.
+ */
+#define DBW_KNN_MAX_K 32
+int dbw_knn_forward(const float* p1, const float* p2, const int64_t* lengths1, const int64_t* lengths2, int64_t N, int64_t P1,
+                    int64_t P2, int32_t K, float* dists, int64_t* idx, void* stream);
+int dbw_knn_backward(const float* p1, const float* p2, const int64_t* lengths1, const int64_t* lengths2, const int64_t* idx,
+                     const float* grad_dists, int64_t N, int64_t P1, int64_t P2, int32_t K, float* grad_p1, float* grad_p2,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
