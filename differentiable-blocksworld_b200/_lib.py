@@ -50,6 +50,11 @@ class DbwEvalGrid(ctypes.Structure):
                 ('block', ctypes.c_int32), ('reserved', ctypes.c_int32)]
 
 
+class DbwLpipsNet(ctypes.Structure):
+    _fields_ = [('conv_w', ctypes.c_void_p * 13), ('conv_b', ctypes.c_void_p * 13), ('lin_w', ctypes.c_void_p * 5),
+                ('shift', ctypes.c_void_p), ('scale', ctypes.c_void_p), ('prepared', ctypes.c_void_p)]
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -65,7 +70,9 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_sizeof_setti
            'dbw_comm_create', 'dbw_comm_buffer', 'dbw_comm_ipc_handle', 'dbw_comm_connect', 'dbw_comm_all_reduce', 'dbw_comm_error', 'dbw_comm_destroy',
            'dbw_eval_sample_setup', 'dbw_eval_sample_count', 'dbw_eval_sample_write', 'dbw_eval_cell_keys',
            'dbw_eval_cell_ranges', 'dbw_eval_downsample_workspace_bytes', 'dbw_eval_radius_downsample', 'dbw_eval_nn_distance',
-           'dbw_knn_forward', 'dbw_knn_backward']
+           'dbw_knn_forward', 'dbw_knn_backward',
+           'dbw_lpips_workspace_bytes', 'dbw_lpips_prepare_weights', 'dbw_lpips_forward', 'dbw_lpips_backward',
+           'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward']
 
 _lib = None
 
@@ -130,6 +137,16 @@ def lib():
         L.dbw_eval_nn_distance.argtypes = [vp, i64, vp, vp, gp, ctypes.c_double, vp, vp]
         L.dbw_knn_forward.argtypes = [vp] * 4 + [i64] * 3 + [ctypes.c_int32] + [vp] * 3
         L.dbw_knn_backward.argtypes = [vp] * 6 + [i64] * 3 + [ctypes.c_int32] + [vp] * 3
+        i32, np_ = ctypes.c_int32, ctypes.POINTER(DbwLpipsNet)
+        L.dbw_lpips_workspace_bytes.argtypes = [i64, i32, i32, i32, ctypes.POINTER(sz), ctypes.POINTER(sz)]
+        L.dbw_lpips_prepare_weights.argtypes = [np_, vp]
+        L.dbw_lpips_forward.argtypes = [np_, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, sz, vp]
+        L.dbw_lpips_backward.argtypes = [np_, vp, i64, i32, i32, i32, i32, vp, vp, sz, vp]
+        L.dbw_lpips_conv3x3.argtypes = [vp] * 5 + [i64] + [i32] * 5 + [vp]
+        L.dbw_lpips_conv_first.argtypes = [vp] * 5 + [i32, vp, i64, i32, i32, vp]
+        L.dbw_lpips_dgrad_last.argtypes = [vp] * 3 + [i32, vp, i64, i32, i32, vp]
+        L.dbw_lpips_maxpool.argtypes = [vp, vp, i64, i32, i32, i32, vp]
+        L.dbw_lpips_maxpool_backward.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

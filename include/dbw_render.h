@@ -403,6 +403,58 @@ int dbw_knn_backward(const float* p1, const float* p2, const int64_t* lengths1, 
                      const float* grad_dists, int64_t N, int64_t P1, int64_t P2, int32_t K, float* grad_p1, float* grad_p2,
                      void* stream);
 
+/*
+ * LPIPS (lpips 0.1.4, LPIPS(net='vgg', version='0.1'), as recalled): the perceptual term of the reference's objective.
+ * in0 (imgs), in1 (rec): (B,3,H,W) fp32 NCHW, 16 <= H, W (relu5_3 is then at least 1x1), 1 <= B <= 65535,
+ * B*H*W < 2^31 - 128.  value[b] = sum over the taps relu1_2 .. relu5_3 of the spatial mean of
+ * lin_k . (dropout(n0 - n1)^2), n = f / (||f||_2 over channels + 1e-10).  With `normalize` the images are first mapped by
+ * 2x - 1; then (x - shift) / scale.  The convolutions of 64..512 channels take TF32 operands (round to nearest, ties
+ * away from zero) and accumulate in fp32; the first layer and its input-gradient are fp32.
+ *
+ * Dropout (p = 0.5, the reference's lin layers in training mode): with `train`, each (image, tap, channel, pixel) element
+ * of the squared difference is kept and doubled when the hash of csrc/dbw_lpips_hash.cuh, for the seed *seed, says so,
+ * and zeroed otherwise.  The forward copies *seed into the workspace for the backward and then increments *seed on the
+ * device, so a captured graph draws a fresh mask on every replay.
+ *
+ * conv_w[l] (C_out, C_in, 3, 3) and conv_b[l] (C_out) of the 13 layers of torchvision's vgg16.features[0:30], lin_w[k]
+ * (C_k) of the 5 heads, shift and scale (3): device fp32.  `prepared` (prepared_bytes from dbw_lpips_workspace_bytes)
+ * holds the TF32-rounded forward copies [co][ky][kx][ci] and input-gradient copies [ci][2-ky][2-kx][co] of layers 1..12,
+ * written by dbw_lpips_prepare_weights (again whenever the weights change).
+ *
+ * dbw_lpips_forward writes value (B).  With save_for_backward it keeps in the workspace what dbw_lpips_backward needs:
+ * every activation of in1, the taps of in0, the seed used; without it, the workspace (sized with the same flag) holds
+ * only the taps of both images.  dbw_lpips_backward writes grad_in1 (B,3,H,W) = sum_b grad_value[b] d value[b] / d in1
+ * from the workspace of a save_for_backward forward (the same normalize and train; the workspace untouched in between).  Both run on `stream` only: no
+ * allocation, no synchronisation (capturable).  The single-layer entry points run the same kernels; dbw_lpips_conv3x3 takes
+ * a K-major weight wt[co][(ky*3+kx)*C_in + ci] already TF32-rounded, and optional bias, and mask (out *= [mask > 0]).
+ */
+typedef struct DbwLpipsNet {
+  const float* conv_w[13];
+  const float* conv_b[13];
+  const float* lin_w[5];
+  const float* shift;
+  const float* scale;
+  void* prepared;
+} DbwLpipsNet;
+
+int dbw_lpips_workspace_bytes(int64_t B, int32_t H, int32_t W, int32_t save_for_backward, size_t* workspace_bytes,
+                              size_t* prepared_bytes);
+int dbw_lpips_prepare_weights(const DbwLpipsNet* net, void* stream);
+int dbw_lpips_forward(const DbwLpipsNet* net, const float* in0, const float* in1, int64_t B, int32_t H, int32_t W, int32_t normalize,
+                      int32_t train, int32_t save_for_backward, uint32_t* seed, float* value, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int dbw_lpips_backward(const DbwLpipsNet* net, const float* grad_value, int64_t B, int32_t H, int32_t W, int32_t normalize,
+                       int32_t train, float* grad_in1, void* workspace, size_t workspace_bytes, void* stream);
+int dbw_lpips_conv3x3(const float* in, const float* wt, const float* bias, const float* mask, float* out, int64_t B, int32_t H,
+                      int32_t W, int32_t C_in, int32_t C_out, int32_t relu, void* stream);
+int dbw_lpips_conv_first(const float* x, const float* w, const float* bias, const float* shift, const float* scale, int32_t normalize,
+                         float* out, int64_t B, int32_t H, int32_t W, void* stream);
+int dbw_lpips_dgrad_last(const float* g, const float* w, const float* scale, int32_t normalize, float* out, int64_t B, int32_t H,
+                         int32_t W, void* stream);
+int dbw_lpips_maxpool(const float* in, float* out, int64_t B, int32_t H, int32_t W, int32_t C, void* stream);
+int dbw_lpips_maxpool_backward(const float* in, const float* gout, float* gin, int64_t B, int32_t H, int32_t W, int32_t C,
+                               void* stream);
+
 #ifdef __cplusplus
 }
 #endif
