@@ -29,6 +29,7 @@
 #include "../../include/dbw_render.h"
 #include "dbw_math.cuh"
 #include "dbw_fraglist.cuh"
+#include "dbw_camera.cuh"
 
 // ------------------------------------------------------------------------------------------------ error plumbing
 static thread_local char g_err[512] = "";
@@ -225,18 +226,9 @@ __global__ void project_verts_backward_kernel(const float* __restrict__ vw, cons
   float ax = 0.f, ay = 0.f, az = 0.f;
   for (int b = lane; b < B; b += 32) {
     const float* r = R + b * 9; const float* t = T + b * 3;
-    const float xv = X * r[0] + Y * r[3] + Z * r[6] + t[0];
-    const float yv = X * r[1] + Y * r[4] + Z * r[7] + t[1];
-    const float zv = X * r[2] + Y * r[5] + Z * r[8] + t[2];
-    const float sgn = (zv > 0.f) ? 1.f : ((zv < 0.f) ? -1.f : 1.f);
-    const bool clamped = fabsf(zv) < eps;
-    const float den = sgn * fmaxf(fabsf(zv), eps);
     const float* g = g_ndc + ((size_t)b * V + v) * 3;
-    const float gx = g[0], gy = g[1], gz = g[2];
-    const float nx = fx * xv + px * zv, ny = fy * yv + py * zv;
-    const float gxv = gx * fx / den, gyv = gy * fy / den;
-    float gzv = gz + (gx * px + gy * py) / den;
-    if (!clamped) gzv -= (gx * nx + gy * ny) / (den * den);
+    float gxv, gyv, gzv;
+    dbw_project_backward(X, Y, Z, r, t, fx, fy, px, py, eps, g[0], g[1], g[2], gxv, gyv, gzv);
     ax += r[0] * gxv + r[1] * gyv + r[2] * gzv;
     ay += r[3] * gxv + r[4] * gyv + r[5] * gzv;
     az += r[6] * gxv + r[7] * gyv + r[8] * gzv;
@@ -246,6 +238,46 @@ __global__ void project_verts_backward_kernel(const float* __restrict__ vw, cons
     ax += __shfl_xor_sync(0xffffffffu, ax, o); ay += __shfl_xor_sync(0xffffffffu, ay, o); az += __shfl_xor_sync(0xffffffffu, az, o);
   }
   if (lane == 0) { g_vw[v * 3] += ax; g_vw[v * 3 + 1] += ay; g_vw[v * 3 + 2] += az; }
+}
+
+// Gradient of the camera poses: one CTA per view sums X_world (x) g_view over the vertices (g_view: the same Jacobian as
+// project_verts_backward_kernel) in a fixed order -- per thread, then xor-shuffles, then the warps in index order -- and
+// adds the view's 9 + 3 sums into g_R / g_T.  Each element receives one atomic add per call, so the two passes of a fused
+// step may accumulate into the same buffers from two streams and still sum to the same bits.
+#define DBW_CAM_NT 256
+__global__ void __launch_bounds__(DBW_CAM_NT) camera_grad_kernel(const float* __restrict__ vw, const float* __restrict__ R,
+                                                                 const float* __restrict__ T, float fx, float fy, float px, float py,
+                                                                 float eps, int V, const float* __restrict__ g_ndc,
+                                                                 float* __restrict__ g_R, float* __restrict__ g_T) {
+  __shared__ float s_part[DBW_CAM_NT / 32][12];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* r = R + b * 9; const float* t = T + b * 3;
+  float acc[12] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};     // g_R (9), g_T (3)
+  for (int v = tid; v < V; v += DBW_CAM_NT) {
+    const float* g = g_ndc + ((size_t)b * V + v) * 3;
+    const float gx = g[0], gy = g[1], gz = g[2];
+    if (gx == 0.f && gy == 0.f && gz == 0.f) continue;          // a vertex no face of this view differentiated
+    const float X = vw[v * 3], Y = vw[v * 3 + 1], Z = vw[v * 3 + 2];
+    float gxv, gyv, gzv;
+    dbw_project_backward(X, Y, Z, r, t, fx, fy, px, py, eps, gx, gy, gz, gxv, gyv, gzv);
+    dbw_camera_accumulate(X, Y, Z, gxv, gyv, gzv, acc, acc + 9);
+  }
+#pragma unroll
+  for (int k = 0; k < 12; ++k) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < 12; ++k) s_part[warp][k] = acc[k];
+  }
+  __syncthreads();
+  if (tid < 12) {
+    float s = 0.f;
+    for (int w = 0; w < DBW_CAM_NT / 32; ++w) s += s_part[w][tid];
+    float* dst = tid < 9 ? (g_R ? g_R + b * 9 + tid : nullptr) : (g_T ? g_T + b * 3 + (tid - 9) : nullptr);
+    if (dst && s != 0.f) atomicAdd(dst, s);
+  }
 }
 
 // order-preserving float <-> int map, so that atomicMin/atomicMax on ints order floats of either sign
@@ -1845,17 +1877,36 @@ extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const floa
                                           size_t workspace_bytes, const float* grad_rgba, const float* grad_scale, float* g_verts,
                                           float* g_faces_alpha, float* g_maps, void* bwd_scratch, size_t bwd_scratch_bytes,
                                           void* stream) {
-  if (validate(s)) return -1;
+  return dbw_render_backward_cameras(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, topk_ids, workspace,
+                                     workspace_bytes, grad_rgba, grad_scale, g_verts, g_faces_alpha, g_maps, nullptr, nullptr,
+                                     bwd_scratch, bwd_scratch_bytes, stream);
+}
+
+extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const float* verts, const int32_t* faces,
+                                           const float* faces_uvs, const int32_t* face_map, const float* maps,
+                                           const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                                           const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
+                                           const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
+                                           float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
+                                           void* stream) {
+  if (validate(s_in)) return -1;
   (void)topk_ids;          // kept in the signature for ABI continuity: the backward streams the workspace's fragment records
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || !workspace || !grad_rgba || !bwd_scratch)
     return fail("dbw_render_backward: null pointer argument");
-  if (!s->save_fragment_state) return fail("dbw_render_backward: the forward must run with save_fragment_state = 1");
+  if (!s_in->save_fragment_state) return fail("dbw_render_backward: the forward must run with save_fragment_state = 1");
+  const bool cams = g_R != nullptr || g_T != nullptr;
+  if (cams && s_in->verts_are_ndc) return fail("dbw_render_backward_cameras: no camera gradient when verts_are_ndc (R and T are not used)");
+  if (cams && (!R || !T)) return fail("dbw_render_backward_cameras: camera gradients need R and T");
+  // every face moves in the image when the camera moves: a call with camera gradients differentiates the static faces too
+  DbwRenderSettings s_local = *s_in;
+  if (cams) s_local.n_static_faces = 0;
+  const DbwRenderSettings* s = &s_local;
   Workspace w = carve(*s, (void*)workspace);
   BwdScratch g = carve_bwd(*s, bwd_scratch);
   if (workspace_bytes < w.total || bwd_scratch_bytes < g.total) return fail("dbw_render_backward: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s->n_views, V = s->n_verts, F = s->n_faces;
-  const bool need_geom = g_verts != nullptr;
+  const bool need_geom = g_verts != nullptr || cams;     // both are reductions of the per-view NDC vertex gradient
   CK(cudaMemsetAsync(bwd_scratch, 0, g.total, st));
   RasterParams P = make_params(*s, w, faces_alpha);
   if (s->maps_are_texels4) P.maps4 = (const float4*)maps;
@@ -1914,11 +1965,15 @@ extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const floa
     face_setup_backward_kernel<<<(B * F + 127) / 128, 128, 0, st>>>(verts_ndc, faces, B, V, F, s->z_clip, s->perspective_correct,
                                                                     g.g_tri, g.g_conv, g_ndc);
     LAUNCH_CK("face_setup_backward_kernel");
-    if (!s->verts_are_ndc) {
+    if (!s->verts_are_ndc && g_verts) {
       if (!R || !T) return fail("dbw_render_backward: R and T are required unless verts_are_ndc");
       project_verts_backward_kernel<<<(V * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, B, V,
                                                                      g.g_verts_ndc, g_verts);
       LAUNCH_CK("project_verts_backward_kernel");
+    }
+    if (cams) {
+      camera_grad_kernel<<<B, DBW_CAM_NT, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, V, g.g_verts_ndc, g_R, g_T);
+      LAUNCH_CK("camera_grad_kernel");
     }
   }
   return 0;

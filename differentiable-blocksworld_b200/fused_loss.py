@@ -100,7 +100,7 @@ class _SceneMSEFn(torch.autograd.Function):
         # every gradient buffer of both passes (and the kernels' scratch, which they expect zeroed... they zero it themselves)
         # comes out of ONE zero-filled arena: one fill launch per step instead of five
         wants = [('gm_b', blk_maps, need[3]), ('gm_e', env_maps, need[1]), ('gv_b', blk_verts, need[2]), ('gv_e', env_verts, need[0]),
-                 ('ga_b', fa, need[4] and fa is not None)]
+                 ('ga_b', fa, need[4] and fa is not None), ('g_R', R, need[5]), ('g_T', T, need[6])]
         total = sum((t.numel() + 3) // 4 * 4 for _, t, on in wants if on)
         arena = torch.zeros(total, device=dev, dtype=torch.float32)
         g, off = {}, 0
@@ -110,14 +110,22 @@ class _SceneMSEFn(torch.autograd.Function):
                 g[name] = arena[off:off + t.numel()].view_as(t)
                 off += (t.numel() + 3) // 4 * 4                      # float4 texel atlases stay 16-byte aligned
 
+        g_R, g_T = g['g_R'], g['g_T']          # both passes accumulate into them (include/dbw_render.h)
+
         def run(cfg, p, fmap, verts, maps, table, alpha, ws, grad, bwd_bytes, g_verts, g_maps, g_alpha):
-            if g_verts is None and g_maps is None and g_alpha is None:
+            if g_verts is None and g_maps is None and g_alpha is None and g_R is None and g_T is None:
                 return
             scratch = torch.empty(bwd_bytes, dtype=torch.uint8, device=dev)
-            _lib.check(L.dbw_render_backward_scaled(ctypes.byref(cfg), _c(verts), _c(p.faces), _c(p.faces_uvs), _c(fmap), _c(maps),
-                                                    _c(table), _c(R), _c(T), _c(alpha), None, _c(ws), ws.numel(), _c(grad),
-                                                    _c(gl), _c(g_verts), _c(g_alpha), _c(g_maps), _c(scratch), scratch.numel(),
-                                                    _stream()), 'dbw_render_backward_scaled')
+            if g_R is None and g_T is None:
+                _lib.check(L.dbw_render_backward_scaled(ctypes.byref(cfg), _c(verts), _c(p.faces), _c(p.faces_uvs), _c(fmap), _c(maps),
+                                                        _c(table), _c(R), _c(T), _c(alpha), None, _c(ws), ws.numel(), _c(grad),
+                                                        _c(gl), _c(g_verts), _c(g_alpha), _c(g_maps), _c(scratch), scratch.numel(),
+                                                        _stream()), 'dbw_render_backward_scaled')
+                return
+            _lib.check(L.dbw_render_backward_cameras(ctypes.byref(cfg), _c(verts), _c(p.faces), _c(p.faces_uvs), _c(fmap), _c(maps),
+                                                     _c(table), _c(R), _c(T), _c(alpha), None, _c(ws), ws.numel(), _c(grad),
+                                                     _c(gl), _c(g_verts), _c(g_alpha), _c(g_maps), _c(g_R), _c(g_T), _c(scratch),
+                                                     scratch.numel(), _stream()), 'dbw_render_backward_cameras')
 
         if OVERLAP_BACKWARD_PASSES:
             global _side_stream
@@ -133,7 +141,7 @@ class _SceneMSEFn(torch.autograd.Function):
             run(cfg_b, blk_pass, fmap_b, blk_verts, blk_maps, table_b, fa, ws_b, g_fg, bwd_b, g['gv_b'], g['gm_b'], g['ga_b'])
             run(cfg_e, env_pass, env_pass.face_map, env_verts, env_maps, table_e, None, ws_e, g_env, bwd_e, g['gv_e'], g['gm_e'], None)
         gv_e, gm_e, gv_b, gm_b, ga_b = g['gv_e'], g['gm_e'], g['gv_b'], g['gm_b'], g['ga_b']
-        return gv_e, gm_e, gv_b, gm_b, ga_b, None, None, None, None, None, None, None, None, None
+        return gv_e, gm_e, gv_b, gm_b, ga_b, g_R, g_T, None, None, None, None, None, None, None
 
 
 def scene_mse(env_verts, env_atlas, blk_verts, blk_atlas, blk_alpha, R, T, imgs, env_pass, blk_pass, blk_face_map,

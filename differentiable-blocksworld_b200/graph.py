@@ -6,9 +6,12 @@ more than the kernels themselves.  Requires the model's static-topology mode (db
 shape that depends on parameter values inside forward()."""
 import torch
 
+from .parallel import refuse_camera_gradients
+
 
 class GraphedStep:
     def __init__(self, view_parallel, example_inp, n_total_views, warmup=3, capture_all_reduce=None, generator=None):
+        refuse_camera_gradients(example_inp, 'GraphedStep')
         self.vp, self.model = view_parallel, view_parallel.model
         # The gradient all-reduce is captured INTO the graph when it is the peer-memory kernel (a plain launch).  An
         # ncclAllReduce is issued right after the replay instead: captured, it hung on 2 GPUs with this image's NCCL (round 1).
@@ -73,6 +76,7 @@ class GraphedStep:
     def run(self, inp=None, non_blocking=True, all_reduce=True):
         """inp: optional dict of (host or device) tensors for this step, copied into the static buffers.
         all_reduce=False skips the collective when it is issued after the replay (a captured one always runs)."""
+        refuse_camera_gradients(inp, 'GraphedStep')
         if inp is not None:
             for k, v in inp.items():
                 if k in self.static_inp:
@@ -100,6 +104,7 @@ class PipelinedGraphedStep:
     the losses of the step that consumed `host_inp`."""
 
     def __init__(self, view_parallel, example_inp, n_total_views, capture_all_reduce=None):
+        refuse_camera_gradients(example_inp, 'PipelinedGraphedStep')
         gen = torch.Generator(device=example_inp['imgs'].device)
         gen.manual_seed(view_parallel.seed)
         self.steps = [GraphedStep(view_parallel, example_inp, n_total_views, capture_all_reduce=capture_all_reduce, generator=gen)
@@ -121,6 +126,8 @@ class PipelinedGraphedStep:
     def run(self, host_inp, next_host_inp=None, all_reduce=True):
         """consume `host_inp` (staged now unless it was prefetched as the previous call's `next_host_inp`) and
         prefetch `next_host_inp` for the following call."""
+        refuse_camera_gradients(host_inp, 'PipelinedGraphedStep')
+        refuse_camera_gradients(next_host_inp, 'PipelinedGraphedStep')
         b = self.i % 2
         cur = torch.cuda.current_stream()
         if not self.primed:

@@ -28,6 +28,17 @@ def shard_views(n_views, world_size, rank):
     return slice(start, start + base + (1 if rank < extra else 0))
 
 
+def refuse_camera_gradients(inp, who):
+    """Camera poses that require grad are refused rather than silently left without a gradient: under view or row-band
+    sharding a rank holds only partial per-view sums of them, and a captured graph's static input buffers do not carry a
+    gradient back to the caller's tensors."""
+    for k in ('R', 'T'):
+        v = inp.get(k) if inp is not None else None
+        if torch.is_tensor(v) and v.requires_grad:
+            raise RuntimeError(f"{who}: inp['{k}'] requires grad, but camera-pose gradients are only computed by a plain "
+                               f"model(inp) step (not sharded, not graph-captured); detach the poses or call the model directly")
+
+
 ROW_BAND = 16          # rows per shardable band: the tallest raster tile (16 x 16, the K <= 4 forward), so tiles stay whole
 
 
@@ -287,6 +298,7 @@ class ViewParallel:
         """forward + backward over this rank's shard.  Returns (losses, reduced): reduced = the gradients are already the
         sum over ranks (the GradSumPoint ran inside the backward); otherwise a leaf all-reduce of the bucket is due.
         collective=False on a step that would reduce inside the backward leaves LOCAL gradients (timing breakdowns only)."""
+        refuse_camera_gradients(inp, 'ViewParallel')
         inside = self.reduces_inside_backward(inp)
         self.model.n_total_views = n_total_views
         self.model.grad_sum_point = self.sum_point if (inside and collective) else None
@@ -301,6 +313,7 @@ class ViewParallel:
 
     def forward_backward(self, inp, labels=None, already_sharded=False, n_total_views=None, all_reduce=True):
         """local forward -> backward -> ONE all-reduce (inside the backward or after it).  Returns the (local) loss dict."""
+        refuse_camera_gradients(inp, 'ViewParallel')
         if not already_sharded:
             inp, n_total_views = self.shard(inp)
         self._sync_rng(inp['imgs'].device)

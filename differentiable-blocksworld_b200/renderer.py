@@ -111,11 +111,26 @@ class _RenderFn(torch.autograd.Function):
             g_fa = torch.zeros_like(fa)
         g_maps = torch.zeros_like(maps) if need_m else None
         scratch = torch.empty(ctx.bwd_bytes, dtype=torch.uint8, device=verts.device)
-        _lib.check(L.dbw_render_backward(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
-                                         _c(map_table), _c(R), _c(T), _c(fa), None, _c(ws), ws.numel(), _c(g_out),
-                                         _c(g_verts), _c(g_fa), _c(g_maps), _c(scratch), scratch.numel(), _stream()),
-                   'dbw_render_backward')
-        return g_verts, g_maps, g_fa, None, None, None, None, None, None, None, None, None, None
+        need_R, need_T = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        if not (need_R or need_T):
+            _lib.check(L.dbw_render_backward(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
+                                             _c(map_table), _c(R), _c(T), _c(fa), None, _c(ws), ws.numel(), _c(g_out),
+                                             _c(g_verts), _c(g_fa), _c(g_maps), _c(scratch), scratch.numel(), _stream()),
+                       'dbw_render_backward')
+            return g_verts, g_maps, g_fa, None, None, None, None, None, None, None, None, None, None
+        if s.verts_are_ndc:
+            raise DbwError('R and T are not part of a render from NDC vertices (verts_are_ndc): they have no gradient')
+        # the camera gradients share one zero-fill; a call with camera gradients also differentiates the static faces
+        # (include/dbw_render.h), so g_verts then holds their vertices' rows too
+        cam = torch.zeros(R.shape[0] * 12, device=verts.device, dtype=torch.float32)
+        g_R, g_T = cam[:R.numel()].view_as(R), cam[R.numel():].view_as(T)
+        _lib.check(L.dbw_render_backward_cameras(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
+                                                 _c(map_table), _c(R), _c(T), _c(fa), None, _c(ws), ws.numel(), _c(g_out), None,
+                                                 _c(g_verts), _c(g_fa), _c(g_maps), _c(g_R if need_R else None),
+                                                 _c(g_T if need_T else None), _c(scratch), scratch.numel(), _stream()),
+                   'dbw_render_backward_cameras')
+        return (g_verts, g_maps, g_fa, g_R if need_R else None, g_T if need_T else None, None, None, None, None, None, None,
+                None, None)
 
 
 _TABLE_CACHE = {}

@@ -68,7 +68,8 @@ typedef struct DbwRenderSettings {
                                  n_faces / alpha_group entries per view: a DBW block is 80 faces with ONE opacity
                                  (src/model/dbw.py:219 repeat_interleave's it per face; that is alpha_group = 1)            */
   int32_t n_static_faces;     /* faces [0, n_static_faces) have constant vertices (the background sphere of the environment,
-                                 src/model/dbw.py:267-280): the backward skips their vertex gradient                        */
+                                 src/model/dbw.py:267-280): the backward skips their vertex gradient.  Ignored (0) by a
+                                 dbw_render_backward_cameras call that asks for camera gradients                            */
   const int32_t* view_rows;   /* DEVICE (B,2) int32 or NULL: [row_begin, row_end) of each view that this call renders / differentiates.
                                  Rows outside are left untouched in every output (and contribute nothing to a fused loss):
                                  a data-parallel step shards at (view, row band) granularity, so 49 views split evenly
@@ -200,6 +201,29 @@ int dbw_render_backward_scaled(const DbwRenderSettings* settings, const float* v
                                const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
                                const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
                                float* g_maps, void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
+
+/*
+ * dbw_render_backward_scaled plus the gradient of the camera poses (PyTorch3D keeps the camera transform inside autograd
+ * behind the reference's renderer, src/model/renderer.py:94, so a loss on the image differentiates R and T):
+ *   g_R (B,3,3), g_T (B,3)  accumulate (the caller zero-fills); either may be NULL.  Row-vector convention
+ *                           X_view = X_world @ R + T:  g_T[b] = sum_v g_view[b,v],  g_R[b][i][j] = sum_v X_world[v][i] g_view[b,v][j],
+ *                           g_view the NDC vertex gradient pulled back through the projection (|z| < proj_eps: no z term).
+ * With both NULL this IS dbw_render_backward_scaled.  With either set:
+ *  - n_static_faces is treated as 0: every face moves in the image when the camera does, so the static faces are
+ *    differentiated too (the background sphere of the environment pass), and g_verts, when not NULL, then also receives the
+ *    rows of the static faces' vertices;
+ *  - the per-view sums run in a fixed order (one CTA per view) and each element of g_R / g_T receives one atomic add per call;
+ *  - with view_rows, the result is the gradient of the rows this call owns: the calls over a partition of the rows sum to
+ *    the gradient of the whole image;
+ *  - verts_are_ndc is an error (R and T are not part of such a render).
+ */
+int dbw_render_backward_cameras(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
+                                const float* faces_uvs, const int32_t* face_map, const float* maps,
+                                const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                                const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
+                                const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
+                                float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
+                                void* stream);
 
 /*
  * Fused scene construction (src/model/dbw.py:267-352), so that a training step needs no eager tensor ops between the
