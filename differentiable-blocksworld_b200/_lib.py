@@ -62,6 +62,7 @@ class DbwMapDesc(ctypes.Structure):
 
 EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_forward_ex', 'dbw_render_backward',
            'dbw_render_forward_loss', 'dbw_render_backward_scaled', 'dbw_render_backward_cameras',
+           'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_composite_mse', 'dbw_composite_mse_backward', 'dbw_render_forward_host', 'dbw_host_arena_release', 'dbw_launch_count',
            'dbw_timing_enable', 'dbw_timing_read', 'dbw_timing_reset', 'dbw_scene_geometry_forward',
            'dbw_scene_geometry_backward', 'dbw_scene_geometry_forward_env', 'dbw_scene_geometry_backward_parts',
@@ -100,6 +101,9 @@ def lib():
         L.dbw_render_forward_loss.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, ctypes.POINTER(DbwLossEpilogue), vp]
         L.dbw_render_backward_scaled.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [sz] + [vp] * 6 + [sz, vp]
         L.dbw_render_backward_cameras.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [sz] + [vp] * 8 + [sz, vp]
+        L.dbw_render_forward_loss_grad.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz, ctypes.POINTER(DbwLossEpilogue),
+                                                                                               ctypes.c_int32, vp, sz, vp]
+        L.dbw_render_backward_deferred.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 7 + [sz, vp]
         L.dbw_composite_mse.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
         L.dbw_composite_mse_backward.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
         L.dbw_render_forward_host.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 6

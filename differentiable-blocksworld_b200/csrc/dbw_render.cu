@@ -131,7 +131,7 @@ static Workspace carve(const DbwRenderSettings& s, void* base) {
   w.nfrag = (unsigned char*)(p + off); off += s.save_fragment_state ? align_up(npx) : 0;
   w.total = off; return w;
 }
-struct BwdScratch { float* g_tri; float* g_conv; float* g_verts_ndc; float4* g_maps4; float4* g_cells; int* bary_flags; size_t total; };
+struct BwdScratch { float* g_tri; float* g_conv; float* g_verts_ndc; float4* g_maps4; float4* g_cells; int* bary_flags; float* g_alpha; size_t total; };
 static size_t bary_flag_count(const DbwRenderSettings& s);
 static BwdScratch carve_bwd(const DbwRenderSettings& s, void* base) {
   BwdScratch w; char* p = (char*)base; size_t off = 0;
@@ -143,6 +143,9 @@ static BwdScratch carve_bwd(const DbwRenderSettings& s, void* base) {
   // cell-map gradients: DBW_CELL_GRAD_COPIES copies of the whole map array (a CTA adds into one of them)
   w.g_cells = (float4*)(p + off);     off += s.maps_are_texels4 == 2 ? align_up((size_t)DBW_CELL_GRAD_COPIES * (s.n_map_floats / 3) * sizeof(float4)) : 0;
   w.bary_flags = (int*)(p + off);     off += align_up(bary_flag_count(s) * sizeof(int));
+  // unscaled opacity gradient of a loss-epilogue forward that differentiates itself (dbw_render_forward_loss_grad)
+  const size_t n_alpha = s.n_faces / (s.alpha_group > 0 ? s.alpha_group : 1);
+  w.g_alpha = (float*)(p + off);      off += align_up(B * n_alpha * sizeof(float));
   w.total = off; return w;
 }
 
@@ -175,17 +178,26 @@ __global__ void maps_to_float4_kernel(const float* __restrict__ maps, float4* __
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_texels; i += gridDim.x * blockDim.x)
     maps4[i] = make_float4(maps[3 * i], maps[3 * i + 1], maps[3 * i + 2], 0.f);
 }
-// g_maps += the sum of the DBW_CELL_GRAD_COPIES cell-gradient copies (maps_are_texels4 = 2)
-__global__ void fold_gcells_kernel(const float4* __restrict__ gc, float4* __restrict__ g_maps, int n) {
+// g_maps += the sum of the DBW_CELL_GRAD_COPIES cell-gradient copies (maps_are_texels4 = 2), times the device scalar *scale
+// (NULL = 1)
+__global__ void fold_gcells_kernel(const float4* __restrict__ gc, float4* __restrict__ g_maps, int n, const float* __restrict__ scale) {
+  const float s = scale ? __ldg(scale) : 1.f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    float4 a = g_maps[i];
+    float4 t = gc[i];
 #pragma unroll
-    for (int r = 0; r < DBW_CELL_GRAD_COPIES; ++r) {
+    for (int r = 1; r < DBW_CELL_GRAD_COPIES; ++r) {
       const float4 c = gc[(size_t)r * n + i];
-      a.x += c.x; a.y += c.y; a.z += c.z;
+      t.x += c.x; t.y += c.y; t.z += c.z;
     }
+    float4 a = g_maps[i];
+    a.x += s * t.x; a.y += s * t.y; a.z += s * t.z;
     g_maps[i] = a;
   }
+}
+// dst += *scale * src
+__global__ void scale_add_kernel(float* __restrict__ dst, const float* __restrict__ src, int n, const float* __restrict__ scale) {
+  const float s = __ldg(scale);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] += s * src[i];
 }
 __global__ void fold_gmaps_kernel(const float4* __restrict__ g4, float* __restrict__ g_maps, int n_texels) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_texels; i += gridDim.x * blockDim.x) {
@@ -450,7 +462,7 @@ struct RasterParams {
   unsigned char* nfrag;      // (B,H,W) number of records written per pixel
   const float* face_shade;   // (B,F,3) per-view per-face colour multiplier (flat shading) or NULL
   float* out_dists;          // (B,K,H,W) signed squared distances of the kept fragments (-1 = empty) or NULL
-  // backward only
+  // backward only (and the forward with ep_grad)
   const float* grad_rgba; float* g_tri; float* g_conv; float* g_faces_alpha; float4* g_maps4;
   float4* g_cells; int n_cells;   // cell-map gradient copies (DBW_CELL_GRAD_COPIES x n_cells) or NULL: cell taps go to g_maps4
   const float* grad_scale;   // device scalar multiplied into grad_rgba (the upstream gradient of a fused loss) or NULL
@@ -458,6 +470,9 @@ struct RasterParams {
   // fused compositing + MSE epilogue of the forward (DbwLossEpilogue); ep_target == NULL: plain render
   const float* ep_env; const float* ep_target; float* ep_g_env; float* ep_rec; float* ep_partials;
   float ep_inv_count; int ep_part_mask;
+  // the epilogue also differentiates the pass (dbw_render_forward_loss_grad): unscaled gradients into g_tri / g_cells /
+  // g_faces_alpha, which then point at the backward scratch
+  int ep_grad;
 };
 
 // Raster CTAs: the 8x4-pixel patches of a CTA's warps tile a 16 x (NT / 16) pixel tile.  The backward kernels and the
@@ -476,6 +491,7 @@ struct RasterParams {
 #ifndef DBW_AGG_MIN
 #define DBW_AGG_MIN 2         // groups of at most this many lanes use plain atomics instead of a warp reduction
 #endif
+#define DBW_ALPHA_SMEM_MAX 512      // opacity entries per view that a CTA may pre-accumulate in shared memory
 
 // opacity of one fragment from its signed squared distance (layered_rgb_blend, src/model/renderer.py:252-257)
 __device__ __forceinline__ float frag_alpha(float d, float sigma, int clip_inside) {
@@ -576,8 +592,14 @@ __device__ __forceinline__ int centre_out(int rank, int n) {
   return (rank & 1) ? c - ((rank + 1) >> 1) : c + (rank >> 1);
 }
 
+__device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4* lA, float* lV, int stride, const int4* s_desc,
+                                                  float* s_galpha, bool live, int n, f2 p, const float (&g)[4], int view,
+                                                  int lane, int warp);
+
 // One kernel for every K: the per-pixel list of the K nearest fragments lives in (dynamic) shared memory (dbw_fraglist.cuh).
-// EP: with the compositing + MSE loss epilogue (DbwLossEpilogue); a template flag so that plain renders carry none of it
+// EP: with the compositing + MSE loss epilogue (DbwLossEpilogue); a template flag so that plain renders carry none of it.
+// With P.ep_grad the epilogue then also runs the pass's detach_bary backward on the list still in shared memory
+// (epilogue_backward): no fragment record and no gradient image goes through HBM.
 template <int NT, bool EP>
 __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_MINB) raster_forward_kernel(const RasterParams P) {
   // faces a tile lists at once (more: chunked path)
@@ -592,6 +614,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   __shared__ int s_count;
   __shared__ __align__(8) uint64_t s_bar;      // mbarrier of the TMA record gather
   extern __shared__ float4 s_dyn[];            // fragment lists: K*NT float4 (pz, bits, sd, u), K*NT float (v); then the map table
+                                               // (and with ep_grad the opacity sums)
   uint32_t bar_phase = 0;
 
   constexpr int TILE_H = NT / 16;
@@ -615,6 +638,9 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   // the map table goes to shared memory too: this thread's entry is loaded now and stored just before the barrier that follows
   // the bin scan, so that nobody waits for it
   int4* const s_desc = reinterpret_cast<int4*>(reinterpret_cast<float*>(s_dyn + (size_t)P.K * NT) + (size_t)P.K * NT);
+  float* const s_galpha = reinterpret_cast<float*>(s_desc + P.M);
+  if (EP && P.ep_grad && P.faces_alpha && P.g_faces_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX)
+    for (int i = tid; i < P.n_alpha; i += NT) s_galpha[i] = 0.f;
   DbwMapDesc my_desc = {0, 0, 0, 0};
   if (tid < P.M) my_desc = P.map_table[tid];
   const int4 vbox = __ldg(reinterpret_cast<const int4*>(P.view_bbox) + view);      // in flight across the barrier
@@ -768,12 +794,13 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   }
 
   float ep_sq = 0.f;          // this pixel's squared error (fused loss epilogue)
+  float ep_g[4] = {0.f, 0.f, 0.f, 0.f};      // d loss / d (this render's RGBA) at the pixel (fused loss epilogue)
+  int n_saved = 0;            // layers blended: those in front of the first fully opaque one
   if (live) {
   // ---- shade + blend the sorted fragments front to back (layered_rgb_blend, Appendix B)
   float occ = 1.f, r = 0.f, g = 0.f, bl = 0.f;
   const size_t plane = (size_t)P.H * P.W;
   const size_t pix = (size_t)yi * P.W + xi;
-  int n_saved = 0;
   float ep_e[3] = {0.f, 0.f, 0.f}, ep_t[3] = {0.f, 0.f, 0.f};
   if (EP) {                     // the epilogue's environment / target pixels: in flight while the fragments are shaded
 #pragma unroll
@@ -790,6 +817,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     if (P.topk) P.topk[((size_t)view * K + k) * plane + pix] = slot;
     if (P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = d0;
     if (occ == 0.f) continue;     // behind a fully opaque fragment (fine phase: alpha = 1 inside a face): contributes exactly 0
+    n_saved = k + 1;
     const float v = lV[k * NT];
     const int face = slot >= P.F ? slot - P.F : slot;
     Texel4 tx;
@@ -804,7 +832,6 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
       const size_t fi = ((size_t)view * K + k) * plane + pix;
       P.frag[fi] = make_float4(e.y, e.w, v, d0);
       P.frag_rgb[fi] = make_float4(tx.color.x, tx.color.y, tx.color.z, 0.f);
-      n_saved = k + 1;
     }
     const float w = occ * a;
     r += w * tx.color.x; g += w * tx.color.y; bl += w * tx.color.z;
@@ -822,7 +849,8 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     o[0] = fc[0]; o[plane] = fc[1]; o[2 * plane] = fc[2]; o[3 * plane] = m;
   } else {
     // fused epilogue (same arithmetic as composite_mse_kernel): composite over the environment render, squared error
-    // against the target, and the gradients of the MSE w.r.t. both layers -- out_rgba receives d loss / d (this render)
+    // against the target, and the gradients of the MSE w.r.t. both layers -- out_rgba (when not NULL) receives
+    // d loss / d (this render)
     float* ge = P.ep_g_env + (size_t)view * 4 * plane + pix;
     float gm = 0.f;
 #pragma unroll
@@ -833,14 +861,16 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
       ep_sq += diff * diff;
       if (P.ep_rec) P.ep_rec[(size_t)view * 3 * plane + (size_t)c * plane + pix] = rc;
       const float gr = 2.f * diff * P.ep_inv_count;
-      o[(size_t)c * plane] = gr * m;
+      ep_g[c] = gr * m;
       ge[(size_t)c * plane] = gr * (1.f - m);
       gm += gr * (fc[c] - ec);
     }
-    o[3 * plane] = gm;
+    ep_g[3] = gm;
+    if (P.out_rgba) { o[0] = ep_g[0]; o[plane] = ep_g[1]; o[2 * plane] = ep_g[2]; o[3 * plane] = gm; }
     ge[3 * plane] = 0.f;
   }
   }   // live
+  if (EP && P.ep_grad) epilogue_backward(P, lA, lV, NT, s_desc, s_galpha, live, n_saved, p, ep_g, view, lane, warp);
   if (EP) {
     // one atomic per warp into a strip of partial sums (the caller adds them up): no single hot address
 #pragma unroll
@@ -848,6 +878,13 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     if (lane == 0 && ep_sq != 0.f) {
       const unsigned cta = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;      // any spread over the strip will do
       atomicAdd(&P.ep_partials[(cta * (NT / 32) + warp) & P.ep_part_mask], ep_sq * P.ep_inv_count);
+    }
+  }
+  if (EP && P.ep_grad && P.faces_alpha && P.g_faces_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX) {
+    __syncthreads();                 // one global atomic per (CTA, opacity entry), as in raster_backward_kernel
+    for (int i = tid; i < P.n_alpha; i += NT) {
+      const float v = s_galpha[i];
+      if (v != 0.f) atomicAdd(&P.g_faces_alpha[(size_t)view * P.alpha_stride + i], v);
     }
   }
 }
@@ -1210,8 +1247,9 @@ __device__ __forceinline__ void warp_agg_add1(float* __restrict__ dst, int key, 
 }
 
 // Distance-path vertex gradient of one layer, keyed by (triangle slot, closest edge): 4 values = (x, y) of the edge's two
-// vertices.  4-wide spread reduction (5 shuffles): total i lands in lane 8 i and goes to float off[i] of the slot's 9.
+// vertices.  Vertex pair of the edge: 0 = (v0, v1), 1 = (v0, v2), 2 = (v1, v2); vertex j's (x, y) live at floats 3j, 3j+1.
 __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int key, const float (&v)[4], int lane) {
+#ifdef DBW_AGG_REDUX
   unsigned todo = __ballot_sync(0xffffffffu, key >= 0);
   while (todo) {
     const int leader = __ffs(todo) - 1;
@@ -1219,10 +1257,8 @@ __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int
     const bool mine = (key == lk);
     const unsigned grp = __ballot_sync(0xffffffffu, mine);
     const int edge = lk & 3;
-    // vertex pair of the edge: 0 = (v0, v1), 1 = (v0, v2), 2 = (v1, v2); vertex j's (x, y) live at floats 3j, 3j+1
     const int ia = edge == 2 ? 3 : 0, ib = edge == 0 ? 3 : 6;
     float* d = g_tri + (size_t)(lk >> 2) * 9;
-#ifdef DBW_AGG_REDUX
     if (mine) {
       float r[4];
       group_sum_redux<4>(grp, v, r);
@@ -1234,25 +1270,23 @@ __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int
       }
     }
     todo &= ~grp;
-    continue;
-#endif
-    if (__popc(grp) <= DBW_AGG_MIN) {
-      if (mine) {
-        if (v[0] != 0.f) atomicAdd(d + ia, v[0]);
-        if (v[1] != 0.f) atomicAdd(d + ia + 1, v[1]);
-        if (v[2] != 0.f) atomicAdd(d + ib, v[2]);
-        if (v[3] != 0.f) atomicAdd(d + ib + 1, v[3]);
-      }
-    } else {
-      float x[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) x[i] = mine ? v[i] : 0.f;
-      const float r = warp_sum_spread<4>(x, lane);
-      const int idx = lane >> 3;
-      if ((lane & 7) == 0 && r != 0.f) atomicAdd(d + (idx < 2 ? ia + idx : ib + idx - 2), r);
-    }
-    todo &= ~grp;
   }
+#else
+  // A patch's halo fragments of one layer lie along many edges, mostly one or two lanes per (slot, edge): every lane adds
+  // its four values with plain atomics, all in the same pass.  Finding the groups first and reducing them one after the
+  // other (a ballot, a shuffle and a ballot per group before any atomic) cost more than the atomics it saved: on an H100
+  // (700 W) at dtu, 2.05 ms for the fused blocks kernel with groups of more than 2 lanes reduced, 2.01 ms with more than
+  // 4, 1.88 ms with none
+  if (key >= 0) {
+    const int edge = key & 3;
+    const int ia = edge == 2 ? 3 : 0, ib = edge == 0 ? 3 : 6;
+    float* d = g_tri + (size_t)(key >> 2) * 9;
+    if (v[0] != 0.f) atomicAdd(d + ia, v[0]);
+    if (v[1] != 0.f) atomicAdd(d + ia + 1, v[1]);
+    if (v[2] != 0.f) atomicAdd(d + ib, v[2]);
+    if (v[3] != 0.f) atomicAdd(d + ib + 1, v[3]);
+  }
+#endif
 }
 
 // Barycentric-path gradient of one fragment with colour gradient (gcx, gcy, gcz): colour -> (ix, iy) -> (u, v) ->
@@ -1291,13 +1325,123 @@ __device__ __forceinline__ bool bary_frag_backward(const RasterParams& P, size_t
   return clipped;
 }
 
+// Pass 2 of a pixel's backward: its n fragments back to front with the division-free suffix recurrence of SURVEY Appendix B,
+// on what pass 1 left in shared memory -- q = (alpha, cdot, e, occ) and the record bits of layer k at s_q[k * stride] and
+// s_bits[k * stride] -- handing d/d(alpha_k) to the opacity sums and, for halo fragments, to the two vertices of the closest
+// edge.  (gr, gg, gb, ga): d loss / d this pass's RGBA at the pixel.  Warp-uniform: every lane makes n_warp (the warp's
+// largest n) trips, so that the aggregation helpers run converged.
+__device__ __forceinline__ void suffix_backward(const RasterParams& P, const float4* s_q, const int* s_bits, int stride, int n,
+                                                int n_warp, f2 p, float gr, float gg, float gb, float ga, int view,
+                                                size_t slot_base, bool want_alpha, bool alpha_in_smem, float* s_galpha,
+                                                bool want_dist, int lane) {
+  if (!want_alpha && !want_dist) return;
+  float Tacc = P.bg0 * gr + P.bg1 * gg + P.bg2 * gb - ga;
+  // the edge geometry of a halo fragment (2 vertices + 1 / |edge|^2, from the face record) is loaded one layer ahead
+  struct EdgeGeom { float4 r0; float2 r1; float4 r3; };
+  auto load_edge = [&](int kk, EdgeGeom& g) {
+    g.r0 = make_float4(0.f, 0.f, 0.f, 0.f); g.r1 = make_float2(0.f, 0.f); g.r3 = g.r0;
+    if (!want_dist || kk < 0 || kk >= n) return;
+    const int bits = s_bits[kk * stride];
+    if (P.clip_inside && !(bits & DBW_FRAG_OUTSIDE_BIT)) return;          // clamp(d, 0): no distance gradient inside the face
+    const size_t gsl = slot_base + (bits & DBW_FRAG_SLOT_MASK);
+    g.r0 = __ldg(&P.rec[gsl * 4]); g.r3 = __ldg(&P.rec[gsl * 4 + 3]);
+    g.r1 = __ldg(reinterpret_cast<const float2*>(&P.rec[gsl * 4 + 1]));
+  };
+  EdgeGeom eg_next;
+  load_edge(n_warp - 1, eg_next);
+  for (int k = n_warp - 1; k >= 0; --k) {
+    const EdgeGeom eg = eg_next;
+    load_edge(k - 1, eg_next);
+    int akey = -1, vkey = -1;
+    float aval = 0.f;
+    float gv4[4] = {0.f, 0.f, 0.f, 0.f};        // (x, y) of the two vertices of the closest edge
+    if (k < n) {
+      const float4 q = s_q[k * stride];        // (alpha, cdot, e, occ)
+      const float g_alpha = q.w * (q.y - Tacc);
+      Tacc = q.x * q.y + (1.f - q.x) * Tacc;
+      if (g_alpha != 0.f) {
+        const int bits = s_bits[k * stride], slot = bits & DBW_FRAG_SLOT_MASK;
+        const int face = slot >= P.F ? slot - P.F : slot;
+        if (want_alpha) { akey = alpha_index(P, alpha_in_smem ? 0 : view, face); aval = g_alpha * q.z; }
+        if (want_dist) {
+          // gradient w.r.t. the SIGNED squared distance: alpha = e(d) * fa, so fa * e = alpha
+          const bool inside = !(bits & DBW_FRAG_OUTSIDE_BIT);
+          float g_sd = 0.f;
+          if (P.clip_inside) { if (!inside) g_sd = g_alpha * (-q.x / P.sigma); }          // clamp(d, 0): flat inside the face
+          else g_sd = g_alpha * (-q.x * (1.f - q.z) / P.sigma);
+          const float g_dist = inside ? -g_sd : g_sd;    // signed = inside ? -dist : dist
+          if (g_dist != 0.f) {
+            const int edge = (bits >> DBW_FRAG_EDGE_SHIFT) & 3;
+            const f2 v0 = {eg.r0.x, eg.r0.y}, v1 = {eg.r0.z, eg.r0.w}, v2 = {eg.r1.x, eg.r1.y};
+            const f2 ea = edge == 2 ? v1 : v0, eb = edge == 0 ? v1 : v2;
+            const float il = edge == 0 ? eg.r3.y : (edge == 1 ? eg.r3.z : eg.r3.w);
+            f2 g_a = {0.f, 0.f}, g_b = {0.f, 0.f};
+            seg_backward(p, ea, eb, il, g_dist, g_a, g_b);
+            vkey = slot * 4 + edge;
+            gv4[0] = g_a.x; gv4[1] = g_a.y; gv4[2] = g_b.x; gv4[3] = g_b.y;
+          }
+        }
+      }
+    }
+    if (want_alpha && __ballot_sync(0xffffffffu, akey >= 0)) warp_agg_add1(alpha_in_smem ? s_galpha : P.g_faces_alpha, akey, aval, lane);
+    if (want_dist && __ballot_sync(0xffffffffu, vkey >= 0)) warp_agg_add_edge(P.g_tri + slot_base * 9, vkey, gv4, lane);
+  }
+}
+
+// The loss epilogue's own backward (raster_forward_kernel<NT, true> with P.ep_grad): the detach_bary backward of the pixel,
+// run right after the epilogue formed g = d loss / d RGBA, unscaled (dbw_render_backward_deferred applies the upstream
+// gradient when it folds the scratch).  The pixel's sorted fragment list is still in shared memory -- lA (pz, bits, signed
+// dist, u) and lV (v), `stride` apart -- so pass 1 re-fetches each layer's texels (L1/L2-resident), scatters the texture
+// gradient into the CTA's cell-gradient copy and overwrites the entry, whose depth and UV are dead by then, with what pass 2
+// needs: (alpha, cdot, e, occ) in lA and the bits in lV.  Pass 2 is suffix_backward.  n: the layers the shading loop
+// blended.  Called by every lane of the warp (lanes that are not `live` take part with empty keys).
+__device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4* lA, float* lV, int stride, const int4* s_desc,
+                                                  float* s_galpha, bool live, int n, f2 p, const float (&g)[4], int view,
+                                                  int lane, int warp) {
+  const float gr = g[0], gg = g[1], gb = g[2], ga = g[3];
+  const bool any_grad = live && ((gr != 0.f) || (gg != 0.f) || (gb != 0.f) || (ga != 0.f));
+  const int n_px = any_grad ? n : 0;
+  int n_warp = n_px;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n_warp = max(n_warp, __shfl_xor_sync(0xffffffffu, n_warp, o));
+  float occ = 1.f;
+  for (int k = 0; k < n_warp; ++k) {
+    int tkey = -1, t01 = -1, t10 = -1, t11 = -1;
+    bool tcells = false;
+    float tg[3] = {0.f, 0.f, 0.f}, tw[4] = {0.f, 0.f, 0.f, 0.f};      // texture gradient = tg x tw (colour x tap weights)
+    if (k < n_px) {
+      const float4 e = lA[k * stride];
+      const int bits = __float_as_int(e.y), slot = bits & DBW_FRAG_SLOT_MASK;
+      const int face = slot >= P.F ? slot - P.F : slot;
+      const int4 desc = s_desc[(unsigned)bits >> DBW_FRAG_MAP_SHIFT];
+      Texel4 tx;
+      fetch_color(P, e.w, lV[k * stride], desc, tx);
+      const float ea = frag_alpha(e.z, P.sigma, P.clip_inside);
+      const float a = P.faces_alpha ? ea * __ldg(&P.faces_alpha[alpha_index(P, view, face)]) : ea;
+      const float cdot = tx.color.x * gr + tx.color.y * gg + tx.color.z * gb;
+      lA[k * stride] = make_float4(a, cdot, ea, occ);
+      lV[k * stride] = __int_as_float(bits);
+      const float w = occ * a;                 // d RGB / d colour_k
+      if (w != 0.f && P.g_maps4) {
+        tkey = tx.tap.i00; t01 = tx.tap.i01; t10 = tx.tap.i10; t11 = tx.tap.i11; tcells = desc.w != 0;
+        tg[0] = w * gr; tg[1] = w * gg; tg[2] = w * gb;
+        tw[0] = tx.tap.w00; tw[1] = tx.tap.w01; tw[2] = tx.tap.w10; tw[3] = tx.tap.w11;
+      }
+      occ *= (1.f - a);
+    }
+    if (P.g_maps4) warp_tex_scatter<false>(P, tkey, t01, t10, t11, tcells, tg, tw, lane, warp);
+  }
+  const bool want_alpha = P.faces_alpha != nullptr && P.g_faces_alpha != nullptr;
+  suffix_backward(P, lA, reinterpret_cast<const int*>(lV), stride, n_px, n_warp, p, gr, gg, gb, ga, view, (size_t)view * 2 * P.F,
+                  want_alpha, want_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX, s_galpha, P.sigma > 0.f && P.g_tri != nullptr, lane);
+}
+
 // One thread per pixel.  Pass 1 streams the pixel's saved fragment records {slot, u, v, signed distance} front to back,
 // re-fetches the four texels of each (the float4 atlas is L2-resident), scatters the texture gradient and -- unless
 // detach_bary -- re-derives the geometry for the barycentric-path vertex gradient (skipped for faces whose vertices are
 // constants; a single-layer pass leaves it to raster_bary_backward_kernel); pass 2 walks back to front with the division-free suffix recurrence of SURVEY Appendix B for d/d(alpha_k)
 // -> opacity and distance -> vertex gradients.  Loops are warp-uniform (trip count = warp max) so that the aggregation
 // helpers run converged.
-#define DBW_ALPHA_SMEM_MAX 512      // opacity entries per view that a CTA may pre-accumulate in shared memory
 // 16 x 8 tiles a backward CTA walks (each warp its own patch of every tile, no barrier between, the next patch's first-level
 // loads in flight).  A single-layer pass is a chain of DRAM latencies per pixel and gains from 8 tiles (on an H100 SXM,
 // 4 tiles: 0.51 ms instead of 0.50 ms for the dtu environment backward); the K = 10 blocks pass walks one (more tiles
@@ -1432,60 +1576,9 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
     }
   }
 
-  // pass 2: suffix recurrence on the stored per-fragment scalars -- no division (alpha may be exactly 1)
-  float Tacc = P.bg0 * gr + P.bg1 * gg + P.bg2 * gb - ga;
-  if (want_alpha || want_dist) {
-    // the edge geometry of a halo fragment (2 vertices + 1 / |edge|^2, from the face record) is loaded one layer ahead
-    struct EdgeGeom { float4 r0; float2 r1; float4 r3; };
-    auto load_edge = [&](int kk, EdgeGeom& g) {
-      g.r0 = make_float4(0.f, 0.f, 0.f, 0.f); g.r1 = make_float2(0.f, 0.f); g.r3 = g.r0;
-      if (!want_dist || kk < 0 || kk >= n) return;
-      const int bits = s_bits[kk * DBW_BWD_NT];
-      if (P.clip_inside && !(bits & DBW_FRAG_OUTSIDE_BIT)) return;          // clamp(d, 0): no distance gradient inside the face
-      const size_t gsl = slot_base + (bits & DBW_FRAG_SLOT_MASK);
-      g.r0 = __ldg(&P.rec[gsl * 4]); g.r3 = __ldg(&P.rec[gsl * 4 + 3]);
-      g.r1 = __ldg(reinterpret_cast<const float2*>(&P.rec[gsl * 4 + 1]));
-    };
-    EdgeGeom eg_next;
-    load_edge(n_warp - 1, eg_next);
-    for (int k = n_warp - 1; k >= 0; --k) {
-      const EdgeGeom eg = eg_next;
-      load_edge(k - 1, eg_next);
-      int akey = -1, vkey = -1;
-      float aval = 0.f;
-      float gv4[4] = {0.f, 0.f, 0.f, 0.f};        // (x, y) of the two vertices of the closest edge
-      if (k < n) {
-        const float4 q = s_q[k * DBW_BWD_NT];      // (alpha, cdot, e, occ)
-        const float g_alpha = q.w * (q.y - Tacc);
-        Tacc = q.x * q.y + (1.f - q.x) * Tacc;
-        if (g_alpha != 0.f) {
-          const int bits = s_bits[k * DBW_BWD_NT], slot = bits & DBW_FRAG_SLOT_MASK;
-          const int face = slot >= P.F ? slot - P.F : slot;
-          if (want_alpha) { akey = alpha_index(P, alpha_in_smem ? 0 : view, face); aval = g_alpha * q.z; }
-          if (want_dist) {
-            // gradient w.r.t. the SIGNED squared distance: alpha = e(d) * fa, so fa * e = alpha
-            const bool inside = !(bits & DBW_FRAG_OUTSIDE_BIT);
-            float g_sd = 0.f;
-            if (P.clip_inside) { if (!inside) g_sd = g_alpha * (-q.x / P.sigma); }          // clamp(d, 0): flat inside the face
-            else g_sd = g_alpha * (-q.x * (1.f - q.z) / P.sigma);
-            const float g_dist = inside ? -g_sd : g_sd;    // signed = inside ? -dist : dist
-            if (g_dist != 0.f) {
-              const int edge = (bits >> DBW_FRAG_EDGE_SHIFT) & 3;
-              const f2 v0 = {eg.r0.x, eg.r0.y}, v1 = {eg.r0.z, eg.r0.w}, v2 = {eg.r1.x, eg.r1.y};
-              const f2 ea = edge == 2 ? v1 : v0, eb = edge == 0 ? v1 : v2;
-              const float il = edge == 0 ? eg.r3.y : (edge == 1 ? eg.r3.z : eg.r3.w);
-              f2 g_a = {0.f, 0.f}, g_b = {0.f, 0.f};
-              seg_backward(p, ea, eb, il, g_dist, g_a, g_b);
-              vkey = slot * 4 + edge;
-              gv4[0] = g_a.x; gv4[1] = g_a.y; gv4[2] = g_b.x; gv4[3] = g_b.y;
-            }
-          }
-        }
-      }
-      if (want_alpha && __ballot_sync(0xffffffffu, akey >= 0)) warp_agg_add1(alpha_in_smem ? s_galpha : P.g_faces_alpha, akey, aval, lane);
-      if (want_dist && __ballot_sync(0xffffffffu, vkey >= 0)) warp_agg_add_edge(P.g_tri + slot_base * 9, vkey, gv4, lane);
-    }
-  }
+  // pass 2: suffix recurrence on the stored per-fragment scalars
+  suffix_backward(P, s_q, s_bits, DBW_BWD_NT, n, n_warp, p, gr, gg, gb, ga, view, slot_base, want_alpha, alpha_in_smem, s_galpha,
+                  want_dist, lane);
   }   // tiles of the strip
   if (alpha_in_smem) {               // one global atomic per (CTA, opacity entry) instead of one per (warp, layer, entry)
     __syncthreads();
@@ -1576,9 +1669,10 @@ __device__ __forceinline__ void lerp_clip_backward(const float* p1, const float*
 
 __global__ void face_setup_backward_kernel(const float* __restrict__ verts_ndc, const int* __restrict__ faces, int B, int V, int F,
                                            float z_clip, int persp, const float* __restrict__ g_tri, const float* __restrict__ g_conv,
-                                           float* __restrict__ g_verts_ndc) {
+                                           const float* __restrict__ scale, float* __restrict__ g_verts_ndc) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * F) return;
+  const float sc = scale ? __ldg(scale) : 1.f;       // g_tri and g_conv are multiplied by *scale (NULL = 1)
   const int b = i / F, f = i - b * F;
   const size_t s0 = (size_t)b * 2 * F + f, s1 = s0 + F;
   float a[3][3]; int vid[3];
@@ -1635,9 +1729,9 @@ __global__ void face_setup_backward_kernel(const float* __restrict__ verts_ndc, 
 #pragma unroll
   for (int j = 0; j < 3; ++j) {
     float* g = g_verts_ndc + ((size_t)b * V + vid[j]) * 3;
-    if (ga[j][0] != 0.f) atomicAdd(g, ga[j][0]);
-    if (ga[j][1] != 0.f) atomicAdd(g + 1, ga[j][1]);
-    if (ga[j][2] != 0.f) atomicAdd(g + 2, ga[j][2]);
+    if (ga[j][0] != 0.f) atomicAdd(g, sc * ga[j][0]);
+    if (ga[j][1] != 0.f) atomicAdd(g + 1, sc * ga[j][1]);
+    if (ga[j][2] != 0.f) atomicAdd(g + 2, sc * ga[j][2]);
   }
 }
 
@@ -1748,7 +1842,7 @@ static size_t frag_smem_bytes(int K, int NT, int M, int n_alpha = 0) {
 template <int NT>
 static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st) {
   const dim3 grid(P.B, (P.W + TILE_W - 1) / TILE_W, (P.H + NT / 16 - 1) / (NT / 16));       // see centre_out()
-  const size_t smem = frag_smem_bytes(P.K, NT, P.M);
+  const size_t smem = frag_smem_bytes(P.K, NT, P.M, P.ep_grad && P.faces_alpha && P.g_faces_alpha ? P.n_alpha : 0);
   auto go = [&](auto kern) -> cudaError_t {
     if (smem > 40 * 1024) { cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); if (e != cudaSuccess) return e; }
     kern<<<grid, NT, smem, st>>>(P);
@@ -1765,11 +1859,13 @@ extern "C" int dbw_render_forward(const DbwRenderSettings* s, const float* verts
                                workspace, workspace_bytes, nullptr, nullptr, stream);
 }
 
+// the backward scratch and the gradients a loss-epilogue forward computes itself (dbw_render_forward_loss_grad)
+struct EpilogueGrad { void* scratch; size_t scratch_bytes; int32_t mask; };
 static int render_forward_impl(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream);
+                               void* stream, const EpilogueGrad* eg = nullptr);
 
 extern "C" int dbw_render_forward_ex(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                      const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
@@ -1791,13 +1887,33 @@ extern "C" int dbw_render_forward_loss(const DbwRenderSettings* s, const float* 
                              workspace, workspace_bytes, nullptr, nullptr, ep, stream);
 }
 
+extern "C" int dbw_render_forward_loss_grad(const DbwRenderSettings* s, const float* verts, const int32_t* faces,
+                                            const float* faces_uvs, const int32_t* face_map, const float* maps,
+                                            const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                                            void* workspace, size_t workspace_bytes, const DbwLossEpilogue* ep, int32_t grad_mask,
+                                            void* bwd_scratch, size_t bwd_scratch_bytes, void* stream) {
+  if (!ep) return fail("dbw_render_forward_loss_grad: null epilogue");
+  if (!ep->env_rgba || !ep->target || !ep->g_env || !ep->loss_partials)
+    return fail("dbw_render_forward_loss_grad: env_rgba, target, g_env and loss_partials are required");
+  if (ep->n_partials < 1 || (ep->n_partials & (ep->n_partials - 1))) return fail("dbw_render_forward_loss_grad: n_partials must be a power of two");
+  if (validate(s)) return -1;
+  if (!s->detach_bary) return fail("dbw_render_forward_loss_grad: the pass must be detach_bary");
+  if (s->maps_are_texels4 != 2) return fail("dbw_render_forward_loss_grad: the maps must be float4 cell maps (maps_are_texels4 = 2)");
+  if (grad_mask & ~(DBW_GRAD_VERTS | DBW_GRAD_MAPS | DBW_GRAD_ALPHA)) return fail("dbw_render_forward_loss_grad: unknown grad_mask bits");
+  if (s->save_fragment_state) return fail("dbw_render_forward_loss_grad: no fragment records are written (save_fragment_state must be 0)");
+  if (!bwd_scratch) return fail("dbw_render_forward_loss_grad: null backward scratch");
+  const EpilogueGrad eg = {bwd_scratch, bwd_scratch_bytes, grad_mask};
+  return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, nullptr, nullptr,
+                             workspace, workspace_bytes, nullptr, nullptr, ep, stream, &eg);
+}
+
 static int render_forward_impl(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream) {
+                               void* stream, const EpilogueGrad* eg) {
   if (validate(s)) return -1;
-  if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || !out_rgba || !workspace)
+  if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || (!out_rgba && !eg) || !workspace)
     return fail("dbw_render_forward: null pointer argument");
   if (!s->verts_are_ndc && (!R || !T)) return fail("dbw_render_forward: R and T are required unless verts_are_ndc");
   Workspace w = carve(*s, workspace);
@@ -1836,6 +1952,16 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
     CK(cudaMemsetAsync(ep->loss_partials, 0, (size_t)ep->n_partials * sizeof(float), st));
     P.ep_env = ep->env_rgba; P.ep_target = ep->target; P.ep_g_env = ep->g_env; P.ep_rec = ep->rec;
     P.ep_partials = ep->loss_partials; P.ep_inv_count = ep->inv_count; P.ep_part_mask = ep->n_partials - 1;
+  }
+  if (eg) {           // the scratch dbw_render_backward_deferred folds: zero-filled here, accumulated by the forward kernel
+    const BwdScratch g = carve_bwd(*s, eg->scratch);
+    if (eg->scratch_bytes < g.total) return fail("dbw_render_forward_loss_grad: backward scratch too small (see dbw_workspace_bytes)");
+    CK(cudaMemsetAsync(eg->scratch, 0, g.total, st));
+    P.ep_grad = 1;
+    if (eg->mask & DBW_GRAD_VERTS) { P.g_tri = g.g_tri; P.g_conv = g.g_conv; }
+    // cell_grad_copy picks the CTA's copy of g_cells; g_maps4 only says that a texture gradient is wanted
+    if (eg->mask & DBW_GRAD_MAPS) { P.g_cells = g.g_cells; P.n_cells = s->n_map_floats / 3; P.g_maps4 = g.g_cells; }
+    if ((eg->mask & DBW_GRAD_ALPHA) && faces_alpha) P.g_faces_alpha = g.g_alpha;
   }
   const int K = s->faces_per_pixel;
   {
@@ -1949,7 +2075,7 @@ extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const 
   if (P.g_cells) {
     const int blocks = stride_grid(n_entries, 8);
     if (blocks < 0) return fail("fold_gcells_kernel: SM count", cudaGetLastError());
-    fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries);
+    fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries, nullptr);
     LAUNCH_CK("fold_gcells_kernel");
   }
   if (g_maps && !s->maps_are_texels4) {
@@ -1963,10 +2089,59 @@ extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const 
     const float* verts_ndc = s->verts_are_ndc ? verts : w.verts_ndc;
     float* g_ndc = s->verts_are_ndc ? g_verts : g.g_verts_ndc;
     face_setup_backward_kernel<<<(B * F + 127) / 128, 128, 0, st>>>(verts_ndc, faces, B, V, F, s->z_clip, s->perspective_correct,
-                                                                    g.g_tri, g.g_conv, g_ndc);
+                                                                    g.g_tri, g.g_conv, nullptr, g_ndc);
     LAUNCH_CK("face_setup_backward_kernel");
     if (!s->verts_are_ndc && g_verts) {
       if (!R || !T) return fail("dbw_render_backward: R and T are required unless verts_are_ndc");
+      project_verts_backward_kernel<<<(V * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, B, V,
+                                                                     g.g_verts_ndc, g_verts);
+      LAUNCH_CK("project_verts_backward_kernel");
+    }
+    if (cams) {
+      camera_grad_kernel<<<B, DBW_CAM_NT, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, V, g.g_verts_ndc, g_R, g_T);
+      LAUNCH_CK("camera_grad_kernel");
+    }
+  }
+  return 0;
+}
+
+extern "C" int dbw_render_backward_deferred(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* R,
+                                            const float* T, const void* workspace, size_t workspace_bytes, const float* grad_scale,
+                                            float* g_verts, float* g_faces_alpha, float* g_maps, float* g_R, float* g_T,
+                                            void* bwd_scratch, size_t bwd_scratch_bytes, void* stream) {
+  if (validate(s)) return -1;
+  if (!verts || !faces || !workspace || !grad_scale || !bwd_scratch) return fail("dbw_render_backward_deferred: null pointer argument");
+  if (s->maps_are_texels4 != 2) return fail("dbw_render_backward_deferred: the maps must be float4 cell maps (maps_are_texels4 = 2)");
+  const bool cams = g_R != nullptr || g_T != nullptr;
+  if (cams && s->verts_are_ndc) return fail("dbw_render_backward_deferred: no camera gradient when verts_are_ndc (R and T are not used)");
+  if ((cams || (g_verts && !s->verts_are_ndc)) && (!R || !T)) return fail("dbw_render_backward_deferred: R and T are required");
+  const Workspace w = carve(*s, (void*)workspace);
+  const BwdScratch g = carve_bwd(*s, bwd_scratch);
+  if (workspace_bytes < w.total || bwd_scratch_bytes < g.total) return fail("dbw_render_backward_deferred: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s->n_views, V = s->n_verts, F = s->n_faces;
+  // the differentiation itself ran inside raster_forward_kernel<NT, true>: this is the blocks backward a caller times
+  ScopedTimer timer(1, s->faces_per_pixel, st);
+  if (g_maps) {
+    const int n_entries = s->n_map_floats / 3;
+    const int blocks = stride_grid(n_entries, 8);
+    if (blocks < 0) return fail("fold_gcells_kernel: SM count", cudaGetLastError());
+    fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries, grad_scale);
+    LAUNCH_CK("fold_gcells_kernel");
+  }
+  if (g_faces_alpha) {
+    const int n_alpha = s->n_faces / (s->alpha_group > 0 ? s->alpha_group : 1);
+    const int n = s->alpha_view_stride ? B * n_alpha : n_alpha;
+    scale_add_kernel<<<(n + 255) / 256, 256, 0, st>>>(g_faces_alpha, g.g_alpha, n, grad_scale);
+    LAUNCH_CK("scale_add_kernel");
+  }
+  if (g_verts || cams) {
+    const float* verts_ndc = s->verts_are_ndc ? verts : w.verts_ndc;
+    float* g_ndc = s->verts_are_ndc ? g_verts : g.g_verts_ndc;
+    face_setup_backward_kernel<<<(B * F + 127) / 128, 128, 0, st>>>(verts_ndc, faces, B, V, F, s->z_clip, s->perspective_correct,
+                                                                    g.g_tri, g.g_conv, grad_scale, g_ndc);
+    LAUNCH_CK("face_setup_backward_kernel");
+    if (!s->verts_are_ndc && g_verts) {
       project_verts_backward_kernel<<<(V * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, B, V,
                                                                      g.g_verts_ndc, g_verts);
       LAUNCH_CK("project_verts_backward_kernel");

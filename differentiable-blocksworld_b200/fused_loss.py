@@ -9,7 +9,10 @@ The blocks pass runs with the loss epilogue of include/dbw_render.h (dbw_render_
 and the MSE gradients w.r.t. both layers happen per pixel inside the rasterizer while the blended colour is in registers.
 Neither `fg` nor `rec` nor the two image-sized gradient round trips of a separate composite kernel ever touch HBM; the
 backward is the two raster backward kernels reading those gradients, scaled on the fly by the upstream gradient of the loss
-(dbw_render_backward_scaled).  Not usable when another loss consumes `rec` with gradient (LPIPS): the model then keeps
+(dbw_render_backward_scaled).  When the blocks pass is detach_bary over cell maps (the coarse phase) and a gradient is wanted,
+it goes further: the blocks forward kernel also runs the pass's backward while the per-pixel fragment lists are still on chip
+(dbw_render_forward_loss_grad), so neither its fragment records nor d loss / d blocks RGBA are written, and the backward only
+folds the accumulated gradients, times the upstream gradient (dbw_render_backward_deferred).  Not usable when another loss consumes `rec` with gradient (LPIPS): the model then keeps
 the separate composite kernel (dbw._CompositeMSE), which accepts a gradient on `rec`."""
 import ctypes
 
@@ -20,10 +23,13 @@ from ._lib import DbwLossEpilogue
 from .renderer import _c, _stream, scene_settings
 
 N_PARTIALS = 1024
+GRAD_VERTS, GRAD_MAPS, GRAD_ALPHA = 1, 2, 4          # grad_mask bits of dbw_render_forward_loss_grad (DBW_GRAD_*)
 # run the two passes' backward kernels concurrently (the environment's on a side stream: parallel branches of the step's CUDA
 # graph).  One GPU, 49 views: no gain (the kernels fill the machine by themselves); 8 GPUs, ~6 views each: the launches are
 # short and one kernel's ramp-up hides the other's tail -- bench.py --overlap-bwd measures it
 OVERLAP_BACKWARD_PASSES = False
+# differentiate the blocks pass inside its loss-epilogue forward kernel where it can (see above); False: the two-kernel path
+FUSE_BLOCKS_BACKWARD = True
 _side_stream = None
 
 
@@ -63,13 +69,19 @@ class _SceneMSEFn(torch.autograd.Function):
         fa = f32(blk_alpha) if blk_alpha is not None else None
         fmap_b = blk_face_map.to(torch.int32).contiguous()
         (cfg_e, table_e), (cfg_b, table_b) = cfgs
+        need = ctx.needs_input_grad
+        # grad mode is off in here: the settings, made outside, say whether a backward may follow (save_fragment_state)
+        fused = (FUSE_BLOCKS_BACKWARD and bool(cfg_b.save_fragment_state) and bool(cfg_b.detach_bary)
+                 and cfg_b.maps_are_texels4 == 2 and any(need[2:7]))
+        if fused:
+            cfg_b = _lib.DbwRenderSettings.from_buffer_copy(cfg_b)
+            cfg_b.save_fragment_state = 0                                     # the fused kernel writes no fragment records
         ws_e, bwd_e = _workspace(cfg_e, dev)
         ws_b, bwd_b = _workspace(cfg_b, dev)
         env_rgba = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)
         _lib.check(L.dbw_render_forward_ex(ctypes.byref(cfg_e), _c(env_verts), _c(env_pass.faces), _c(env_pass.faces_uvs),
                                            _c(env_pass.face_map), _c(env_maps), _c(table_e), _c(R), _c(T), None, _c(env_rgba),
                                            None, _c(ws_e), ws_e.numel(), None, None, _stream()), 'dbw_render_forward_ex')
-        g_fg = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)       # d loss / d blocks RGBA (unscaled)
         g_env = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)      # d loss / d env RGBA (unscaled)
         partials = torch.empty(N_PARTIALS, dtype=torch.float32, device=dev)
         rec = torch.empty(B, 3, H, W, dtype=torch.float32, device=dev) if want_rec else None
@@ -77,11 +89,23 @@ class _SceneMSEFn(torch.autograd.Function):
         ep.env_rgba, ep.target, ep.g_env = env_rgba.data_ptr(), imgs.data_ptr(), g_env.data_ptr()
         ep.rec = rec.data_ptr() if rec is not None else None
         ep.loss_partials, ep.n_partials, ep.inv_count = partials.data_ptr(), N_PARTIALS, float(inv_count)
-        _lib.check(L.dbw_render_forward_loss(ctypes.byref(cfg_b), _c(blk_verts), _c(blk_pass.faces), _c(blk_pass.faces_uvs),
-                                             _c(fmap_b), _c(blk_maps), _c(table_b), _c(R), _c(T), _c(fa), _c(g_fg), None,
-                                             _c(ws_b), ws_b.numel(), ctypes.byref(ep), _stream()), 'dbw_render_forward_loss')
+        g_fg = scratch_b = None
+        if fused:
+            mask = ((GRAD_VERTS if need[2] or need[5] or need[6] else 0) | (GRAD_MAPS if need[3] else 0)
+                    | (GRAD_ALPHA if need[4] and fa is not None else 0))
+            scratch_b = torch.empty(bwd_b, dtype=torch.uint8, device=dev)    # unscaled gradients, folded by the backward
+            _lib.check(L.dbw_render_forward_loss_grad(ctypes.byref(cfg_b), _c(blk_verts), _c(blk_pass.faces), _c(blk_pass.faces_uvs),
+                                                      _c(fmap_b), _c(blk_maps), _c(table_b), _c(R), _c(T), _c(fa), _c(ws_b),
+                                                      ws_b.numel(), ctypes.byref(ep), mask, _c(scratch_b), scratch_b.numel(),
+                                                      _stream()), 'dbw_render_forward_loss_grad')
+        else:
+            g_fg = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)   # d loss / d blocks RGBA (unscaled)
+            _lib.check(L.dbw_render_forward_loss(ctypes.byref(cfg_b), _c(blk_verts), _c(blk_pass.faces), _c(blk_pass.faces_uvs),
+                                                 _c(fmap_b), _c(blk_maps), _c(table_b), _c(R), _c(T), _c(fa), _c(g_fg), None,
+                                                 _c(ws_b), ws_b.numel(), ctypes.byref(ep), _stream()), 'dbw_render_forward_loss')
         loss = partials.sum()
-        ctx.save_for_backward(env_verts, env_maps, blk_verts, blk_maps, fa, R, T, fmap_b, table_e, table_b, ws_e, ws_b, g_fg, g_env)
+        ctx.save_for_backward(env_verts, env_maps, blk_verts, blk_maps, fa, R, T, fmap_b, table_e, table_b, ws_e, ws_b, g_fg, g_env,
+                              scratch_b)
         ctx.meta = (env_pass, blk_pass, cfg_e, cfg_b, bwd_e, bwd_b)
         if want_rec:
             ctx.mark_non_differentiable(rec)
@@ -90,7 +114,7 @@ class _SceneMSEFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_loss, _g_rec=None):
-        env_verts, env_maps, blk_verts, blk_maps, fa, R, T, fmap_b, table_e, table_b, ws_e, ws_b, g_fg, g_env = ctx.saved_tensors
+        env_verts, env_maps, blk_verts, blk_maps, fa, R, T, fmap_b, table_e, table_b, ws_e, ws_b, g_fg, g_env, scratch_b = ctx.saved_tensors
         env_pass, blk_pass, cfg_e, cfg_b, bwd_e, bwd_b = ctx.meta
         L = _lib.lib()
         dev = blk_verts.device
@@ -127,6 +151,16 @@ class _SceneMSEFn(torch.autograd.Function):
                                                      _c(gl), _c(g_verts), _c(g_alpha), _c(g_maps), _c(g_R), _c(g_T), _c(scratch),
                                                      scratch.numel(), _stream()), 'dbw_render_backward_cameras')
 
+        def run_blocks():
+            if scratch_b is None:
+                run(cfg_b, blk_pass, fmap_b, blk_verts, blk_maps, table_b, fa, ws_b, g_fg, bwd_b, g['gv_b'], g['gm_b'], g['ga_b'])
+                return
+            # the blocks pass was differentiated by its forward kernel: fold its scratch into the gradients, times g_loss
+            _lib.check(L.dbw_render_backward_deferred(ctypes.byref(cfg_b), _c(blk_verts), _c(blk_pass.faces), _c(R), _c(T), _c(ws_b),
+                                                      ws_b.numel(), _c(gl), _c(g['gv_b']), _c(g['ga_b']), _c(g['gm_b']), _c(g_R),
+                                                      _c(g_T), _c(scratch_b), scratch_b.numel(), _stream()),
+                       'dbw_render_backward_deferred')
+
         if OVERLAP_BACKWARD_PASSES:
             global _side_stream
             cur = torch.cuda.current_stream()
@@ -135,10 +169,10 @@ class _SceneMSEFn(torch.autograd.Function):
             _side_stream.wait_stream(cur)
             with torch.cuda.stream(_side_stream):
                 run(cfg_e, env_pass, env_pass.face_map, env_verts, env_maps, table_e, None, ws_e, g_env, bwd_e, g['gv_e'], g['gm_e'], None)
-            run(cfg_b, blk_pass, fmap_b, blk_verts, blk_maps, table_b, fa, ws_b, g_fg, bwd_b, g['gv_b'], g['gm_b'], g['ga_b'])
+            run_blocks()
             cur.wait_stream(_side_stream)
         else:
-            run(cfg_b, blk_pass, fmap_b, blk_verts, blk_maps, table_b, fa, ws_b, g_fg, bwd_b, g['gv_b'], g['gm_b'], g['ga_b'])
+            run_blocks()
             run(cfg_e, env_pass, env_pass.face_map, env_verts, env_maps, table_e, None, ws_e, g_env, bwd_e, g['gv_e'], g['gm_e'], None)
         gv_e, gm_e, gv_b, gm_b, ga_b = g['gv_e'], g['gm_e'], g['gv_b'], g['gm_b'], g['ga_b']
         return gv_e, gm_e, gv_b, gm_b, ga_b, g_R, g_T, None, None, None, None, None, None, None

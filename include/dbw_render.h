@@ -194,6 +194,35 @@ int dbw_render_forward_loss(const DbwRenderSettings* settings, const float* vert
                             float* out_g_rgba, int32_t* topk_ids, void* workspace, size_t workspace_bytes,
                             const DbwLossEpilogue* epilogue, void* stream);
 
+/*
+ * dbw_render_forward_loss for a detach_bary pass over float4 cell maps (maps_are_texels4 = 2) that also runs the pass's
+ * backward inside the same kernel, on the per-pixel fragment lists while they are still on chip: the texture scatter, the
+ * opacity sums and the distance-path vertex gradients go, unscaled, into `bwd_scratch` (dbw_workspace_bytes' bwd size; the
+ * call zero-fills it), and dbw_render_backward_deferred later folds them into the caller's gradients, multiplied by the
+ * upstream gradient of the loss.  No fragment records are written (save_fragment_state must be 0) and no d loss / d RGBA
+ * image either; g_env is written as by dbw_render_forward_loss.  grad_mask: which gradients the later fold will ask for
+ * (DBW_GRAD_VERTS also for camera gradients).  The loss terms are those of dbw_render_forward_loss, bit for bit.
+ */
+#define DBW_GRAD_VERTS 1
+#define DBW_GRAD_MAPS 2
+#define DBW_GRAD_ALPHA 4
+int dbw_render_forward_loss_grad(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
+                                 const float* faces_uvs, const int32_t* face_map, const float* maps,
+                                 const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                                 void* workspace, size_t workspace_bytes, const DbwLossEpilogue* epilogue, int32_t grad_mask,
+                                 void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
+
+/*
+ * The rest of the backward of a dbw_render_forward_loss_grad call (same settings, workspace and scratch): adds
+ * *grad_scale (device scalar, required) times the scratch into g_maps (the cell-gradient copies), g_faces_alpha and, through
+ * the face setup and projection backward, g_verts, g_R and g_T (any may be NULL; camera gradients as in
+ * dbw_render_backward_cameras).  A gradient whose grad_mask bit the forward did not set comes out unchanged.
+ */
+int dbw_render_backward_deferred(const DbwRenderSettings* settings, const float* verts, const int32_t* faces, const float* R,
+                                 const float* T, const void* workspace, size_t workspace_bytes, const float* grad_scale,
+                                 float* g_verts, float* g_faces_alpha, float* g_maps, float* g_R, float* g_T,
+                                 void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
+
 /* dbw_render_backward with grad_rgba multiplied by the device scalar *grad_scale (NULL = 1) as it is read. */
 int dbw_render_backward_scaled(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
                                const float* faces_uvs, const int32_t* face_map, const float* maps,
