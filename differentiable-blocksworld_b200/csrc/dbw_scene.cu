@@ -22,15 +22,15 @@ extern void dbw_count_launch_(void);
 // ------------------------------------------------------------------------------------------------ geometry
 #include "dbw_scene_math.cuh"
 
-// out: (N*Vb + Vg, 3) world-space vertices, blocks first then the ground; with env_static (n_static > 0) the layout is
-// (n_static + Vg + N*Vb, 3): the static environment vertices (copied), the ground, then the blocks
+// out: (N*Vb + Vg, 3) world-space vertices, blocks first then the ground; with env_layout it is (n_static + Vg + N*Vb, 3): the
+// static environment vertices (copied; there may be none), the ground, then the blocks
 __global__ void scene_geometry_forward_kernel(const GeomParams P, float* __restrict__ out, const float* __restrict__ env_static,
-                                              int n_static) {
+                                              int n_static, bool env_layout) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int nb = P.n_blocks * P.verts_per_block;
   if (i < n_static * 3) out[i] = env_static[i];
   if (i >= nb + P.n_ground_verts) return;
-  if (n_static > 0) out += (ptrdiff_t)(n_static + (i < nb ? P.n_ground_verts : -nb)) * 3;      // blocks move behind the ground
+  if (env_layout) out += (ptrdiff_t)(n_static + (i < nb ? P.n_ground_verts : -nb)) * 3;      // blocks move behind the ground
   const int prim = i < nb ? i / P.verts_per_block : P.n_blocks;
   const int v = i < nb ? i - prim * P.verts_per_block : i - nb;
   float u[3], aux[6], R[9], sc[3] = {1.f, 1.f, 1.f};
@@ -146,7 +146,7 @@ extern "C" int dbw_scene_geometry_forward(const DbwSceneGeometry* g, float* vert
     return dbw_fail_("dbw_scene_geometry_forward: bad sizes", cudaSuccess);
   const int n = g->n_blocks * g->verts_per_block + g->n_ground_verts;
   if (n == 0) return 0;
-  scene_geometry_forward_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(make_geom(g), verts_out, nullptr, 0);
+  scene_geometry_forward_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(make_geom(g), verts_out, nullptr, 0, false);
   SCENE_LAUNCH_CK("scene_geometry_forward_kernel");
   return 0;
 }
@@ -160,7 +160,7 @@ extern "C" int dbw_scene_geometry_forward_env(const DbwSceneGeometry* g, const f
   const int threads = n > n_env_static * 3 ? n : n_env_static * 3;
   if (threads == 0) return 0;
   scene_geometry_forward_kernel<<<(threads + 127) / 128, 128, 0, (cudaStream_t)stream>>>(make_geom(g), verts_out, env_static_verts,
-                                                                                         n_env_static);
+                                                                                         n_env_static, true);
   SCENE_LAUNCH_CK("scene_geometry_forward_kernel");
   return 0;
 }
