@@ -426,7 +426,9 @@ class DifferentiableBlocksWorld(nn.Module):
             self._passes = (key, ScenePass(st['faces_e'], st['fvu_e'], st['fmap_e'], env_table, self.renderer_env,
                                            n_static_faces=self.bkg_n_faces),
                             ScenePass(st['faces_b'], st['fvu_b'], st['fmap_b'], table, renderer, alpha_group=self.alpha_group_faces or self.BNF))
-        return scene_mse(env_verts, env_atlas, blk_verts, atlas, alpha, inp['R'], inp['T'], inp['imgs'], self._passes[1],
+        # data parallel with pose gradients: the poses are this rank's slices of pose leaves that went through the sum point
+        R, T = self.grad_sum_point.cameras(inp) if self.grad_sum_point is not None else (inp['R'], inp['T'])
+        return scene_mse(env_verts, env_atlas, blk_verts, atlas, alpha, R, T, inp['imgs'], self._passes[1],
                          self._passes[2], fmap, n_total_views=self.n_total_views or len(inp['imgs']), view_rows=inp.get('rows'))
 
     def can_sum_gradients_at_scene_tensors(self, imgs):

@@ -3,16 +3,27 @@ back-propagate to every leaf parameter -- captured once on static buffers and re
 hundred kernel launches of 2-100 us each (scene construction, two rasterization passes, their backward, the
 reductions); replaying them as one graph removes the launch gaps and the Python/autograd dispatch that otherwise cost
 more than the kernels themselves.  Requires the model's static-topology mode (dbw.py): no host synchronisation and no
-shape that depends on parameter values inside forward()."""
+shape that depends on parameter values inside forward().
+
+Camera-pose gradients (a ViewParallel built with max_pose_views > 0, and poses that require grad in example_inp): the inputs
+are the full batch; the step keeps this rank's slice of the per-view inputs and the full-batch poses as static LEAF buffers
+that require grad, renders from their slices inside the graph, and after each replay back-propagates the (summed) pose
+gradient into the caller's graph behind run()'s inp['R'] / inp['T'] -- a small eager backward outside the graph."""
 import torch
 
-from .parallel import refuse_camera_gradients
+from .parallel import pose_backward, refuse_camera_gradients, wants_pose_gradients
 
 
 class GraphedStep:
     def __init__(self, view_parallel, example_inp, n_total_views, warmup=3, capture_all_reduce=None, generator=None):
-        refuse_camera_gradients(example_inp, 'GraphedStep')
         self.vp, self.model = view_parallel, view_parallel.model
+        self.pose = None                   # (R, T, views): static full-batch pose leaves and this rank's views of them
+        if wants_pose_gradients(example_inp):
+            view_parallel.check_pose_views(example_inp, 'GraphedStep')
+            if n_total_views != len(example_inp['imgs']):
+                raise ValueError('GraphedStep: with camera-pose gradients example_inp is the full batch of n_total_views views')
+            self.pose = view_parallel.pose_leaves(example_inp)
+            example_inp = {k: v for k, v in view_parallel.shard(example_inp)[0].items() if k not in ('R', 'T')}
         # The gradient all-reduce is captured INTO the graph when it is the peer-memory kernel (a plain launch).  An
         # ncclAllReduce is issued right after the replay instead: captured, it hung on 2 GPUs with this image's NCCL (round 1).
         if capture_all_reduce is None:
@@ -65,22 +76,56 @@ class GraphedStep:
         # the gradient tensors THIS capture writes (bucket views when the gradients are gathered, else tensors of the graph's
         # private pool): another GraphedStep on the same model (PipelinedGraphedStep) leaves its own in the .grad attributes
         self.grads = [p.grad for p in self.vp.bucket.params]
+        self.pose_grads = self.vp.pose_grads(self.pose) if self.pose is not None else None
 
     def _body(self):
-        losses, reduced = self.vp.local_step(self.static_inp, None, self.n_total, collective=self.capture_all_reduce)
+        losses, reduced = self.vp.local_step(self.static_inp, None, self.n_total, collective=self.capture_all_reduce, poses=self.pose)
         self.inside = self.vp.reduces_inside_backward(self.static_inp)      # the collective sits INSIDE the backward (parallel.GradSumPoint)
         if self.capture_all_reduce and not reduced:
-            self.vp.bucket.all_reduce(self.vp.group)
+            self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views)
         return losses
+
+    @property
+    def _pose_views(self):
+        return self.n_total if self.pose is not None else 0
+
+    def check_poses(self, inp):
+        """poses in `inp` must require grad exactly when this step was captured with pose gradients"""
+        if inp is None or not any(k in inp for k in ('R', 'T')):
+            return
+        if self.pose is None and wants_pose_gradients(inp):
+            if self.vp.max_pose_views == 0:
+                refuse_camera_gradients(inp, 'GraphedStep')
+            raise RuntimeError('GraphedStep: these poses require grad, but the step was captured with poses that do not; '
+                               'build the step from an example whose poses require grad')
+        if self.pose is not None and not wants_pose_gradients(inp):
+            raise RuntimeError('GraphedStep: the step was captured with poses that require grad, but these do not')
+
+    def staged(self, inp):
+        """[(static buffer, value)] for the tensors of `inp` that a run copies into the static inputs: with pose gradients,
+        this rank's slice of the full-batch per-view tensors; the poses themselves are not among them (load_poses)"""
+        if self.pose is not None:
+            inp = self.vp.take({k: v for k, v in inp.items() if k not in ('R', 'T')}, self.pose[2], self.n_total)
+        return [(self.static_inp[k], v) for k, v in inp.items() if k in self.static_inp]
+
+    def load_poses(self, inp, non_blocking=True):
+        """copy inp's full-batch poses into the static pose leaves (on the current stream)"""
+        with torch.no_grad():
+            for k, leaf in zip(('R', 'T'), self.pose[:2]):
+                if k in inp:
+                    leaf.copy_(inp[k].detach(), non_blocking=non_blocking)
 
     def run(self, inp=None, non_blocking=True, all_reduce=True):
         """inp: optional dict of (host or device) tensors for this step, copied into the static buffers.
-        all_reduce=False skips the collective when it is issued after the replay (a captured one always runs)."""
-        refuse_camera_gradients(inp, 'GraphedStep')
+        all_reduce=False skips the collective when it is issued after the replay (a captured one always runs).
+        With pose gradients, inp holds the full batch, and the summed pose gradient is back-propagated into the graph
+        behind inp['R'] / inp['T'] (without them, it stays in the static leaves' .grad)."""
+        self.check_poses(inp)
         if inp is not None:
-            for k, v in inp.items():
-                if k in self.static_inp:
-                    self.static_inp[k].copy_(v, non_blocking=non_blocking)
+            if self.pose is not None:
+                self.load_poses(inp, non_blocking)
+            for buf, v in self.staged(inp):
+                buf.copy_(v, non_blocking=non_blocking)
         if self._phase() != self.phase:          # a schedule milestone was crossed (coarse -> fine, decimation off): re-capture
             self._capture()
         self._bind_buffers()                       # eager code in between (evaluation, another GraphedStep) may have re-pointed them
@@ -90,21 +135,29 @@ class GraphedStep:
         self.graph.replay()
         for p, g in zip(self.vp.bucket.params, self.grads):
             p.grad = g
+        if self.pose is not None:
+            for q, g in zip(self.pose, self.pose_grads):
+                q.grad = g
         if not self.capture_all_reduce and all_reduce and self.vp.world_size > 1:
             if self.inside:
                 raise RuntimeError('this step sums its gradients inside the backward (parallel.GradSumPoint) but was captured '
                                    'with capture_all_reduce=False: its gradients are local and cannot be reduced afterwards')
-            self.vp.bucket.all_reduce(self.vp.group)
+            self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views)
+        if self.pose is not None and inp is not None:
+            pose_backward(inp, self.pose_grads)
         return self.losses
 
 
 class PipelinedGraphedStep:
     """Two GraphedSteps on alternating static input buffers: while step i replays, the inputs of step i+1 are copied
     host->device on a side stream (what a prefetching DataLoader does for src/trainer.py:141).  `run(host_inp)` returns
-    the losses of the step that consumed `host_inp`."""
+    the losses of the step that consumed `host_inp`.  Poses that require grad are NOT prefetched: an optimiser step may
+    change them between the prefetch and the step that consumes them, so they are copied into that step's static leaves on
+    the current stream right before its replay."""
 
     def __init__(self, view_parallel, example_inp, n_total_views, capture_all_reduce=None):
-        refuse_camera_gradients(example_inp, 'PipelinedGraphedStep')
+        if wants_pose_gradients(example_inp):
+            view_parallel.check_pose_views(example_inp, 'PipelinedGraphedStep')
         gen = torch.Generator(device=example_inp['imgs'].device)
         gen.manual_seed(view_parallel.seed)
         self.steps = [GraphedStep(view_parallel, example_inp, n_total_views, capture_all_reduce=capture_all_reduce, generator=gen)
@@ -118,16 +171,15 @@ class PipelinedGraphedStep:
     def _stage(self, b, host_inp):
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(self.free[b])
-            for k, v in host_inp.items():
-                if k in self.steps[b].static_inp:
-                    self.steps[b].static_inp[k].copy_(v, non_blocking=True)
+            for buf, v in self.steps[b].staged(host_inp):
+                buf.copy_(v, non_blocking=True)
             self.ready[b].record(self.copy_stream)
 
     def run(self, host_inp, next_host_inp=None, all_reduce=True):
         """consume `host_inp` (staged now unless it was prefetched as the previous call's `next_host_inp`) and
         prefetch `next_host_inp` for the following call."""
-        refuse_camera_gradients(host_inp, 'PipelinedGraphedStep')
-        refuse_camera_gradients(next_host_inp, 'PipelinedGraphedStep')
+        for x in (host_inp, next_host_inp):
+            self.steps[0].check_poses(x)
         b = self.i % 2
         cur = torch.cuda.current_stream()
         if not self.primed:
@@ -140,7 +192,10 @@ class PipelinedGraphedStep:
         else:
             self.primed = False
         cur.wait_event(self.ready[b])
-        losses = self.steps[b].run(all_reduce=all_reduce)
+        poses = None
+        if self.steps[b].pose is not None:          # the poses as they are now, not as they were at the prefetch
+            poses = {k: host_inp[k] for k in ('R', 'T') if k in host_inp}
+        losses = self.steps[b].run(poses, all_reduce=all_reduce)
         self.free[b].record(cur)
         self.i += 1
         return losses

@@ -12,7 +12,11 @@ Correctness conditions handled here:
   * view-independent terms (parsimony / TV / overlap, dbw.py:373-405) are computed identically on every rank: divided by
     the world size before a leaf SUM, counted once when the SUM happens at the scene tensors (they do not pass through it);
   * the opacity noise (dbw.py:300-301) and the overlap sample points (dbw.py:393) come from a generator that every
-    rank seeds identically at every step."""
+    rank seeds identically at every step.
+Camera poses that require grad (ViewParallel(max_pose_views=N)): the step renders its shard from slices of full-batch pose
+leaves, so each rank's pose gradient is a (B, 12) block with zeros on the views it did not render; that block rides in the same
+one collective as the scene's gradients (the tail of the leaf bucket, or through the GradSumPoint), and the sum is handed on
+to the caller's R / T with one small eager backward."""
 import ctypes
 
 import torch
@@ -35,8 +39,21 @@ def refuse_camera_gradients(inp, who):
     for k in ('R', 'T'):
         v = inp.get(k) if inp is not None else None
         if torch.is_tensor(v) and v.requires_grad:
-            raise RuntimeError(f"{who}: inp['{k}'] requires grad, but camera-pose gradients are only computed by a plain "
-                               f"model(inp) step (not sharded, not graph-captured); detach the poses or call the model directly")
+            raise RuntimeError(f"{who}: inp['{k}'] requires grad, but this step was not built for camera-pose gradients: "
+                               f"construct its ViewParallel with max_pose_views >= the views of a step, detach the poses, or "
+                               f"call the model directly")
+
+
+def wants_pose_gradients(inp):
+    """inp's camera poses require grad"""
+    return inp is not None and any(torch.is_tensor(inp.get(k)) and inp[k].requires_grad for k in ('R', 'T'))
+
+
+def pose_backward(inp, grads):
+    """continue the step's summed pose gradients (g_R (B,3,3), g_T (B,3)) into the caller's graph behind inp['R'] / inp['T']"""
+    pairs = [(inp[k], g) for k, g in zip(('R', 'T'), grads) if torch.is_tensor(inp.get(k)) and inp[k].requires_grad]
+    if pairs:
+        torch.autograd.backward([t for t, _ in pairs], [g.to(t.dtype) for t, g in pairs])
 
 
 ROW_BAND = 16          # rows per shardable band: the tallest raster tile (16 x 16, the K <= 4 forward), so tiles stay whole
@@ -125,9 +142,30 @@ class GradSumPoint:
 
     def __init__(self, peer):
         self.peer = peer
+        self.pose_leaves = None          # (R (B,3,3), T (B,3), views): full-batch pose leaves that ride through the point
+        self._cameras = None
 
     def __call__(self, *tensors):
-        return _GradSumFn.apply(self, *tensors)
+        if self.pose_leaves is None:
+            return _GradSumFn.apply(self, *tensors)
+        R, T, views = self.pose_leaves
+        *out, R, T = _GradSumFn.apply(self, *tensors, R, T)
+        self._cameras = (R[views], T[views])
+        return tuple(out)
+
+    def ride(self, poses):
+        """poses = (R, T, views) or None: from the next call on, the pose leaves pass through the point with the scene tensors,
+        so their gradients join the same one exchange; the model then renders from cameras()"""
+        self.pose_leaves, self._cameras = poses, None
+
+    def cameras(self, inp):
+        """the (R, T) a model renders its shard from, read after it has called the point: this rank's slices of the point's pose
+        outputs when pose leaves ride along, inp's own poses otherwise"""
+        if self.pose_leaves is None:
+            return inp['R'], inp['T']
+        if self._cameras is None:
+            raise RuntimeError('GradSumPoint.cameras() before the point was called on the scene tensors')
+        return self._cameras
 
     def sum_over_ranks(self, grads):
         n = sum(g.numel() for g in grads)
@@ -148,21 +186,25 @@ class GradSumPoint:
 class GradBucket:
     """All parameter gradients as views into one flat buffer -> a single all-reduce per step."""
 
-    def __init__(self, params, peer_factory=None, min_floats=0):
+    def __init__(self, params, peer_factory=None, min_floats=0, max_pose_views=0):
         """peer_factory(n_floats, device) -> PeerAllReduce or None: when given and successful, the flat buffer IS the peer-memory
         arena's bucket (csrc/dbw_comm.cu) and all_reduce() is its kernel; else a plain tensor and torch.distributed.
-        min_floats: capacity the arena needs for its other user (GradSumPoint)"""
+        min_floats: capacity the arena needs for its other user (GradSumPoint).
+        max_pose_views: room for the pose gradients of that many views (12 floats each: the B x 9 entries of g_R, then the
+        B x 3 of g_T) after the parameter gradients, gathered and all-reduced with them"""
         self.params = [p for p in params if p.requires_grad]
         n = sum(p.numel() for p in self.params)
         ref = self.params[0]
         self.n = n
         n_pad = (n + 3) // 4 * 4                     # padded: 128-bit all-reduce lanes
-        self.peer = peer_factory(max(n_pad, (int(min_floats) + 3) // 4 * 4), ref.device) if peer_factory is not None else None
+        n_all = n_pad + 12 * int(max_pose_views)
+        self.peer = peer_factory(max(n_all, (int(min_floats) + 3) // 4 * 4), ref.device) if peer_factory is not None else None
         if self.peer is not None:
             self.peer.flat.zero_()
-            self.flat = self.peer.flat[:n_pad]
+            self._all = self.peer.flat[:n_all]
         else:
-            self.flat = torch.zeros(n_pad, dtype=ref.dtype, device=ref.device)
+            self._all = torch.zeros(n_all, dtype=ref.dtype, device=ref.device)
+        self.flat = self._all[:n_pad]               # the parameter gradients; the pose region follows it
         self._zeros = {}
         off, self.views = 0, []
         for p in self.params:
@@ -177,40 +219,51 @@ class GradBucket:
         for p, v in zip(self.params, self.views):
             p.grad = v
 
-    def backward(self, total, gather=True):
+    def backward(self, total, gather=True, poses=()):
         """Back-propagate `total` and leave every parameter's gradient in the flat bucket with ONE gather kernel: the
         parameters enter the backward without .grad, so autograd hands over each gradient tensor as it is (no zero-fill
         of the bucket, no accumulate-add per parameter); a single cat then writes them into the flat buffer and the
         .grad attributes become the bucket views again.  CUDA-graph capturable.  gather=False stops after the backward:
-        the .grad attributes are autograd's own tensors and the flat buffer is not written (no collective reads it)."""
-        for p in self.params:
+        the .grad attributes are autograd's own tensors and the flat buffer is not written (no collective reads it).
+        poses: the step's pose leaves (R (B,3,3), T (B,3)); the same cat writes their gradients into the pose region"""
+        for p in (*self.params, *poses):
             p.grad = None
         total.backward()
         if not gather:
             return
-        pieces = []
-        for p in self.params:
-            g = p.grad
-            if g is None:                                # unused in this phase (e.g. opacities once they are frozen)
-                if id(p) not in self._zeros:
-                    self._zeros[id(p)] = torch.zeros(p.numel(), dtype=self.flat.dtype, device=self.flat.device)
-                g = self._zeros[id(p)]
-            pieces.append(g.reshape(-1))
+        pieces = [(p.grad if p.grad is not None else self._zero(p.numel())).reshape(-1) for p in self.params]
+        n = self.n                                       # a None gradient: unused in this phase (e.g. frozen opacities)
+        if poses:
+            if self.flat.numel() > n:
+                pieces.append(self._zero(self.flat.numel() - n))
+            pieces += [(q.grad if q.grad is not None else self._zero(q.numel())).reshape(-1) for q in poses]
+            n = self.flat.numel() + sum(q.numel() for q in poses)
         with torch.no_grad():
-            torch.cat(pieces, out=self.flat[:self.n])
+            torch.cat(pieces, out=self._all[:n])
         for p, v in zip(self.params, self.views):
             p.grad = v
+        o = self.flat.numel()
+        for q in poses:
+            q.grad = self._all[o:o + q.numel()].view_as(q)
+            o += q.numel()
+
+    def _zero(self, n):
+        if n not in self._zeros:
+            self._zeros[n] = torch.zeros(n, dtype=self.flat.dtype, device=self.flat.device)
+        return self._zeros[n]
 
     def grads_flat(self):
         """the gradients as one flat vector in bucket order, whichever way the last backward left them"""
         return torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).reshape(-1) for p in self.params])
 
-    def all_reduce(self, group=None):
+    def all_reduce(self, group=None, pose_views=0):
+        """sum the bucket over the ranks; pose_views: the pose gradients of that many views ride in the same collective"""
         if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
+            buf = self._all[:self.flat.numel() + 12 * pose_views]
             if self.peer is not None:
-                self.peer.all_reduce(self.flat)
+                self.peer.all_reduce(buf)
             else:
-                dist.all_reduce(self.flat, op=dist.ReduceOp.SUM, group=group)
+                dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
 
     @property
     def nbytes(self):
@@ -224,7 +277,7 @@ class ViewParallel:
     VIEW_KEYS = ('imgs', 'R', 'T', 'K')
 
     def __init__(self, model, group=None, seed=227391, row_bands=False, collective='nccl', reduce_at='auto', gather_grads=None,
-                 peer_factory=None):
+                 peer_factory=None, max_pose_views=0):
         """collective: 'nccl' (torch.distributed all_reduce; also what gloo groups use), 'p2p' (the NVLink peer-memory kernel
         of csrc/dbw_comm.cu, CUDA-graph capturable) or 'auto' (p2p if it initialises on this node, else nccl).
         reduce_at: 'leaf' (all-reduce the parameter gradients after the backward), 'scene' (sum the gradients of the scene
@@ -235,8 +288,13 @@ class ViewParallel:
         None: only when a leaf all-reduce reads the bucket (world > 1 and no reduction inside the backward) -- otherwise the
         .grad attributes are autograd's own tensors and bucket.grads_flat() concatenates them on demand.
         peer_factory(n_floats, device) -> object with `.flat` (the bucket) and `.all_reduce(prefix_of_flat)`: replaces the
-        peer-memory arena (tests run the scene-level reduction over gloo with it)"""
+        peer-memory arena (tests run the scene-level reduction over gloo with it).
+        max_pose_views: 0 refuses camera poses that require grad; N > 0 reserves 12 N floats of the bucket / arena and accepts
+        them on steps of at most N views.  Such a step takes FULL-BATCH inputs (all views' imgs, K, R, T, identical on every
+        rank) and leaves the gradient of the global loss with respect to all B views' poses in the caller's graph, the same
+        on every rank (pose_step)"""
         self.model, self.group, self.seed = model, group, seed
+        self.max_pose_views = int(max_pose_views)
         self.reduce_at, self.gather_grads = reduce_at, gather_grads
         self.row_bands = row_bands          # shard at (view, row band) granularity (needs the model's fused-loss path)
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -253,7 +311,8 @@ class ViewParallel:
                 return None
 
         want_point = reduce_at in ('scene', 'auto') and hasattr(model, 'grad_sum_floats')
-        self.bucket = GradBucket(model.parameters(), peer_factory or arena_factory, model.grad_sum_floats() if want_point else 0)
+        self.bucket = GradBucket(model.parameters(), peer_factory or arena_factory,
+                                 model.grad_sum_floats() + 12 * self.max_pose_views if want_point else 0, self.max_pose_views)
         self.sum_point = GradSumPoint(self.bucket.peer) if (want_point and self.bucket.peer is not None) else None
         if reduce_at == 'scene' and self.sum_point is None and self.world_size > 1:
             raise RuntimeError("reduce_at='scene' needs the peer-memory collective (collective='p2p' or 'auto') and a model with grad_sum_floats()")
@@ -270,18 +329,50 @@ class ViewParallel:
         """this rank's part of a batch: whole views, or -- with row_bands -- the views it touches plus `rows` (B_local, 2):
         the [row_begin, row_end) of each that it renders (the model hands them to the kernels, dbw_render.h view_rows)"""
         B = len(inp['imgs'])
-        out = dict(inp)
+        sl, rows = self.views(B, inp['imgs'].shape[-2])
+        out = self.take(inp, sl, B)
+        if rows is not None:
+            out['rows'] = rows
+        return out, B
+
+    def views(self, n_views, height):
+        """this rank's views of a step (a slice) and, with row_bands, the (B_local, 2) rows it renders of each (else None)"""
         if self.row_bands and self.world_size > 1:
-            pieces = shard_row_bands(B, inp['imgs'].shape[-2], self.world_size, self.rank)
+            pieces = shard_row_bands(n_views, height, self.world_size, self.rank)
             idx = [v for v, _, _ in pieces]
             sl = slice(idx[0], idx[-1] + 1) if idx else slice(0, 0)
-            out['rows'] = torch.tensor([[a, b] for _, a, b in pieces], dtype=torch.int32).reshape(-1, 2)
-        else:
-            sl = shard_views(B, self.world_size, self.rank)
+            return sl, torch.tensor([[a, b] for _, a, b in pieces], dtype=torch.int32).reshape(-1, 2)
+        return shard_views(n_views, self.world_size, self.rank), None
+
+    def take(self, inp, views, n_views):
+        """inp with every per-view tensor of the n_views-view step sliced to `views`"""
+        out = dict(inp)
         for k in self.VIEW_KEYS:
-            if k in inp and torch.is_tensor(inp[k]) and inp[k].shape[:1] == (B,):
-                out[k] = inp[k][sl]
-        return out, B
+            if k in inp and torch.is_tensor(inp[k]) and inp[k].shape[:1] == (n_views,):
+                out[k] = inp[k][views]
+        return out
+
+    def check_pose_views(self, inp, who):
+        """a step whose poses require grad: refused unless this wrapper reserved room for at least its B views"""
+        if self.max_pose_views == 0:
+            refuse_camera_gradients(inp, who)
+        B = len(inp['imgs'])
+        if B > self.max_pose_views:
+            raise ValueError(f'{who}: a step of {B} views with camera-pose gradients, but the ViewParallel reserved room for '
+                             f'max_pose_views={self.max_pose_views}')
+        for k, shape in (('R', (B, 3, 3)), ('T', (B, 3))):
+            if tuple(inp[k].shape) != shape:
+                raise ValueError(f"{who}: with camera-pose gradients inp['{k}'] is the full batch {shape}, got {tuple(inp[k].shape)}")
+
+    def pose_leaves(self, inp):
+        """(R, T, views): leaves holding the values of inp's full-batch poses, which the step renders its shard from"""
+        B = len(inp['imgs'])
+        return (inp['R'].detach().to(torch.float32, copy=True).requires_grad_(True),
+                inp['T'].detach().to(torch.float32, copy=True).requires_grad_(True), self.views(B, inp['imgs'].shape[-2])[0])
+
+    @staticmethod
+    def pose_grads(poses):
+        return [q.grad if q.grad is not None else torch.zeros_like(q) for q in poses[:2]]
 
     def _sync_rng(self, device):
         g = getattr(self.model, 'noise_generator', None)
@@ -294,33 +385,54 @@ class ViewParallel:
         """this step's gradients are summed over the ranks inside the backward, at the scene tensors (GradSumPoint)"""
         return self.sum_point is not None and self.model.can_sum_gradients_at_scene_tensors(inp['imgs'])
 
-    def local_step(self, inp, labels, n_total_views, collective=True):
+    def local_step(self, inp, labels, n_total_views, collective=True, poses=None):
         """forward + backward over this rank's shard.  Returns (losses, reduced): reduced = the gradients are already the
         sum over ranks (the GradSumPoint ran inside the backward); otherwise a leaf all-reduce of the bucket is due.
-        collective=False on a step that would reduce inside the backward leaves LOCAL gradients (timing breakdowns only)."""
-        refuse_camera_gradients(inp, 'ViewParallel')
+        collective=False on a step that would reduce inside the backward leaves LOCAL gradients (timing breakdowns only).
+        poses: (R, T, views) of pose_leaves(): the shard renders from R[views], T[views]; the leaves' (B-row) gradients go
+        through the GradSumPoint with the scene tensors, or into the bucket's pose region for the leaf all-reduce."""
+        if poses is None:
+            refuse_camera_gradients(inp, 'ViewParallel')
         inside = self.reduces_inside_backward(inp)
         self.model.n_total_views = n_total_views
         self.model.grad_sum_point = self.sum_point if (inside and collective) else None
+        if poses is not None:
+            R, T, views = poses
+            if self.model.grad_sum_point is not None:          # the model renders from sum_point.cameras()
+                self.sum_point.ride(poses)
+                inp = dict(inp, R=R.detach()[views], T=T.detach()[views])
+            else:
+                inp = dict(inp, R=R[views], T=T[views])
         try:
             losses = self.model(inp, labels)
             gather = self.gather_grads if self.gather_grads is not None else (self.world_size > 1 and not inside)
             self.bucket.backward(self.weighted_total(losses, len(inp['imgs']), n_total_views, replicated_everywhere=inside),
-                                 gather=gather)
+                                 gather=gather, poses=poses[:2] if poses is not None else ())
         finally:
             self.model.grad_sum_point = None
+            if self.sum_point is not None:
+                self.sum_point.ride(None)
         return losses, inside and collective
 
     def forward_backward(self, inp, labels=None, already_sharded=False, n_total_views=None, all_reduce=True):
-        """local forward -> backward -> ONE all-reduce (inside the backward or after it).  Returns the (local) loss dict."""
-        refuse_camera_gradients(inp, 'ViewParallel')
+        """local forward -> backward -> ONE all-reduce (inside the backward or after it).  Returns the (local) loss dict.
+        With poses that require grad (max_pose_views > 0) inp is the full batch; the pose gradient of the global loss is
+        back-propagated into the caller's graph behind inp['R'] / inp['T'] before returning."""
+        full, poses = inp, None
+        if wants_pose_gradients(inp):
+            self.check_pose_views(inp, 'ViewParallel')
+            if already_sharded:
+                raise ValueError('ViewParallel: a step with camera-pose gradients takes the full batch (already_sharded=False)')
+            poses = self.pose_leaves(inp)
         if not already_sharded:
             inp, n_total_views = self.shard(inp)
         self._sync_rng(inp['imgs'].device)
         self._step += 1
-        losses, reduced = self.local_step(inp, labels, n_total_views, collective=all_reduce)
+        losses, reduced = self.local_step(inp, labels, n_total_views, collective=all_reduce, poses=poses)
         if all_reduce and not reduced:
-            self.bucket.all_reduce(self.group)
+            self.bucket.all_reduce(self.group, pose_views=n_total_views if poses is not None else 0)
+        if poses is not None:
+            pose_backward(full, self.pose_grads(poses))
         return losses
 
     def weighted_total(self, losses, n_local_views, n_total_views, replicated_everywhere=False):
