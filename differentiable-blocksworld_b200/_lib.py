@@ -73,7 +73,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_sizeof_setti
            'dbw_eval_cell_ranges', 'dbw_eval_downsample_workspace_bytes', 'dbw_eval_radius_downsample', 'dbw_eval_nn_distance',
            'dbw_knn_forward', 'dbw_knn_backward',
            'dbw_lpips_workspace_bytes', 'dbw_lpips_prepare_weights', 'dbw_lpips_forward', 'dbw_lpips_backward',
-           'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward']
+           'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward',
+           'dbw_lpips_head_forward', 'dbw_lpips_head_backward']
 
 _lib = None
 
@@ -152,6 +153,8 @@ def lib():
         L.dbw_lpips_dgrad_last.argtypes = [vp] * 3 + [i32, vp, i64, i32, i32, vp]
         L.dbw_lpips_maxpool.argtypes = [vp, vp, i64, i32, i32, i32, vp]
         L.dbw_lpips_maxpool_backward.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp]
+        L.dbw_lpips_head_forward.argtypes = [vp] * 3 + [i64] + [i32] * 5 + [vp, vp, vp]
+        L.dbw_lpips_head_backward.argtypes = [vp] * 3 + [i64] + [i32] * 5 + [vp, vp, i32, vp, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

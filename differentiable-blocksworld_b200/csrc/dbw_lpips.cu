@@ -46,10 +46,11 @@ Dims dims_of(int64_t B, int H, int W) {
 }
 
 int64_t align64(int64_t n) { return (n + 63) & ~int64_t(63); }        // floats: 256-byte aligned regions
+int64_t head_chunks(int H, int W) { return ((int64_t)H * W + HEAD_PIX - 1) / HEAD_PIX; }
 
 // workspace layout, in floats: rec activations of the 13 layers (only its 5 taps when no backward follows), the 5 taps of
 // imgs, two scratch tensors of B*H*W*64 (pool outputs and the intermediates not kept in the forward, the running gradient
-// in the backward), the head partials, the seed the forward used
+// in the backward), the head partials, the seed the forward used (the contract is stated in include/dbw_render.h)
 struct Layout {
   int64_t act[LP_LAYERS], tap0[5], s0, s1, partials, seed, total;
   int64_t chunks[5], part_off[5];
@@ -71,7 +72,7 @@ Layout layout_of(const Dims& d, bool save) {
   L.partials = o;
   int64_t p = 0;
   for (int k = 0; k < 5; ++k) {
-    L.chunks[k] = ((int64_t)d.H[k] * d.W[k] + HEAD_PIX - 1) / HEAD_PIX;
+    L.chunks[k] = head_chunks(d.H[k], d.W[k]);
     L.part_off[k] = p; p += d.B * L.chunks[k];
   }
   o += align64(p);
@@ -552,33 +553,40 @@ int pool_backward(const float* in, const float* gout, float* gin, int64_t B, int
   return 0;
 }
 
-int head_forward(int k, const float* f0, const float* f1, const float* lin, const Dims& d, const Layout& L, int train,
-                 const uint32_t* seed, float* ws, cudaStream_t st) {
-  const dim3 grid((unsigned)L.chunks[k], (unsigned)d.B);
-  const int HW = d.H[k] * d.W[k];
-  float* part = ws + L.partials + L.part_off[k];
-  const int n = (int)L.chunks[k];
-  switch (LP_TAP_C[k]) {
-    case 64: lpips_head_forward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, part, n); break;
-    case 128: lpips_head_forward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, part, n); break;
-    case 256: lpips_head_forward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, part, n); break;
-    default: lpips_head_forward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, part, n); break;
+// partials (B, head_chunks(H, W)); C is one of 64, 128, 256, 512
+int head_forward(const float* f0, const float* f1, const float* lin, int64_t B, int H, int W, int C, int tap, int train,
+                 const uint32_t* seed, float* part, cudaStream_t st) {
+  const int n = (int)head_chunks(H, W);
+  const dim3 grid((unsigned)n, (unsigned)B);
+  const int HW = H * W;
+  switch (C) {
+    case 64: lpips_head_forward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
+    case 128: lpips_head_forward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
+    case 256: lpips_head_forward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
+    default: lpips_head_forward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
   }
   LP_LAUNCH_CK("lpips_head_forward_kernel");
   return 0;
 }
 
-int head_backward(int k, const float* f0, const float* f1, const float* lin, const Dims& d, const Layout& L, int train,
+int head_backward(const float* f0, const float* f1, const float* lin, int64_t B, int H, int W, int C, int tap, int train,
                   const uint32_t* seed, const float* grad_value, int accumulate, float* g, cudaStream_t st) {
-  const dim3 grid((unsigned)L.chunks[k], (unsigned)d.B);
-  const int HW = d.H[k] * d.W[k];
-  switch (LP_TAP_C[k]) {
-    case 64: lpips_head_backward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, grad_value, accumulate, g); break;
-    case 128: lpips_head_backward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, grad_value, accumulate, g); break;
-    case 256: lpips_head_backward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, grad_value, accumulate, g); break;
-    default: lpips_head_backward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, lin, HW, d.W[k], k, train, seed, grad_value, accumulate, g); break;
+  const dim3 grid((unsigned)head_chunks(H, W), (unsigned)B);
+  const int HW = H * W;
+  switch (C) {
+    case 64: lpips_head_backward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
+    case 128: lpips_head_backward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
+    case 256: lpips_head_backward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
+    default: lpips_head_backward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
   }
   LP_LAUNCH_CK("lpips_head_backward_kernel");
+  return 0;
+}
+
+int check_head_args(const char* what, int64_t B, int H, int W, int C, int tap) {
+  if (B < 1 || B > 65535 || H < 1 || W < 1 || H > 32767 || W > 32767 || (C != 64 && C != 128 && C != 256 && C != 512) || tap < 0 ||
+      tap > 4)
+    return dbw_fail_(what, cudaSuccess);
   return 0;
 }
 
@@ -660,7 +668,9 @@ extern "C" int dbw_lpips_forward(const DbwLpipsNet* net, const float* in0, const
     }
   }
   for (int k = 0; k < 5; ++k)
-    if (const int rc = head_forward(k, T[k], out1[LP_TAP_LAYER[k]], net->lin_w[k], d, L, train, seed, ws, st)) return rc;
+    if (const int rc = head_forward(T[k], out1[LP_TAP_LAYER[k]], net->lin_w[k], B, d.H[k], d.W[k], LP_TAP_C[k], k, train, seed,
+                                    ws + L.partials + L.part_off[k], st))
+      return rc;
   PartDesc pd;
   for (int k = 0; k < 5; ++k) { pd.off[k] = L.part_off[k]; pd.chunks[k] = L.chunks[k]; pd.inv_hw[k] = 1.f / (float)(d.H[k] * d.W[k]); }
   lpips_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value, seed, (uint32_t*)(ws + L.seed));
@@ -693,7 +703,8 @@ extern "C" int dbw_lpips_backward(const DbwLpipsNet* net, const float* grad_valu
         if (const int rc = pool_backward(act, G[cur], G[cur ^ 1], B, d.H[lv], d.W[lv], LP_COUT[l], st)) return rc;
         cur ^= 1;
       }
-      if (const int rc = head_backward(lv, ws + L.tap0[lv], act, net->lin_w[lv], d, L, train, seed_used, grad_value, !deepest, G[cur], st))
+      if (const int rc = head_backward(ws + L.tap0[lv], act, net->lin_w[lv], B, d.H[lv], d.W[lv], LP_TAP_C[lv], lv, train, seed_used,
+                                       grad_value, !deepest, G[cur], st))
         return rc;
     }
     // input gradient of layer l; masked by the ReLU below unless a pool sits in between
@@ -741,4 +752,25 @@ extern "C" int dbw_lpips_maxpool_backward(const float* in, const float* gout, fl
   if (B < 1 || H < 1 || W < 1 || C < 4 || C % 4) return dbw_fail_("dbw_lpips_maxpool_backward: bad sizes", cudaSuccess);
   if (!in || !gout || !gin) return dbw_fail_("dbw_lpips_maxpool_backward: null pointer argument", cudaSuccess);
   return pool_backward(in, gout, gin, B, H, W, C, (cudaStream_t)stream);
+}
+
+extern "C" int dbw_lpips_head_forward(const float* f0, const float* f1, const float* lin, int64_t B, int32_t H, int32_t W, int32_t C,
+                                      int32_t tap, int32_t train, const uint32_t* seed, float* partials, void* stream) {
+  if (const int rc = check_head_args("dbw_lpips_head_forward: bad sizes (1 <= B <= 65535, 1 <= H, W <= 32767, C = 64, 128, 256 or "
+                                     "512, 0 <= tap <= 4)", B, H, W, C, tap))
+    return rc;
+  if (!f0 || !f1 || !lin || (train && !seed) || !partials)
+    return dbw_fail_("dbw_lpips_head_forward: null pointer argument", cudaSuccess);
+  return head_forward(f0, f1, lin, B, H, W, C, tap, train, seed, partials, (cudaStream_t)stream);
+}
+
+extern "C" int dbw_lpips_head_backward(const float* f0, const float* f1, const float* lin, int64_t B, int32_t H, int32_t W, int32_t C,
+                                       int32_t tap, int32_t train, const uint32_t* seed, const float* grad_value,
+                                       int32_t accumulate, float* g, void* stream) {
+  if (const int rc = check_head_args("dbw_lpips_head_backward: bad sizes (1 <= B <= 65535, 1 <= H, W <= 32767, C = 64, 128, 256 or "
+                                     "512, 0 <= tap <= 4)", B, H, W, C, tap))
+    return rc;
+  if (!f0 || !f1 || !lin || (train && !seed) || !grad_value || !g)
+    return dbw_fail_("dbw_lpips_head_backward: null pointer argument", cudaSuccess);
+  return head_backward(f0, f1, lin, B, H, W, C, tap, train, seed, grad_value, accumulate, g, (cudaStream_t)stream);
 }

@@ -480,6 +480,23 @@ int dbw_knn_backward(const float* p1, const float* p2, const int64_t* lengths1, 
  * from the workspace of a save_for_backward forward (the same normalize and train; the workspace untouched in between).  Both run on `stream` only: no
  * allocation, no synchronisation (capturable).  The single-layer entry points run the same kernels; dbw_lpips_conv3x3 takes
  * a K-major weight wt[co][(ky*3+kx)*C_in + ci] already TF32-rounded, and optional bias, and mask (out *= [mask > 0]).
+ *
+ * The workspace, in floats, with H_k = H >> k, W_k = W >> k the sizes after k pools and every region starting at a
+ * multiple of 64 floats (its length rounded up to a multiple of 64), in this order:
+ *  - act[l], l = 0..12: rec's activation after layer l's ReLU, NHWC (B, H_k, W_k, C_out[l]) at the layer's level k
+ *    (0,0, 1,1, 2,2,2, 3,3,3, 4,4,4).  Without save_for_backward only the taps l = 1, 3, 6, 9, 12 have a region;
+ *  - tap0[k], k = 0..4: imgs' taps relu1_2 .. relu5_3, NHWC (B, H_k, W_k, C_k), C_k = 64, 128, 256, 512, 512;
+ *  - s0, s1: scratch of B*H*W*64 floats each;
+ *  - the head partials: per tap k in order (not padded between taps), B x ceil(H_k W_k / 64) floats, partial[b][c] the sum
+ *    of the head over pixels 64c .. 64c + 63 of image b (row-major), as dbw_lpips_head_forward writes it;
+ *  - 64 floats whose first holds the uint32 seed the forward used.
+ * value[b] is sum_k (sum_c partial[b][c], in c order) * (1 / (H_k W_k) in fp32), summed over k in order.
+ *
+ * dbw_lpips_head_forward and dbw_lpips_head_backward run one head, as the whole term does, on NHWC features f0 (imgs) and
+ * f1 (rec) of shape (B, H, W, C), C = 64, 128, 256 or 512, with lin (C) and the dropout of tap `tap` (0..4) for the seed
+ * *seed when `train` (without `train`, seed may be NULL).  The forward writes partials (B, ceil(H*W / 64)) as above.  The
+ * backward writes g (B, H, W, C) = (d sum_b grad_value[b] head_b / d f1 + (accumulate ? g : 0)) * [f1 > 0], head_b being the
+ * spatial mean of image b's head.
  */
 typedef struct DbwLpipsNet {
   const float* conv_w[13];
@@ -507,6 +524,11 @@ int dbw_lpips_dgrad_last(const float* g, const float* w, const float* scale, int
 int dbw_lpips_maxpool(const float* in, float* out, int64_t B, int32_t H, int32_t W, int32_t C, void* stream);
 int dbw_lpips_maxpool_backward(const float* in, const float* gout, float* gin, int64_t B, int32_t H, int32_t W, int32_t C,
                                void* stream);
+int dbw_lpips_head_forward(const float* f0, const float* f1, const float* lin, int64_t B, int32_t H, int32_t W, int32_t C,
+                           int32_t tap, int32_t train, const uint32_t* seed, float* partials, void* stream);
+int dbw_lpips_head_backward(const float* f0, const float* f1, const float* lin, int64_t B, int32_t H, int32_t W, int32_t C,
+                            int32_t tap, int32_t train, const uint32_t* seed, const float* grad_value, int32_t accumulate,
+                            float* g, void* stream);
 
 #ifdef __cplusplus
 }

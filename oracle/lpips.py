@@ -38,15 +38,17 @@ def hash_image(seed, tap, image):
     return _fmix(_fmix(s) ^ np.uint32(image))[0]
 
 
-def mask_np(seed, tap, B, C, H, W):
-    """(B,C,H,W) float64 dropout mask of one tap: 2 where the element is kept, 0 where dropped"""
+def mask_np(seed, tap, B, C, H, W, images=None):
+    """(B,C,H,W) float64 dropout mask of one tap: 2 where the element is kept, 0 where dropped; with `images` (indices
+    into the batch), only those images' masks, (len(images),C,H,W)"""
+    images = range(B) if images is None else images
     with np.errstate(over='ignore'):
-        out = np.empty((B, C, H, W))
+        out = np.empty((len(images), C, H, W))
         c = np.arange(C, dtype=np.uint32)[:, None, None]
         yx = (np.arange(H, dtype=np.uint32)[:, None] << np.uint32(16)) | np.arange(W, dtype=np.uint32)[None, :]
-        for b in range(B):
+        for i, b in enumerate(images):
             h = _fmix(_fmix(np.uint32(hash_image(seed, tap, b)) ^ c) ^ yx[None])
-            out[b] = np.where(h < np.uint32(0x80000000), 2.0, 0.0)
+            out[i] = np.where(h < np.uint32(0x80000000), 2.0, 0.0)
     return out
 
 
