@@ -36,7 +36,8 @@ class DbwSceneGeometry(ctypes.Structure):
 
 class DbwLossEpilogue(ctypes.Structure):
     _fields_ = [('env_rgba', ctypes.c_void_p), ('target', ctypes.c_void_p), ('g_env', ctypes.c_void_p), ('rec', ctypes.c_void_p),
-                ('loss_partials', ctypes.c_void_p), ('n_partials', ctypes.c_int32), ('inv_count', ctypes.c_float)]
+                ('loss_partials', ctypes.c_void_p), ('n_partials', ctypes.c_int32), ('inv_count', ctypes.c_float),
+                ('env_alpha_unread', ctypes.c_int32)]
 
 
 class DbwTexJob(ctypes.Structure):
@@ -60,7 +61,7 @@ class DbwMapDesc(ctypes.Structure):
                 ('reserved', ctypes.c_int32)]
 
 
-EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_forward_ex', 'dbw_render_backward',
+EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_forward_ex', 'dbw_render_backward',
            'dbw_render_forward_loss', 'dbw_render_backward_scaled', 'dbw_render_backward_cameras',
            'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_composite_mse', 'dbw_composite_mse_backward', 'dbw_render_forward_host', 'dbw_host_arena_release', 'dbw_launch_count',
@@ -126,6 +127,8 @@ def lib():
         L.dbw_comm_destroy.argtypes = [vp]
         L.dbw_debug_generic_kernel_only.restype = None
         L.dbw_debug_generic_kernel_only.argtypes = [ctypes.c_int]
+        L.dbw_debug_keep_unread_outputs.restype = None
+        L.dbw_debug_keep_unread_outputs.argtypes = [ctypes.c_int]
         L.dbw_texture_prep_forward_multi.argtypes = [ctypes.POINTER(DbwTexJob), ctypes.c_int32, vp]
         L.dbw_texture_prep_backward_multi.argtypes = [ctypes.POINTER(DbwTexJob), ctypes.c_int32, vp]
         L.dbw_timing_enable.restype = None

@@ -59,6 +59,10 @@ static int stride_grid(long long n, int per_sm) {
 static int g_no_hard_kernel = 0;
 // test hook: 1 routes hard single-layer renders through the generic kernel (the two must agree bit for bit)
 extern "C" void dbw_debug_generic_kernel_only(int on) { g_no_hard_kernel = on; }
+static int g_keep_unread = 0;
+// test hook: 1 keeps the outputs no backward reads -- the colour records of a pass without an opacity or distance path, and
+// the alpha plane of a loss epilogue's g_env -- so that a test can compare against the computation that still writes them
+extern "C" void dbw_debug_keep_unread_outputs(int on) { g_keep_unread = on; }
 extern "C" int dbw_abi_version(void) { return DBW_ABI_VERSION; }
 extern "C" size_t dbw_sizeof_settings(void) { return sizeof(DbwRenderSettings); }
 extern "C" const char* dbw_last_error(void) { return g_err; }
@@ -106,6 +110,13 @@ struct Workspace {
   int* cbin_count; int* cbin_list; int cbin_nx, cbin_ny;       // coarse bins (DBW_CBIN x DBW_CBIN pixels): slot lists per (view, bin)
   float4* frag; float4* frag_rgb; unsigned char* nfrag; size_t total;
 };
+// Does the forward keep each fragment's colour?  The backward reads it only for colour . gradient, which feeds nothing but
+// the suffix pass of the opacity and distance gradients.  A single-layer hard pass (sigma = 0: no distance path) whose
+// caller declared it free of opacities (save_fragment_state = 2) has neither.
+static bool keeps_colours(const DbwRenderSettings& s) {
+  if (!s.save_fragment_state) return false;
+  return g_keep_unread || !(s.save_fragment_state == 2 && s.faces_per_pixel == 1 && s.sigma == 0.f);
+}
 static Workspace carve(const DbwRenderSettings& s, void* base) {
   Workspace w; char* p = (char*)base; size_t off = 0;
   const size_t B = s.n_views, V = s.n_verts, S = 2 * (size_t)s.n_faces;
@@ -127,7 +138,8 @@ static Workspace carve(const DbwRenderSettings& s, void* base) {
   w.maps4 = (float4*)(p + off);    off += s.maps_are_texels4 ? 0 : align_up((size_t)(s.n_map_floats / 3) * sizeof(float4));
   const size_t npx = B * (size_t)s.height * s.width;
   w.frag = (float4*)(p + off);     off += s.save_fragment_state ? align_up(npx * (size_t)s.faces_per_pixel * sizeof(float4)) : 0;
-  w.frag_rgb = (float4*)(p + off); off += s.save_fragment_state ? align_up(npx * (size_t)s.faces_per_pixel * sizeof(float4)) : 0;
+  const bool rgb = keeps_colours(s);
+  w.frag_rgb = rgb ? (float4*)(p + off) : nullptr; off += rgb ? align_up(npx * (size_t)s.faces_per_pixel * sizeof(float4)) : 0;
   w.nfrag = (unsigned char*)(p + off); off += s.save_fragment_state ? align_up(npx) : 0;
   w.total = off; return w;
 }
@@ -165,6 +177,7 @@ static int validate(const DbwRenderSettings* s) {
   if (s->n_faces % ag) return fail("n_faces must be a multiple of alpha_group");
   if (s->alpha_view_stride != 0 && s->alpha_view_stride != s->n_faces / ag) return fail("alpha_view_stride must be 0 or n_faces / alpha_group");
   if (s->n_static_faces < 0 || s->n_static_faces > s->n_faces) return fail("n_static_faces out of range [0, n_faces]");
+  if (s->save_fragment_state < 0 || s->save_fragment_state > 2) return fail("save_fragment_state must be 0, 1 or 2");
   if (2 * (long long)s->n_faces > DBW_FRAG_SLOT_MASK) return fail("too many faces: triangle slots are stored in 20 bits");
   if (s->n_maps > DBW_FRAG_MAX_MAPS) return fail("too many texture maps: a fragment's map is stored in 9 bits");
   if (s->sigma < 0.f || s->blur_radius < 0.f) return fail("sigma and blur_radius must be >= 0");
@@ -470,6 +483,7 @@ struct RasterParams {
   // fused compositing + MSE epilogue of the forward (DbwLossEpilogue); ep_target == NULL: plain render
   const float* ep_env; const float* ep_target; float* ep_g_env; float* ep_rec; float* ep_partials;
   float ep_inv_count; int ep_part_mask;
+  int ep_skip_env_alpha;     // DbwLossEpilogue.env_alpha_unread: the alpha plane of ep_g_env is not written
   // the epilogue also differentiates the pass (dbw_render_forward_loss_grad): unscaled gradients into g_tri / g_cells /
   // g_faces_alpha, which then point at the backward scratch
   int ep_grad;
@@ -580,7 +594,7 @@ __device__ __forceinline__ void shade_geometry(const RasterParams& P, int view, 
 #define DBW_BWD_BARY_MINB 4       // backward with the barycentric path: more live state (128 registers)
 #endif
 #ifndef DBW_BWD_GEOM_MINB
-#define DBW_BWD_GEOM_MINB 5       // barycentric path of a single-layer pass alone (raster_bary_backward_kernel, 92 registers)
+#define DBW_BWD_GEOM_MINB 5       // barycentric path of a single-layer pass alone (raster_bary_backward_kernel, 93 registers)
 #endif
 
 // CTA -> (view, tile) mapping of the raster kernels.  CTAs are dispatched in linear grid order, so the grid is laid out as
@@ -831,7 +845,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     if (P.frag) {                 // what the backward streams instead of re-deriving geometry and texels: two 16 B records
       const size_t fi = ((size_t)view * K + k) * plane + pix;
       P.frag[fi] = make_float4(e.y, e.w, v, d0);
-      P.frag_rgb[fi] = make_float4(tx.color.x, tx.color.y, tx.color.z, 0.f);
+      if (P.frag_rgb) P.frag_rgb[fi] = make_float4(tx.color.x, tx.color.y, tx.color.z, 0.f);
     }
     const float w = occ * a;
     r += w * tx.color.x; g += w * tx.color.y; bl += w * tx.color.z;
@@ -867,7 +881,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     }
     ep_g[3] = gm;
     if (P.out_rgba) { o[0] = ep_g[0]; o[plane] = ep_g[1]; o[2 * plane] = ep_g[2]; o[3 * plane] = gm; }
-    ge[3 * plane] = 0.f;
+    if (!P.ep_skip_env_alpha) ge[3 * plane] = 0.f;
   }
   }   // live
   if (EP && P.ep_grad) epilogue_backward(P, lA, lV, NT, s_desc, s_galpha, live, n_saved, p, ep_g, view, lane, warp);
@@ -1014,7 +1028,7 @@ __global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const R
   if (P.frag) {
     const size_t fi = (size_t)view * plane + pix;
     P.frag[fi] = make_float4(__int_as_float(best_slot | (map_id << DBW_FRAG_MAP_SHIFT)), u, v, -1.f);
-    P.frag_rgb[fi] = make_float4(tx.color.x, tx.color.y, tx.color.z, 0.f);
+    if (P.frag_rgb) P.frag_rgb[fi] = make_float4(tx.color.x, tx.color.y, tx.color.z, 0.f);
     P.nfrag[fi] = 1;
   }
   if (P.topk) P.topk[(size_t)view * plane + pix] = best_slot;
@@ -1475,6 +1489,9 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
   const bool alpha_in_smem = want_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX;       // few opacity entries: hot addresses
   if (alpha_in_smem) for (int i = tid; i < P.n_alpha; i += DBW_BWD_NT) s_galpha[i] = 0.f;
   const bool want_dist = P.sigma > 0.f && P.g_tri != nullptr;
+  // d loss / d alpha of the pixel feeds only the suffix pass; without it a zero alpha gradient changes no result (a pixel
+  // whose only non-zero gradient is alpha's contributes zeros), and the plane is not read -- a loss epilogue may not write it
+  const bool want_ga = want_alpha || want_dist;
   const size_t slot_base = (size_t)view * 2 * P.F;
   __syncthreads();
 
@@ -1488,10 +1505,11 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
     if (t < DBW_BWD_TILES && xi < P.W && y < P.H && y >= row_lo && y < row_hi) {
       const size_t px = (size_t)y * P.W + xi;
       const float* go = P.grad_rgba + (size_t)view * 4 * plane + px;
-      f.g0 = go[0]; f.g1 = go[plane]; f.g2 = go[2 * plane]; f.g3 = go[3 * plane];
+      f.g0 = go[0]; f.g1 = go[plane]; f.g2 = go[2 * plane];
+      if (want_ga) f.g3 = go[3 * plane];
       f.n = (int)P.nfrag[(size_t)view * plane + px];
       f.rec = P.frag[(size_t)view * P.K * plane + px];          // speculative: a valid workspace address whether or not a
-      f.rgb = P.frag_rgb[(size_t)view * P.K * plane + px];      // fragment exists
+      if (P.frag_rgb) f.rgb = P.frag_rgb[(size_t)view * P.K * plane + px];      // fragment exists (no colours: see keeps_colours)
     }
   };
   First first_next;
@@ -1615,20 +1633,36 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DBW_BWD_GEOM_MINB) raster_bary_bac
   const float gs = P.grad_scale ? __ldg(P.grad_scale) : 1.f;
   const size_t slot_base = (size_t)view * 2 * P.F;
   __syncthreads();
+  // As in raster_backward_kernel<K1>: each warp walks its patches on its own, and the next patch's fragment count, record and
+  // RGB gradient are in flight while the current one is processed.  The record is loaded whether or not a fragment exists
+  // (a valid workspace address either way), so that the three loads do not wait on each other.
+  struct First { bool n; float4 rec; float g0, g1, g2; };
+  auto load_first = [&](int t, First& f) {
+    f.n = false; f.rec = make_float4(0.f, 0.f, 0.f, 0.f); f.g0 = f.g1 = f.g2 = 0.f;
+    const int y = (strip * DBW_BWD_TILES_K1 + t) * TH + (warp >> 1) * 4 + (lane >> 3);
+    if (t < DBW_BWD_TILES_K1 && xi < P.W && y < P.H && y >= row_lo && y < row_hi) {
+      const size_t px = (size_t)y * P.W + xi;
+      f.n = P.nfrag[(size_t)view * plane + px] != 0;
+      f.rec = P.frag[(size_t)view * plane + px];
+      const float* go = P.grad_rgba + (size_t)view * 4 * plane + px;
+      f.g0 = go[0]; f.g1 = go[plane]; f.g2 = go[2 * plane];
+    }
+  };
+  First first_next;
+  load_first(0, first_next);
   for (int t = 0; t < DBW_BWD_TILES_K1; ++t) {
+    const First first = first_next;
+    load_first(t + 1, first_next);
     const int yi = (strip * DBW_BWD_TILES_K1 + t) * TH + (warp >> 1) * 4 + (lane >> 3);
-    const bool live = xi < P.W && yi < P.H && yi >= row_lo && yi < row_hi;
-    const size_t pix = live ? (size_t)yi * P.W + xi : 0;
     int key = -1, ckey = -1;
     float gv9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float gc9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (live && P.nfrag[(size_t)view * plane + pix]) {
-      const float4 fr = P.frag[(size_t)view * plane + pix];
+    if (first.n) {                  // only a pixel of the call's rows has one (load_first)
+      const float4 fr = first.rec;
       const int bits = __float_as_int(fr.x), slot = bits & DBW_FRAG_SLOT_MASK;
       const int face = slot >= P.F ? slot - P.F : slot;
       if (face >= P.n_static_faces) {
-        const float* go = P.grad_rgba + (size_t)view * 4 * plane + pix;
-        const float gr = go[0] * gs, gg = go[plane] * gs, gb = go[2 * plane] * gs;
+        const float gr = first.g0 * gs, gg = first.g1 * gs, gb = first.g2 * gs;
         const float fa = ALPHA ? __ldg(&P.faces_alpha[alpha_index(P, view, face)]) : 1.f;
         const float w = frag_alpha(fr.w, P.sigma, P.clip_inside) * fa;        // the only layer: occlusion 1
         if (w != 0.f && (gr != 0.f || gg != 0.f || gb != 0.f)) {
@@ -1916,6 +1950,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || (!out_rgba && !eg) || !workspace)
     return fail("dbw_render_forward: null pointer argument");
   if (!s->verts_are_ndc && (!R || !T)) return fail("dbw_render_forward: R and T are required unless verts_are_ndc");
+  if (s->save_fragment_state == 2 && faces_alpha) return fail("dbw_render_forward: save_fragment_state = 2 declares a pass without faces_alpha");
   Workspace w = carve(*s, workspace);
   if (workspace_bytes < w.total) return fail("dbw_render_forward: workspace too small (see dbw_workspace_bytes)");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1952,6 +1987,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
     CK(cudaMemsetAsync(ep->loss_partials, 0, (size_t)ep->n_partials * sizeof(float), st));
     P.ep_env = ep->env_rgba; P.ep_target = ep->target; P.ep_g_env = ep->g_env; P.ep_rec = ep->rec;
     P.ep_partials = ep->loss_partials; P.ep_inv_count = ep->inv_count; P.ep_part_mask = ep->n_partials - 1;
+    P.ep_skip_env_alpha = ep->env_alpha_unread && !g_keep_unread;
   }
   if (eg) {           // the scratch dbw_render_backward_deferred folds: zero-filled here, accumulated by the forward kernel
     const BwdScratch g = carve_bwd(*s, eg->scratch);
@@ -2019,7 +2055,8 @@ extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const 
   (void)topk_ids;          // kept in the signature for ABI continuity: the backward streams the workspace's fragment records
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || !workspace || !grad_rgba || !bwd_scratch)
     return fail("dbw_render_backward: null pointer argument");
-  if (!s_in->save_fragment_state) return fail("dbw_render_backward: the forward must run with save_fragment_state = 1");
+  if (!s_in->save_fragment_state) return fail("dbw_render_backward: the forward must run with save_fragment_state = 1 or 2");
+  if (s_in->save_fragment_state == 2 && faces_alpha) return fail("dbw_render_backward: save_fragment_state = 2 declares a pass without faces_alpha");
   const bool cams = g_R != nullptr || g_T != nullptr;
   if (cams && s_in->verts_are_ndc) return fail("dbw_render_backward_cameras: no camera gradient when verts_are_ndc (R and T are not used)");
   if (cams && (!R || !T)) return fail("dbw_render_backward_cameras: camera gradients need R and T");

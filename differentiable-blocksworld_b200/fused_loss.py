@@ -89,6 +89,9 @@ class _SceneMSEFn(torch.autograd.Function):
         ep.env_rgba, ep.target, ep.g_env = env_rgba.data_ptr(), imgs.data_ptr(), g_env.data_ptr()
         ep.rec = rec.data_ptr() if rec is not None else None
         ep.loss_partials, ep.n_partials, ep.inv_count = partials.data_ptr(), N_PARTIALS, float(inv_count)
+        # the environment renders without opacities; when it is also hard, its backward has neither an opacity nor a distance
+        # path and never reads the alpha plane of g_env (its only reader), so the epilogue does not write it
+        ep.env_alpha_unread = int(cfg_e.sigma == 0.0)
         g_fg = scratch_b = None
         if fused:
             mask = ((GRAD_VERTS if need[2] or need[5] or need[6] else 0) | (GRAD_MAPS if need[3] else 0)

@@ -209,8 +209,10 @@ def scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigm
                         n_map_floats=(maps.numel() // 4 * 3) if maps_are_texels4 else maps.numel(),
                         # 2: float4 maps with cell maps among them (the backward then spreads their gradient over copies)
                         maps_are_texels4=(2 if any(len(e) > 3 and e[3] for e in map_table_host) else 1) if maps_are_texels4 else 0,
-                        # what a backward streams: one 16 B record per kept fragment, written only when one may follow
-                        save_fragment_state=torch.is_grad_enabled(), alpha_group=alpha_group, n_static_faces=n_static_faces,
+                        # what a backward streams, written only when one may follow: records and colours of the kept
+                        # fragments; 2 = a pass without opacities (a hard single-layer one then needs no colours)
+                        save_fragment_state=(1 if faces_alpha is not None else 2) if torch.is_grad_enabled() else 0,
+                        alpha_group=alpha_group, n_static_faces=n_static_faces,
                         view_rows=view_rows)
     return cfg, map_table
 

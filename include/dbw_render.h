@@ -61,9 +61,12 @@ typedef struct DbwRenderSettings {
                                  cell collects the gradient of f x f texels: one copy would serialise the atomics of
                                  every warp that covers it)                                                               */
   int32_t save_fragment_state;/* 1: the forward also keeps one 16 B record {triangle slot | closest edge, u, v, signed squared
-                                 distance} per kept fragment (+ a per-pixel count byte) in its workspace; dbw_render_backward*
-                                 streams these instead of re-deriving geometry and REQUIRES them.  Costs
-                                 B*H*W*(16 K + 1) bytes of workspace ADDRESS space (only fragments that exist are touched)  */
+                                 distance} and one 16 B colour {r, g, b, -} per kept fragment (+ a per-pixel count byte) in its
+                                 workspace; dbw_render_backward* streams these instead of re-deriving geometry and REQUIRES
+                                 them.  Costs B*H*W*(32 K + 1) bytes of workspace ADDRESS space (only fragments that exist are
+                                 touched).  2: the same for a pass without opacities (faces_alpha must then be NULL in the
+                                 forward and the backward); when it is also hard and single-layer (sigma = 0, K = 1) its
+                                 backward has no use for the colours and they are not kept: B*H*W*(16 + 1) bytes            */
   int32_t alpha_group;        /* faces sharing one opacity entry (0/1: one per face).  faces_alpha / g_faces_alpha then have
                                  n_faces / alpha_group entries per view: a DBW block is 80 faces with ONE opacity
                                  (src/model/dbw.py:219 repeat_interleave's it per face; that is alpha_group = 1)            */
@@ -92,6 +95,10 @@ typedef struct DbwMapDesc { int32_t offset, height, width, reserved; } DbwMapDes
 int dbw_abi_version(void);
 /* Test hook: 1 = hard single-layer renders (K = 1, sigma = 0) go through the generic raster kernel instead of their dedicated one. */
 void dbw_debug_generic_kernel_only(int on);
+/* Test hook: 1 = keep writing what no backward reads (the colours of a save_fragment_state = 2 hard single-layer pass, the
+ * alpha plane of an env_alpha_unread epilogue's g_env), for tests that compare against the computation that writes them.  Set it before
+ * dbw_workspace_bytes: it changes the forward workspace's size. */
+void dbw_debug_keep_unread_outputs(int on);
 /* sizeof(DbwRenderSettings) as compiled into the library: lets a binding verify its mirror of the struct. */
 size_t dbw_sizeof_settings(void);
 const char* dbw_last_error(void);
@@ -174,7 +181,7 @@ int dbw_composite_mse_backward(int32_t n_views, int32_t height, int32_t width, c
  * environment and the RGB loss (dbw.py:366-367, nn.MSELoss) done in the rasterizer's epilogue, per pixel, while the blended
  * colour is still in registers:
  *     rec = rgb * a + (1 - a) * rgb_env ;  loss = sum((rec - target)^2) * inv_count
- * Instead of the image, `out_rgba` receives d loss / d (this layer's RGBA) and `g_env` d loss / d env_rgba (alpha plane 0),
+ * Instead of the image, `out_rgba` receives d loss / d (this layer's RGBA) and `g_env` d loss / d env_rgba (alpha plane 0, or unwritten: env_alpha_unread),
  * i.e. exactly the grad_rgba inputs of the two dbw_render_backward calls (scaled there by the upstream gradient of the
  * loss through `grad_scale`): no composite kernel, no image round trip through HBM in either direction.
  */
@@ -186,6 +193,9 @@ typedef struct DbwLossEpilogue {
   float* loss_partials;       /* (n_partials) out: zero-filled by the call, then partial sums; loss = their sum            */
   int32_t n_partials;         /* power of two, >= 1                                                                        */
   float inv_count;            /* weight / (B_total * 3 * H * W): the mean of nn.MSELoss over the GLOBAL batch              */
+  int32_t env_alpha_unread;   /* 1: nothing reads the alpha plane of g_env and it is left unwritten -- the environment's
+                                 backward has no opacity and no distance path (sigma = 0, faces_alpha NULL), and such a
+                                 dbw_render_backward* never reads grad_rgba's alpha plane.  0: the plane is written (zeros) */
 } DbwLossEpilogue;
 
 int dbw_render_forward_loss(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
