@@ -56,6 +56,11 @@ class DbwLpipsNet(ctypes.Structure):
                 ('shift', ctypes.c_void_p), ('scale', ctypes.c_void_p), ('prepared', ctypes.c_void_p)]
 
 
+class DbwLpipsTargetCache(ctypes.Structure):
+    _fields_ = [('arena', ctypes.c_void_p), ('N', ctypes.c_int64), ('H', ctypes.c_int32), ('W', ctypes.c_int32),
+                ('normalize', ctypes.c_int32)]
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -75,7 +80,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_u
            'dbw_knn_forward', 'dbw_knn_backward',
            'dbw_lpips_workspace_bytes', 'dbw_lpips_prepare_weights', 'dbw_lpips_forward', 'dbw_lpips_backward',
            'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward',
-           'dbw_lpips_head_forward', 'dbw_lpips_head_backward']
+           'dbw_lpips_head_forward', 'dbw_lpips_head_backward',
+           'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached']
 
 _lib = None
 
@@ -158,6 +164,11 @@ def lib():
         L.dbw_lpips_maxpool_backward.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp]
         L.dbw_lpips_head_forward.argtypes = [vp] * 3 + [i64] + [i32] * 5 + [vp, vp, vp]
         L.dbw_lpips_head_backward.argtypes = [vp] * 3 + [i64] + [i32] * 5 + [vp, vp, i32, vp, vp]
+        cp = ctypes.POINTER(DbwLpipsTargetCache)
+        L.dbw_lpips_cache_bytes.argtypes = [i32, i32, ctypes.POINTER(sz)]
+        L.dbw_lpips_cache_targets.argtypes = [np_, vp, cp, i64, vp, sz, vp]
+        L.dbw_lpips_forward_cached.argtypes = [np_, cp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+        L.dbw_lpips_backward_cached.argtypes = [np_, cp, vp, vp, i64, i32, i32, i32, i32, vp, vp, sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

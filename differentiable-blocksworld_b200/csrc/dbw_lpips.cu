@@ -20,6 +20,7 @@
 
 #include "../../include/dbw_render.h"
 #include "dbw_lpips_hash.cuh"
+#include "dbw_lpips_cache.cuh"
 
 extern int dbw_fail_(const char* what, cudaError_t e);
 extern void dbw_count_launch_(void);
@@ -122,12 +123,19 @@ __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], 
 
 // out[m][n] = epilogue(sum_k A[m][k] wt[n][k]),  A[m][(ky*3+kx)*Cin + ci] = in[pixel m shifted by (ky-1, kx-1)][ci] (0 off
 // the image); epilogue: + bias[n], ReLU, * [mask[m][n] > 0], each when requested.  M = B*H*W, Cin % 32 == 0, Cout % BN == 0.
-template <int BN>
+// BOUNDED (the target cache's miss chain): only the first *count images are computed, M = min(M, *count H W); the CTAs
+// past them exit at once.  An output row depends on its own image and the weights only, in a K order fixed by Cin, and the
+// tile shape by Cout alone, so a row gives the same bits at any position in any batch.
+template <int BN, bool BOUNDED>
 __global__ void __launch_bounds__(CV_THREADS, 2) lpips_conv3x3_kernel(const float* __restrict__ in, const float* __restrict__ wt,
                                                                       const float* __restrict__ bias, const float* __restrict__ mask,
                                                                       float* __restrict__ out, int M, int H, int W, int Cin,
-                                                                      int Cout, int relu) {
+                                                                      int Cout, int relu, const int* __restrict__ count) {
   using C = CvCfg<BN>;
+  if constexpr (BOUNDED) {
+    M = min(M, *count * H * W);
+    if ((int)blockIdx.x * CV_BM >= M) return;
+  }
   extern __shared__ __align__(16) float smem[];
   float* sA = smem;
   float* sB = smem + CV_STAGES * C::A_FLOATS;
@@ -237,28 +245,33 @@ __global__ void __launch_bounds__(CV_THREADS, 2) lpips_conv3x3_kernel(const floa
 
 // ------------------------------------------------------------------------------------------------ first layer (3 -> 64)
 // 4 threads per pixel, 16 output channels each; fp32 FMA.  x' = normalize ? 2x - 1 : x, then (x' - shift) / scale; the
-// zero padding is of the scaled image
+// zero padding is of the scaled image.  GATHER (the target cache's miss chain): output image s < *count reads image
+// route[s][1] of x
+template <bool GATHER>
 __global__ void __launch_bounds__(256) lpips_conv_first_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                                const float* __restrict__ bias, const float* __restrict__ shift,
                                                                const float* __restrict__ scale, int normalize,
-                                                               float* __restrict__ out, int64_t M, int H, int W) {
+                                                               float* __restrict__ out, int64_t M, int H, int W,
+                                                               const int32_t* __restrict__ route, const int* __restrict__ count) {
   __shared__ float ws[27][64];       // [(ci*3+ky)*3+kx][co]
   __shared__ float bs[64];
   for (int i = threadIdx.x; i < 27 * 64; i += blockDim.x) ws[i % 27][i / 27] = w[i];
   if (threadIdx.x < 64) bs[threadIdx.x] = bias[threadIdx.x];
   __syncthreads();
   const int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if constexpr (GATHER) M = min(M, (int64_t)*count * H * W);
   if (q >= 4 * M) return;
   const int64_t m = q >> 2;
   const int cg = (int)(q & 3) * 16;
   const int64_t HW = (int64_t)H * W, b = m / HW;
+  const int64_t bx = GATHER ? (int64_t)route[2 * b + 1] : b;
   const int rem = (int)(m - b * HW), y = rem / W, xx = rem - (rem / W) * W;
   float acc[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) acc[j] = bs[cg + j];
   for (int ci = 0; ci < 3; ++ci) {
     const float sh = shift[ci], sc = scale[ci];
-    const float* plane = x + (b * 3 + ci) * HW;
+    const float* plane = x + (bx * 3 + ci) * HW;
 #pragma unroll
     for (int ky = 0; ky < 3; ++ky)
 #pragma unroll
@@ -324,10 +337,14 @@ __global__ void __launch_bounds__(256) lpips_dgrad_last_kernel(const float* __re
 }
 
 // ------------------------------------------------------------------------------------------------ max-pool 2x2, stride 2, floor
-__global__ void lpips_pool_kernel(const float4* __restrict__ in, float4* __restrict__ out, int64_t n_out, int H, int W, int C4) {
+// BOUNDED: only the first *count images
+template <bool BOUNDED>
+__global__ void lpips_pool_kernel(const float4* __restrict__ in, float4* __restrict__ out, int64_t n_out, int H, int W, int C4,
+                                  const int* __restrict__ count) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n_out) return;
   const int OH = H / 2, OW = W / 2;
+  if constexpr (BOUNDED) n_out = min(n_out, (int64_t)*count * OH * OW * C4);
+  if (i >= n_out) return;
   const int c = (int)(i % C4);
   const int64_t p = i / C4;
   const int ox = (int)(p % OW), oy = (int)((p / OW) % OH);
@@ -373,11 +390,20 @@ __device__ __forceinline__ float warp_sum0(float v) {      // lane 0's tree sum,
   return __shfl_sync(0xffffffffu, v, 0);
 }
 
+// ROUTED (the target cache): image b's f0 is entry route[b][0] of cache_f0 for a hit (>= 0), else miss slot
+// -(route[b][0] + 1) of f0.  The dropout stays keyed on b.
 template <int C>
+__device__ __forceinline__ const float* routed_f0(const float* f0, const float* cache_f0, const int32_t* route, int b, int HW) {
+  const int r = route[2 * b];
+  return r >= 0 ? cache_f0 + (int64_t)r * HW * C : f0 + (int64_t)(-r - 1) * HW * C;
+}
+
+template <int C, bool ROUTED>
 __global__ void __launch_bounds__(256) lpips_head_forward_kernel(const float* __restrict__ f0, const float* __restrict__ f1,
                                                                  const float* __restrict__ lin, int HW, int W, int tap, int train,
                                                                  const uint32_t* __restrict__ seed, float* __restrict__ partials,
-                                                                 int n_chunks) {
+                                                                 int n_chunks, const int32_t* __restrict__ route,
+                                                                 const float* __restrict__ cache_f0) {
   constexpr int NPL = C / 32;
   __shared__ float wsum[8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, b = blockIdx.y;
@@ -385,15 +411,16 @@ __global__ void __launch_bounds__(256) lpips_head_forward_kernel(const float* __
 #pragma unroll
   for (int j = 0; j < NPL; ++j) wl[j] = lin[lane + 32 * j];
   const uint32_t himg = train ? dbw_lpips_hash_image(*seed, (uint32_t)tap, (uint32_t)b) : 0u;
+  const float* f0b = ROUTED ? routed_f0<C>(f0, cache_f0, route, b, HW) : f0;
   float acc = 0.f;
   for (int s = 0; s < HEAD_PIX / 8; ++s) {
     const int p = blockIdx.x * HEAD_PIX + warp * (HEAD_PIX / 8) + s;
     if (p >= HW) break;
-    const int64_t base = ((int64_t)b * HW + p) * C;
+    const int64_t base = ((int64_t)b * HW + p) * C, base0 = ROUTED ? (int64_t)p * C : base;
     float u0[NPL], u1[NPL], s0 = 0.f, s1 = 0.f;
 #pragma unroll
     for (int j = 0; j < NPL; ++j) {
-      u0[j] = f0[base + lane + 32 * j]; u1[j] = f1[base + lane + 32 * j];
+      u0[j] = f0b[base0 + lane + 32 * j]; u1[j] = f1[base + lane + 32 * j];
       s0 = fmaf(u0[j], u0[j], s0); s1 = fmaf(u1[j], u1[j], s1);
     }
     const float d0 = __fsqrt_rn(warp_sum0(s0)) + LP_EPS, d1 = __fsqrt_rn(warp_sum0(s1)) + LP_EPS;
@@ -419,12 +446,13 @@ __global__ void __launch_bounds__(256) lpips_head_forward_kernel(const float* __
 }
 
 // g <- (d value / d f1 + (accumulate ? g : 0)) * [f1 > 0]; d value / d f1 is scaled by grad_value[b] / HW
-template <int C>
+template <int C, bool ROUTED>
 __global__ void __launch_bounds__(256) lpips_head_backward_kernel(const float* __restrict__ f0, const float* __restrict__ f1,
                                                                   const float* __restrict__ lin, int HW, int W, int tap, int train,
                                                                   const uint32_t* __restrict__ seed,
                                                                   const float* __restrict__ grad_value, int accumulate,
-                                                                  float* __restrict__ g) {
+                                                                  float* __restrict__ g, const int32_t* __restrict__ route,
+                                                                  const float* __restrict__ cache_f0) {
   constexpr int NPL = C / 32;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, b = blockIdx.y;
   const float gs = __fdiv_rn(grad_value[b], (float)HW);
@@ -432,14 +460,15 @@ __global__ void __launch_bounds__(256) lpips_head_backward_kernel(const float* _
 #pragma unroll
   for (int j = 0; j < NPL; ++j) wl[j] = lin[lane + 32 * j] * gs;
   const uint32_t himg = train ? dbw_lpips_hash_image(*seed, (uint32_t)tap, (uint32_t)b) : 0u;
+  const float* f0b = ROUTED ? routed_f0<C>(f0, cache_f0, route, b, HW) : f0;
   for (int s = 0; s < HEAD_PIX / 8; ++s) {
     const int p = blockIdx.x * HEAD_PIX + warp * (HEAD_PIX / 8) + s;
     if (p >= HW) break;
-    const int64_t base = ((int64_t)b * HW + p) * C;
+    const int64_t base = ((int64_t)b * HW + p) * C, base0 = ROUTED ? (int64_t)p * C : base;
     float u0[NPL], u1[NPL], s0 = 0.f, s1 = 0.f;
 #pragma unroll
     for (int j = 0; j < NPL; ++j) {
-      u0[j] = f0[base + lane + 32 * j]; u1[j] = f1[base + lane + 32 * j];
+      u0[j] = f0b[base0 + lane + 32 * j]; u1[j] = f1[base + lane + 32 * j];
       s0 = fmaf(u0[j], u0[j], s0); s1 = fmaf(u1[j], u1[j], s1);
     }
     const float r1 = __fsqrt_rn(warp_sum0(s1));
@@ -494,36 +523,130 @@ __global__ void lpips_prepare_kernel(const float* __restrict__ w, float* __restr
   bwd[((int64_t)ci * 9 + (8 - tap)) * Cout + co] = v;           // (2-ky)*3 + (2-kx) = 8 - tap
 }
 
+// ------------------------------------------------------------------------------------------------ target cache
+constexpr int FP_CHUNKS = 32;                // fingerprint partials per image
+constexpr int LOOKUP_THREADS = 512;
+
+// part[b][blockIdx.x] = this CTA's share of the fingerprint of image b (n floats each) of x
+__global__ void __launch_bounds__(256) lpips_fingerprint_kernel(const float* __restrict__ x, int64_t n, uint64_t* __restrict__ part) {
+  __shared__ uint64_t wsum[8];
+  const int64_t b = blockIdx.y;
+  const uint32_t* u = reinterpret_cast<const uint32_t*>(x) + b * n;
+  uint64_t s = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    s += dbw_lpips_fp_term((uint64_t)i, u[i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint64_t t = 0;
+    for (int w = 0; w < 8; ++w) t += wsum[w];
+    part[b * FP_CHUNKS + blockIdx.x] = t;
+  }
+}
+
+__global__ void lpips_fingerprint_sum_kernel(const uint64_t* __restrict__ part, int64_t N, uint64_t* __restrict__ fp) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= N) return;
+  uint64_t t = 0;
+  for (int c = 0; c < FP_CHUNKS; ++c) t += part[e * FP_CHUNKS + c];
+  fp[e] = t;
+}
+
+// one CTA per image b of x: route[b][1] = the first cache entry whose fingerprint matches and whose stored image is the same
+// bit for bit, or -1
+__global__ void __launch_bounds__(LOOKUP_THREADS) lpips_lookup_kernel(const float* __restrict__ x, int64_t n,
+                                                                      const uint64_t* __restrict__ part,
+                                                                      const uint64_t* __restrict__ cache_fp,
+                                                                      const float* __restrict__ cache_img, int64_t N,
+                                                                      int32_t* __restrict__ route) {
+  __shared__ uint64_t fp;
+  const int64_t b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    uint64_t t = 0;
+    for (int c = 0; c < FP_CHUNKS; ++c) t += part[b * FP_CHUNKS + c];
+    fp = t;
+  }
+  __syncthreads();
+  const uint32_t* u = reinterpret_cast<const uint32_t*>(x) + b * n;
+  auto same_image = [&](int64_t e) {
+    const uint32_t* v = reinterpret_cast<const uint32_t*>(cache_img) + e * n;
+    int diff = 0;
+    for (int64_t i = threadIdx.x; i < n && !diff; i += blockDim.x) diff = u[i] != v[i];
+    return !__syncthreads_or(diff);
+  };
+  const int hit = dbw_lpips_find(fp, cache_fp, N, same_image);
+  if (threadIdx.x == 0) route[2 * b + 1] = hit;
+}
+
+__global__ void lpips_route_kernel(int32_t* __restrict__ route, int64_t B, int* __restrict__ n_miss, int32_t* __restrict__ n_hits) {
+  if (threadIdx.x != 0) return;
+  const int m = dbw_lpips_route(route, B);
+  *n_miss = m;
+  if (n_hits) *n_hits = (int32_t)(B - m);
+}
+
+// the arena, in floats: tap[k] (N, H_k W_k, C_k) for k = 0..4, the N uint64 fingerprints, the N images (N, 3, H, W).  Every
+// tap holds a multiple of 64 floats per image, so an arena of N images is N times the bytes of one.
+struct CacheLayout { int64_t tap[5], fp, img, total; };
+
+CacheLayout cache_layout_of(int64_t N, int H, int W) {
+  const Dims d = dims_of(1, H, W);
+  CacheLayout C; int64_t o = 0;
+  for (int k = 0; k < 5; ++k) { C.tap[k] = o; o += N * d.H[k] * d.W[k] * LP_TAP_C[k]; }
+  C.fp = o; o += 2 * N;
+  C.img = o; o += N * 3 * (int64_t)H * W;
+  C.total = o;
+  return C;
+}
+
 // ------------------------------------------------------------------------------------------------ launchers
 // the dynamic shared-memory limit is a per-device attribute: set before every launch (cheap), as the raster kernels do
+template <bool BOUNDED>
 int set_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(lpips_conv3x3_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, CvCfg<128>::SMEM);
+  cudaError_t e = cudaFuncSetAttribute(lpips_conv3x3_kernel<128, BOUNDED>, cudaFuncAttributeMaxDynamicSharedMemorySize, CvCfg<128>::SMEM);
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(lpips_conv3x3_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, CvCfg<64>::SMEM);
+    e = cudaFuncSetAttribute(lpips_conv3x3_kernel<64, BOUNDED>, cudaFuncAttributeMaxDynamicSharedMemorySize, CvCfg<64>::SMEM);
   if (e != cudaSuccess) return dbw_fail_("lpips: cudaFuncSetAttribute", e);
   return 0;
 }
 
-int conv3x3(const float* in, const float* wt, const float* bias, const float* mask, float* out, int64_t B, int H, int W, int Cin,
-            int Cout, int relu, cudaStream_t st) {
-  if (const int rc = set_attrs()) return rc;
+// count: NULL, or the device count of images to compute (the grid still covers B)
+template <bool BOUNDED>
+int conv3x3_launch(const float* in, const float* wt, const float* bias, const float* mask, float* out, int64_t B, int H, int W, int Cin,
+                   int Cout, int relu, const int* count, cudaStream_t st) {
+  if (const int rc = set_attrs<BOUNDED>()) return rc;
   const int64_t M = B * H * W;
   if (M == 0) return 0;
   if (Cout == 64) {
     const dim3 grid((unsigned)((M + CV_BM - 1) / CV_BM), (unsigned)(Cout / 64));
-    lpips_conv3x3_kernel<64><<<grid, CV_THREADS, CvCfg<64>::SMEM, st>>>(in, wt, bias, mask, out, (int)M, H, W, Cin, Cout, relu);
+    lpips_conv3x3_kernel<64, BOUNDED><<<grid, CV_THREADS, CvCfg<64>::SMEM, st>>>(in, wt, bias, mask, out, (int)M, H, W, Cin, Cout, relu,
+                                                                                 count);
   } else {
     const dim3 grid((unsigned)((M + CV_BM - 1) / CV_BM), (unsigned)(Cout / 128));
-    lpips_conv3x3_kernel<128><<<grid, CV_THREADS, CvCfg<128>::SMEM, st>>>(in, wt, bias, mask, out, (int)M, H, W, Cin, Cout, relu);
+    lpips_conv3x3_kernel<128, BOUNDED><<<grid, CV_THREADS, CvCfg<128>::SMEM, st>>>(in, wt, bias, mask, out, (int)M, H, W, Cin, Cout,
+                                                                                   relu, count);
   }
   LP_LAUNCH_CK("lpips_conv3x3_kernel");
   return 0;
 }
 
+int conv3x3(const float* in, const float* wt, const float* bias, const float* mask, float* out, int64_t B, int H, int W, int Cin,
+            int Cout, int relu, cudaStream_t st, const int* count = nullptr) {
+  return count ? conv3x3_launch<true>(in, wt, bias, mask, out, B, H, W, Cin, Cout, relu, count, st)
+               : conv3x3_launch<false>(in, wt, bias, mask, out, B, H, W, Cin, Cout, relu, nullptr, st);
+}
+
+// route, count: NULL, or the miss chain's gather (output image s < *count reads image route[s][1] of x)
 int conv_first(const float* x, const float* w, const float* bias, const float* shift, const float* scale, int normalize, float* out,
-               int64_t B, int H, int W, cudaStream_t st) {
+               int64_t B, int H, int W, cudaStream_t st, const int32_t* route = nullptr, const int* count = nullptr) {
   const int64_t M = B * H * W;
-  lpips_conv_first_kernel<<<(unsigned)((4 * M + 255) / 256), 256, 0, st>>>(x, w, bias, shift, scale, normalize, out, M, H, W);
+  const unsigned grid = (unsigned)((4 * M + 255) / 256);
+  if (count)
+    lpips_conv_first_kernel<true><<<grid, 256, 0, st>>>(x, w, bias, shift, scale, normalize, out, M, H, W, route, count);
+  else
+    lpips_conv_first_kernel<false><<<grid, 256, 0, st>>>(x, w, bias, shift, scale, normalize, out, M, H, W, nullptr, nullptr);
   LP_LAUNCH_CK("lpips_conv_first_kernel");
   return 0;
 }
@@ -536,10 +659,14 @@ int dgrad_last(const float* gz, const float* w, const float* scale, int normaliz
   return 0;
 }
 
-int pool(const float* in, float* out, int64_t B, int H, int W, int C, cudaStream_t st) {
+int pool(const float* in, float* out, int64_t B, int H, int W, int C, cudaStream_t st, const int* count = nullptr) {
   const int64_t n = B * (H / 2) * (W / 2) * (C / 4);
   if (n == 0) return 0;
-  lpips_pool_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const float4*)in, (float4*)out, n, H, W, C / 4);
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  if (count)
+    lpips_pool_kernel<true><<<grid, 256, 0, st>>>((const float4*)in, (float4*)out, n, H, W, C / 4, count);
+  else
+    lpips_pool_kernel<false><<<grid, 256, 0, st>>>((const float4*)in, (float4*)out, n, H, W, C / 4, nullptr);
   LP_LAUNCH_CK("lpips_pool_kernel");
   return 0;
 }
@@ -553,31 +680,53 @@ int pool_backward(const float* in, const float* gout, float* gin, int64_t B, int
   return 0;
 }
 
-// partials (B, head_chunks(H, W)); C is one of 64, 128, 256, 512
+template <int C>
+void head_forward_c(dim3 grid, const float* f0, const float* f1, const float* lin, int HW, int W, int tap, int train,
+                    const uint32_t* seed, float* part, int n, const int32_t* route, const float* cache_f0, cudaStream_t st) {
+  if (route)
+    lpips_head_forward_kernel<C, true><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n, route, cache_f0);
+  else
+    lpips_head_forward_kernel<C, false><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n, nullptr, nullptr);
+}
+
+// partials (B, head_chunks(H, W)); C is one of 64, 128, 256, 512.  route, cache_f0: NULL, or image b's f0 per route[b][0]
 int head_forward(const float* f0, const float* f1, const float* lin, int64_t B, int H, int W, int C, int tap, int train,
-                 const uint32_t* seed, float* part, cudaStream_t st) {
+                 const uint32_t* seed, float* part, cudaStream_t st, const int32_t* route = nullptr, const float* cache_f0 = nullptr) {
   const int n = (int)head_chunks(H, W);
   const dim3 grid((unsigned)n, (unsigned)B);
   const int HW = H * W;
   switch (C) {
-    case 64: lpips_head_forward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
-    case 128: lpips_head_forward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
-    case 256: lpips_head_forward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
-    default: lpips_head_forward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, part, n); break;
+    case 64: head_forward_c<64>(grid, f0, f1, lin, HW, W, tap, train, seed, part, n, route, cache_f0, st); break;
+    case 128: head_forward_c<128>(grid, f0, f1, lin, HW, W, tap, train, seed, part, n, route, cache_f0, st); break;
+    case 256: head_forward_c<256>(grid, f0, f1, lin, HW, W, tap, train, seed, part, n, route, cache_f0, st); break;
+    default: head_forward_c<512>(grid, f0, f1, lin, HW, W, tap, train, seed, part, n, route, cache_f0, st); break;
   }
   LP_LAUNCH_CK("lpips_head_forward_kernel");
   return 0;
 }
 
+template <int C>
+void head_backward_c(dim3 grid, const float* f0, const float* f1, const float* lin, int HW, int W, int tap, int train,
+                     const uint32_t* seed, const float* grad_value, int accumulate, float* g, const int32_t* route,
+                     const float* cache_f0, cudaStream_t st) {
+  if (route)
+    lpips_head_backward_kernel<C, true><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g, route,
+                                                              cache_f0);
+  else
+    lpips_head_backward_kernel<C, false><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g,
+                                                               nullptr, nullptr);
+}
+
 int head_backward(const float* f0, const float* f1, const float* lin, int64_t B, int H, int W, int C, int tap, int train,
-                  const uint32_t* seed, const float* grad_value, int accumulate, float* g, cudaStream_t st) {
+                  const uint32_t* seed, const float* grad_value, int accumulate, float* g, cudaStream_t st,
+                  const int32_t* route = nullptr, const float* cache_f0 = nullptr) {
   const dim3 grid((unsigned)head_chunks(H, W), (unsigned)B);
   const int HW = H * W;
   switch (C) {
-    case 64: lpips_head_backward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
-    case 128: lpips_head_backward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
-    case 256: lpips_head_backward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
-    default: lpips_head_backward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g); break;
+    case 64: head_backward_c<64>(grid, f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g, route, cache_f0, st); break;
+    case 128: head_backward_c<128>(grid, f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g, route, cache_f0, st); break;
+    case 256: head_backward_c<256>(grid, f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g, route, cache_f0, st); break;
+    default: head_backward_c<512>(grid, f0, f1, lin, HW, W, tap, train, seed, grad_value, accumulate, g, route, cache_f0, st); break;
   }
   LP_LAUNCH_CK("lpips_head_backward_kernel");
   return 0;
@@ -602,6 +751,131 @@ bool net_ok(const DbwLpipsNet* net) {
   for (int l = 0; l < LP_LAYERS; ++l) if (!net->conv_w[l] || !net->conv_b[l]) return false;
   for (int k = 0; k < 5; ++k) if (!net->lin_w[k]) return false;
   return true;
+}
+
+// the 13 layers of one image batch x: out[l] receives layer l's activation (pool outputs go to S0).  With route and count
+// (the miss chain), only the images of route[s][1] for slots s < *count, compacted in slot order.
+int trunk(const DbwLpipsNet* net, const float* x, float* const* out, float* S0, const Dims& d, int normalize, cudaStream_t st,
+          const int32_t* route = nullptr, const int* count = nullptr) {
+  const float* prep = (const float*)net->prepared;
+  const int64_t B = d.B;
+  if (const int rc = conv_first(x, net->conv_w[0], net->conv_b[0], net->shift, net->scale, normalize, out[0], B, d.H[0], d.W[0], st,
+                                route, count))
+    return rc;
+  const float* cur = out[0];
+  for (int l = 1; l < LP_LAYERS; ++l) {
+    const int lv = LP_LEVEL[l];
+    if (lv != LP_LEVEL[l - 1]) {
+      if (const int rc = pool(cur, S0, B, d.H[lv - 1], d.W[lv - 1], LP_CIN[l], st, count)) return rc;
+      cur = S0;
+    }
+    if (const int rc = conv3x3(cur, prep + wfwd_off(l), net->conv_b[l], nullptr, out[l], B, d.H[lv], d.W[lv], LP_CIN[l], LP_COUT[l], 1,
+                               st, count))
+      return rc;
+    cur = out[l];
+  }
+  return 0;
+}
+
+// imgs keeps only its taps: the other layers alternate between the scratch tensors (pool outputs go to S0)
+void imgs_outputs(float* S0, float* S1, float* const* T, float** out) {
+  float* o[LP_LAYERS] = {S1, T[0], S1, T[1], S1, S0, T[2], S1, S0, T[3], S1, S0, T[4]};
+  for (int l = 0; l < LP_LAYERS; ++l) out[l] = o[l];
+}
+
+bool cache_ok(const DbwLpipsTargetCache* c) { return c && c->arena && c->N >= 1 && c->N < ((int64_t)1 << 31); }
+
+// the whole forward; cache: NULL, or the target cache (route and n_hits as dbw_lpips_forward_cached takes them)
+int forward_impl(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const float* in0, const float* in1, int64_t B, int H, int W,
+                 int normalize, int train, int save_for_backward, uint32_t* seed, float* value, int32_t* route, int32_t* n_hits,
+                 void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const Dims d = dims_of(B, H, W);
+  const bool save = save_for_backward != 0;
+  const Layout L = layout_of(d, save);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_forward: workspace too small", cudaSuccess);
+  float* ws = (float*)workspace;
+  float *S0 = ws + L.s0, *S1 = ws + L.s1, *T[5];
+  for (int k = 0; k < 5; ++k) T[k] = ws + L.tap0[k];
+  float* out0[LP_LAYERS];
+  imgs_outputs(S0, S1, T, out0);
+  // rec keeps every activation for the backward, or like imgs only its taps
+  float* out1[LP_LAYERS];
+  for (int l = 0; l < LP_LAYERS; ++l) out1[l] = L.act[l] >= 0 ? ws + L.act[l] : out0[l];
+  const float* cache_tap[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+  if (cache) {
+    // look imgs up (fingerprint partials in S1, the miss count beside the seed), then run its chain over the misses only:
+    // their taps land in the first n_miss images of tap0
+    const CacheLayout C = cache_layout_of(cache->N, H, W);
+    const float* arena = (const float*)cache->arena;
+    for (int k = 0; k < 5; ++k) cache_tap[k] = arena + C.tap[k];
+    const int64_t n = 3 * (int64_t)H * W;
+    uint64_t* part = (uint64_t*)S1;
+    int* n_miss = (int*)(ws + L.seed) + 1;
+    lpips_fingerprint_kernel<<<dim3(FP_CHUNKS, (unsigned)B), 256, 0, st>>>(in0, n, part);
+    LP_LAUNCH_CK("lpips_fingerprint_kernel");
+    lpips_lookup_kernel<<<(unsigned)B, LOOKUP_THREADS, 0, st>>>(in0, n, part, (const uint64_t*)(arena + C.fp), arena + C.img, cache->N,
+                                                                route);
+    LP_LAUNCH_CK("lpips_lookup_kernel");
+    lpips_route_kernel<<<1, 32, 0, st>>>(route, B, n_miss, n_hits);
+    LP_LAUNCH_CK("lpips_route_kernel");
+    if (const int rc = trunk(net, in0, out0, S0, d, normalize, st, route, n_miss)) return rc;
+  } else if (const int rc = trunk(net, in0, out0, S0, d, normalize, st)) {
+    return rc;
+  }
+  if (const int rc = trunk(net, in1, out1, S0, d, normalize, st)) return rc;
+  for (int k = 0; k < 5; ++k)
+    if (const int rc = head_forward(T[k], out1[LP_TAP_LAYER[k]], net->lin_w[k], B, d.H[k], d.W[k], LP_TAP_C[k], k, train, seed,
+                                    ws + L.partials + L.part_off[k], st, cache ? route : nullptr, cache_tap[k]))
+      return rc;
+  PartDesc pd;
+  for (int k = 0; k < 5; ++k) { pd.off[k] = L.part_off[k]; pd.chunks[k] = L.chunks[k]; pd.inv_hw[k] = 1.f / (float)(d.H[k] * d.W[k]); }
+  lpips_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value, seed, (uint32_t*)(ws + L.seed));
+  LP_LAUNCH_CK("lpips_reduce_kernel");
+  return 0;
+}
+
+int backward_impl(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const int32_t* route, const float* grad_value, int64_t B,
+                  int H, int W, int normalize, int train, float* grad_in1, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const Dims d = dims_of(B, H, W);
+  const Layout L = layout_of(d, true);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_backward: workspace too small", cudaSuccess);
+  float* ws = (float*)workspace;
+  const float* prep = (const float*)net->prepared;
+  const uint32_t* seed_used = (const uint32_t*)(ws + L.seed);
+  const float* cache_tap[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+  if (cache) {
+    const CacheLayout C = cache_layout_of(cache->N, H, W);
+    for (int k = 0; k < 5; ++k) cache_tap[k] = (const float*)cache->arena + C.tap[k];
+  }
+  float* G[2] = {ws + L.s0, ws + L.s1};
+  int cur = 0;                        // G[cur] holds the gradient at the pre-activation of layer l
+  for (int l = LP_LAYERS - 1; l >= 1; --l) {
+    const int lv = LP_LEVEL[l];
+    const float* act = ws + L.act[l];
+    if (l == LP_TAP_LAYER[lv]) {
+      const bool deepest = lv == 4;
+      if (!deepest) {                 // G[cur] holds the gradient at the next pool's output: route it back to this tap
+        if (const int rc = pool_backward(act, G[cur], G[cur ^ 1], B, d.H[lv], d.W[lv], LP_COUT[l], st)) return rc;
+        cur ^= 1;
+      }
+      if (const int rc = head_backward(ws + L.tap0[lv], act, net->lin_w[lv], B, d.H[lv], d.W[lv], LP_TAP_C[lv], lv, train, seed_used,
+                                       grad_value, !deepest, G[cur], st, cache ? route : nullptr, cache_tap[lv]))
+        return rc;
+    }
+    // input gradient of layer l; masked by the ReLU below unless a pool sits in between
+    const bool after_pool = LP_LEVEL[l - 1] != lv;
+    if (const int rc = conv3x3(G[cur], prep + wbwd_off(l), nullptr, after_pool ? nullptr : ws + L.act[l - 1], G[cur ^ 1], B,
+                               d.H[lv], d.W[lv], LP_COUT[l], LP_CIN[l], 0, st))
+      return rc;
+    cur ^= 1;
+  }
+  return dgrad_last(G[cur], net->conv_w[0], net->scale, normalize, grad_in1, B, H, W, st);
+}
+
+int check_cache(const char* what, const DbwLpipsTargetCache* cache, int H, int W, int normalize) {
+  if (!cache_ok(cache)) return dbw_fail_(what, cudaSuccess);
+  if (cache->H != H || cache->W != W || (cache->normalize != 0) != (normalize != 0)) return dbw_fail_(what, cudaSuccess);
+  return 0;
 }
 
 }  // namespace
@@ -637,45 +911,8 @@ extern "C" int dbw_lpips_forward(const DbwLpipsNet* net, const float* in0, const
     return rc;
   if (!net_ok(net) || !in0 || !in1 || !seed || !value || !workspace)
     return dbw_fail_("dbw_lpips_forward: null pointer argument", cudaSuccess);
-  const Dims d = dims_of(B, H, W);
-  const bool save = save_for_backward != 0;
-  const Layout L = layout_of(d, save);
-  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_forward: workspace too small", cudaSuccess);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* ws = (float*)workspace;
-  const float* prep = (const float*)net->prepared;
-  float *S0 = ws + L.s0, *S1 = ws + L.s1, *T[5];
-  for (int k = 0; k < 5; ++k) T[k] = ws + L.tap0[k];
-  // imgs keeps only its taps: the other layers alternate between the scratch tensors (pool outputs go to S0)
-  float* out0[LP_LAYERS] = {S1, T[0], S1, T[1], S1, S0, T[2], S1, S0, T[3], S1, S0, T[4]};
-  // rec keeps every activation for the backward, or like imgs only its taps
-  float* out1[LP_LAYERS];
-  for (int l = 0; l < LP_LAYERS; ++l) out1[l] = L.act[l] >= 0 ? ws + L.act[l] : out0[l];
-  for (int img = 0; img < 2; ++img) {
-    float* const* out = img ? out1 : out0;
-    if (const int rc = conv_first(img ? in1 : in0, net->conv_w[0], net->conv_b[0], net->shift, net->scale, normalize, out[0], B, H, W, st))
-      return rc;
-    const float* cur = out[0];
-    for (int l = 1; l < LP_LAYERS; ++l) {
-      const int lv = LP_LEVEL[l];
-      if (lv != LP_LEVEL[l - 1]) {
-        if (const int rc = pool(cur, S0, B, d.H[lv - 1], d.W[lv - 1], LP_CIN[l], st)) return rc;
-        cur = S0;
-      }
-      if (const int rc = conv3x3(cur, prep + wfwd_off(l), net->conv_b[l], nullptr, out[l], B, d.H[lv], d.W[lv], LP_CIN[l], LP_COUT[l], 1, st))
-        return rc;
-      cur = out[l];
-    }
-  }
-  for (int k = 0; k < 5; ++k)
-    if (const int rc = head_forward(T[k], out1[LP_TAP_LAYER[k]], net->lin_w[k], B, d.H[k], d.W[k], LP_TAP_C[k], k, train, seed,
-                                    ws + L.partials + L.part_off[k], st))
-      return rc;
-  PartDesc pd;
-  for (int k = 0; k < 5; ++k) { pd.off[k] = L.part_off[k]; pd.chunks[k] = L.chunks[k]; pd.inv_hw[k] = 1.f / (float)(d.H[k] * d.W[k]); }
-  lpips_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value, seed, (uint32_t*)(ws + L.seed));
-  LP_LAUNCH_CK("lpips_reduce_kernel");
-  return 0;
+  return forward_impl(net, nullptr, in0, in1, B, H, W, normalize, train, save_for_backward, seed, value, nullptr, nullptr, workspace,
+                      workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int dbw_lpips_backward(const DbwLpipsNet* net, const float* grad_value, int64_t B, int32_t H, int32_t W,
@@ -685,36 +922,84 @@ extern "C" int dbw_lpips_backward(const DbwLpipsNet* net, const float* grad_valu
     return rc;
   if (!net_ok(net) || !grad_value || !grad_in1 || !workspace)
     return dbw_fail_("dbw_lpips_backward: null pointer argument", cudaSuccess);
-  const Dims d = dims_of(B, H, W);
-  const Layout L = layout_of(d, true);
-  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_backward: workspace too small", cudaSuccess);
+  return backward_impl(net, nullptr, nullptr, grad_value, B, H, W, normalize, train, grad_in1, workspace, workspace_bytes,
+                       (cudaStream_t)stream);
+}
+
+extern "C" int dbw_lpips_cache_bytes(int32_t H, int32_t W, size_t* bytes_per_image) {
+  if (const int rc = check_dims("dbw_lpips_cache_bytes: bad sizes (16 <= H, W <= 32767)", 1, H, W)) return rc;
+  if (!bytes_per_image) return dbw_fail_("dbw_lpips_cache_bytes: null pointer argument", cudaSuccess);
+  *bytes_per_image = (size_t)cache_layout_of(1, H, W).total * 4;
+  return 0;
+}
+
+extern "C" int dbw_lpips_cache_targets(const DbwLpipsNet* net, const float* imgs, const DbwLpipsTargetCache* cache, int64_t chunk,
+                                       void* workspace, size_t workspace_bytes, void* stream) {
+  if (!cache) return dbw_fail_("dbw_lpips_cache_targets: null pointer argument", cudaSuccess);
+  if (const int rc = check_dims("dbw_lpips_cache_targets: bad sizes (1 <= chunk <= 65535, 16 <= H, W <= 32767, chunk*H*W < 2^31 - 128)",
+                                chunk, cache->H, cache->W))
+    return rc;
+  if (!net_ok(net) || !imgs || !cache_ok(cache) || !workspace)
+    return dbw_fail_("dbw_lpips_cache_targets: null pointer argument or bad cache (arena, 1 <= N < 2^31)", cudaSuccess);
+  const int H = cache->H, W = cache->W;
+  const Layout L = layout_of(dims_of(chunk, H, W), false);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_cache_targets: workspace too small", cudaSuccess);
   cudaStream_t st = (cudaStream_t)stream;
+  const CacheLayout C = cache_layout_of(cache->N, H, W);
+  float* arena = (float*)cache->arena;
   float* ws = (float*)workspace;
-  const float* prep = (const float*)net->prepared;
-  const uint32_t* seed_used = (const uint32_t*)(ws + L.seed);
-  float* G[2] = {ws + L.s0, ws + L.s1};
-  int cur = 0;                        // G[cur] holds the gradient at the pre-activation of layer l
-  for (int l = LP_LAYERS - 1; l >= 1; --l) {
-    const int lv = LP_LEVEL[l];
-    const float* act = ws + L.act[l];
-    if (l == LP_TAP_LAYER[lv]) {
-      const bool deepest = lv == 4;
-      if (!deepest) {                 // G[cur] holds the gradient at the next pool's output: route it back to this tap
-        if (const int rc = pool_backward(act, G[cur], G[cur ^ 1], B, d.H[lv], d.W[lv], LP_COUT[l], st)) return rc;
-        cur ^= 1;
-      }
-      if (const int rc = head_backward(ws + L.tap0[lv], act, net->lin_w[lv], B, d.H[lv], d.W[lv], LP_TAP_C[lv], lv, train, seed_used,
-                                       grad_value, !deepest, G[cur], st))
-        return rc;
-    }
-    // input gradient of layer l; masked by the ReLU below unless a pool sits in between
-    const bool after_pool = LP_LEVEL[l - 1] != lv;
-    if (const int rc = conv3x3(G[cur], prep + wbwd_off(l), nullptr, after_pool ? nullptr : ws + L.act[l - 1], G[cur ^ 1], B,
-                               d.H[lv], d.W[lv], LP_COUT[l], LP_CIN[l], 0, st))
-      return rc;
-    cur ^= 1;
+  const int64_t n = 3 * (int64_t)H * W;
+  float* img = arena + C.img;
+  cudaError_t e = cudaMemcpyAsync(img, imgs, (size_t)(cache->N * n) * 4, cudaMemcpyDeviceToDevice, st);
+  if (e != cudaSuccess) return dbw_fail_("dbw_lpips_cache_targets: cudaMemcpyAsync", e);
+  // chunk by chunk: the fingerprints (partials in S1), then the taps straight into the arena, by the kernels (and so to the
+  // bits) of the per-call forward
+  for (int64_t n0 = 0; n0 < cache->N; n0 += chunk) {
+    const int64_t nb = cache->N - n0 < chunk ? cache->N - n0 : chunk;
+    const Dims d = dims_of(nb, H, W);
+    uint64_t* part = (uint64_t*)(ws + L.s1);
+    lpips_fingerprint_kernel<<<dim3(FP_CHUNKS, (unsigned)nb), 256, 0, st>>>(img + n0 * n, n, part);
+    LP_LAUNCH_CK("lpips_fingerprint_kernel");
+    lpips_fingerprint_sum_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, st>>>(part, nb, (uint64_t*)(arena + C.fp) + n0);
+    LP_LAUNCH_CK("lpips_fingerprint_sum_kernel");
+    float* T[5];
+    for (int k = 0; k < 5; ++k) T[k] = arena + C.tap[k] + n0 * d.H[k] * d.W[k] * LP_TAP_C[k];
+    float* out[LP_LAYERS];
+    imgs_outputs(ws + L.s0, ws + L.s1, T, out);
+    if (const int rc = trunk(net, img + n0 * n, out, ws + L.s0, d, cache->normalize, st)) return rc;
   }
-  return dgrad_last(G[cur], net->conv_w[0], net->scale, normalize, grad_in1, B, H, W, st);
+  return 0;
+}
+
+extern "C" int dbw_lpips_forward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const float* in0, const float* in1,
+                                        int64_t B, int32_t H, int32_t W, int32_t normalize, int32_t train, int32_t save_for_backward,
+                                        uint32_t* seed, float* value, int32_t* route, int32_t* n_hits, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+  if (const int rc = check_dims("dbw_lpips_forward_cached: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B,
+                                H, W))
+    return rc;
+  if (!net_ok(net) || !in0 || !in1 || !seed || !value || !route || !workspace)
+    return dbw_fail_("dbw_lpips_forward_cached: null pointer argument", cudaSuccess);
+  if (const int rc = check_cache("dbw_lpips_forward_cached: bad cache (NULL arena, N < 1, or another H, W or normalize)", cache, H, W,
+                                 normalize))
+    return rc;
+  return forward_impl(net, cache, in0, in1, B, H, W, normalize, train, save_for_backward, seed, value, route, n_hits, workspace,
+                      workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int dbw_lpips_backward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const int32_t* route,
+                                         const float* grad_value, int64_t B, int32_t H, int32_t W, int32_t normalize, int32_t train,
+                                         float* grad_in1, void* workspace, size_t workspace_bytes, void* stream) {
+  if (const int rc = check_dims("dbw_lpips_backward_cached: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B,
+                                H, W))
+    return rc;
+  if (!net_ok(net) || !route || !grad_value || !grad_in1 || !workspace)
+    return dbw_fail_("dbw_lpips_backward_cached: null pointer argument", cudaSuccess);
+  if (const int rc = check_cache("dbw_lpips_backward_cached: bad cache (NULL arena, N < 1, or another H, W or normalize)", cache, H, W,
+                                 normalize))
+    return rc;
+  return backward_impl(net, cache, route, grad_value, B, H, W, normalize, train, grad_in1, workspace, workspace_bytes,
+                       (cudaStream_t)stream);
 }
 
 // single layers, for tests and per-layer timing (scripts/bench_lpips.py)

@@ -199,6 +199,26 @@ class DifferentiableBlocksWorld(nn.Module):
             del self.perceptual_loss
         self.perceptual_loss = fn
 
+    def cache_perceptual_targets(self, imgs_or_dataset):
+        """register the training images with the installed PerceptualTerm(perceptual.LPIPS): later steps read their LPIPS
+        taps from a device cache instead of recomputing them, with the same results bit for bit (images not in the cache
+        are computed as before).  imgs_or_dataset: an (N,3,H,W) tensor, or an iterable of (3,H,W) / (B,3,H,W) tensors or
+        of dicts holding them under 'imgs' (the reference's datasets).  Returns the cache's device bytes.  A GraphedStep
+        captured before this call keeps computing its targets: build the step after registering."""
+        from .perceptual import LPIPS
+        term = getattr(self, 'perceptual_loss', None)
+        net = getattr(term, 'loss', None)
+        if not (isinstance(term, PerceptualTerm) and isinstance(net, LPIPS)):
+            raise TypeError('cache_perceptual_targets: the installed perceptual term is not PerceptualTerm(dbw_b200.perceptual.LPIPS) '
+                            f'(got {type(term).__name__}); install one with set_perceptual_loss()')
+        if torch.is_tensor(imgs_or_dataset):
+            imgs = imgs_or_dataset
+        else:
+            items = [x['imgs'] if isinstance(x, dict) else x for x in imgs_or_dataset]
+            imgs = torch.cat([x.detach().reshape(-1, *x.shape[-3:]).to(net.scaling_layer.shift.device) for x in items])
+        net.cache_targets(imgs.detach().to(net.scaling_layer.shift.device), normalize=True)
+        return net.target_cache_bytes(imgs.shape[-2], imgs.shape[-1], len(imgs))
+
     def set_cur_epoch(self, epoch):
         self.cur_epoch = epoch
 

@@ -14,7 +14,13 @@ the module's `training` flag, as in the reference (trainer.py calls model.train(
 (image, tap, channel, pixel) element is kept with probability 1/2 and doubled, by a counter-based hash of a seed held in
 a device buffer that the forward advances (csrc/dbw_lpips_hash.cuh; not torch's dropout stream).  The 64..512-channel
 convolutions take TF32 operands and accumulate in fp32, as the reference's cuDNN convolutions do under torch 1.12's
-default allow_tf32.  Gradients flow to `in1` only; CUDA float32 tensors only (no CPU fallback)."""
+default allow_tf32.  Gradients flow to `in1` only; CUDA float32 tensors only (no CPU fallback).
+
+Target cache (opt in): `cache_targets(imgs)` computes the taps of fixed `in0` images (a scene's training views) once;
+every later forward looks each `in0` image up on the device (a fingerprint, confirmed by comparing the whole image bit for
+bit) and runs the VGG16 trunk of `in0` over the misses only.  Results are the uncached ones bit for bit, hits or not; the
+caller never says which view is which.  A forward uses the cache when its `normalize` and (H, W) are the cache's; any
+change of the weights drops it."""
 import ctypes
 from collections import OrderedDict
 
@@ -88,29 +94,53 @@ class _Vgg(nn.Module):
 
 class _LpipsFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, in0, in1, mod, normalize, train, save):
+    def forward(ctx, in0, in1, mod, normalize, train, save, cache):
         B, _, H, W = in1.shape
         net = mod._net_struct()
         ws_bytes = mod._bytes(B, H, W, save)[0]
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=in1.device)
         value = torch.empty(B, dtype=torch.float32, device=in1.device)
-        check(_lib.lib().dbw_lpips_forward(ctypes.byref(net), _vp(in0), _vp(in1), B, H, W, int(normalize), int(train),
-                                           int(save), _vp(mod.seed), _vp(value), _vp(ws), ws_bytes, _stream(in1.device)), 'dbw_lpips_forward')
-        ctx.mod, ctx.flags = mod, (int(normalize), int(train))
-        ctx.save_for_backward(ws)
+        if cache is None:
+            route = torch.empty(0, dtype=torch.int32, device=in1.device)
+            check(_lib.lib().dbw_lpips_forward(ctypes.byref(net), _vp(in0), _vp(in1), B, H, W, int(normalize), int(train), int(save),
+                                               _vp(mod.seed), _vp(value), _vp(ws), ws_bytes, _stream(in1.device)), 'dbw_lpips_forward')
+        else:
+            route = torch.empty(B, 2, dtype=torch.int32, device=in1.device)
+            check(_lib.lib().dbw_lpips_forward_cached(ctypes.byref(net), ctypes.byref(cache.desc), _vp(in0), _vp(in1), B, H, W,
+                                                      int(normalize), int(train), int(save), _vp(mod.seed), _vp(value), _vp(route),
+                                                      _vp(cache.hits), _vp(ws), ws_bytes, _stream(in1.device)),
+                  'dbw_lpips_forward_cached')
+        # the cache object holds the arena the backward reads, even if the module's cache is replaced in between
+        ctx.mod, ctx.flags, ctx.cache = mod, (int(normalize), int(train)), cache
+        ctx.save_for_backward(ws, route)
         ctx.shape = in1.shape
         return value.view(B, 1, 1, 1)
 
     @staticmethod
     def backward(ctx, grad_value):
-        (ws,) = ctx.saved_tensors
+        ws, route = ctx.saved_tensors
         B, _, H, W = ctx.shape
         g = grad_value.reshape(B).to(torch.float32).contiguous()
         grad = torch.empty(ctx.shape, dtype=torch.float32, device=ws.device)
         net = ctx.mod._net_struct()
-        check(_lib.lib().dbw_lpips_backward(ctypes.byref(net), _vp(g), B, H, W, ctx.flags[0], ctx.flags[1], _vp(grad), _vp(ws),
-                                            ws.numel(), _stream(ws.device)), 'dbw_lpips_backward')
-        return None, grad, None, None, None, None
+        if ctx.cache is None:
+            check(_lib.lib().dbw_lpips_backward(ctypes.byref(net), _vp(g), B, H, W, ctx.flags[0], ctx.flags[1], _vp(grad), _vp(ws),
+                                                ws.numel(), _stream(ws.device)), 'dbw_lpips_backward')
+        else:
+            check(_lib.lib().dbw_lpips_backward_cached(ctypes.byref(net), ctypes.byref(ctx.cache.desc), _vp(route), _vp(g), B, H, W,
+                                                       ctx.flags[0], ctx.flags[1], _vp(grad), _vp(ws), ws.numel(),
+                                                       _stream(ws.device)), 'dbw_lpips_backward_cached')
+        return None, grad, None, None, None, None, None
+
+
+class _TargetCache:
+    """a registered target cache: the arena (device bytes), its C descriptor, the weights key it was computed with, and
+    `hits`, a device int32 (1,) the cached forwards write their hit count to"""
+
+    def __init__(self, arena, N, H, W, normalize, key):
+        self.arena, self.N, self.H, self.W, self.normalize, self.key = arena, N, H, W, bool(normalize), key
+        self.desc = _lib.DbwLpipsTargetCache(arena.data_ptr(), N, H, W, int(normalize))
+        self.hits = torch.zeros(1, dtype=torch.int32, device=arena.device)
 
 
 def _vp(t):
@@ -139,6 +169,7 @@ class LPIPS(nn.Module):
         self.register_buffer('seed', torch.zeros(1, dtype=torch.int32), persistent=False)
         self.register_buffer('prepared', torch.zeros(0), persistent=False)
         self._prepared_key = None
+        self._target_cache = None
 
     # ------------------------------------------------------------------ construction
     @classmethod
@@ -224,6 +255,57 @@ class LPIPS(nn.Module):
               'dbw_lpips_prepare_weights')
         self._prepared_key = key
 
+    # ------------------------------------------------------------------ target cache
+    def target_cache_bytes(self, H, W, N=1):
+        """device bytes of a target cache of N images of H x W: their five taps in fp32, a copy of each image and its
+        fingerprint (about 59.9 MB per 300x400 image, 221 MB per 576x768 one)"""
+        b = ctypes.c_size_t(0)
+        check(_lib.lib().dbw_lpips_cache_bytes(H, W, ctypes.byref(b)), 'dbw_lpips_cache_bytes')
+        return N * b.value
+
+    def cache_targets(self, imgs, normalize=True, chunk=8):
+        """register (N,3,H,W) CUDA float32 target images, replacing any previous cache: later forwards with the same
+        `normalize` and (H, W) read the taps of any `in0` image equal to one of them, bit for bit, from the cache instead of
+        recomputing them.  `chunk` images are computed at a time.  A CUDA graph captured before this call keeps computing
+        its targets, and one captured with a cache must be captured again after the cache is replaced or cleared."""
+        if not (torch.is_tensor(imgs) and imgs.is_cuda and imgs.dtype == torch.float32 and imgs.dim() == 4 and imgs.shape[1] == 3):
+            raise DbwError(f'LPIPS.cache_targets: expected (N,3,H,W) CUDA float32 images, got '
+                           f'{tuple(imgs.shape) if torch.is_tensor(imgs) else type(imgs).__name__}')
+        N, _, H, W = imgs.shape
+        if N < 1 or min(H, W) < 16:
+            raise DbwError(f'LPIPS.cache_targets: need N >= 1 and H, W >= 16, got {tuple(imgs.shape)}')
+        self.clear_target_cache()
+        self._prepare()
+        dev = self.prepared.device
+        imgs = imgs.detach().to(dev).contiguous()
+        cache = _TargetCache(torch.empty(self.target_cache_bytes(H, W, N), dtype=torch.uint8, device=dev), N, H, W, normalize,
+                             self._prepared_key)
+        c = max(1, min(N, int(chunk)))
+        ws = torch.empty(self._bytes(c, H, W, False)[0], dtype=torch.uint8, device=dev)
+        check(_lib.lib().dbw_lpips_cache_targets(ctypes.byref(self._net_struct()), _vp(imgs), ctypes.byref(cache.desc), c, _vp(ws),
+                                                 ws.numel(), _stream(dev)), 'dbw_lpips_cache_targets')
+        self._target_cache = cache
+
+    def clear_target_cache(self):
+        """drop the target cache (its device memory is freed once no pending backward holds it)"""
+        self._target_cache = None
+
+    @property
+    def target_hits(self):
+        """device int32 (1,): the hit count of the last forward that used the cache (None without a cache); not synchronised"""
+        return self._target_cache.hits if self._target_cache is not None else None
+
+    def _usable_cache(self, in0, normalize):
+        c = self._target_cache
+        if c is None:
+            return None
+        if c.key != self._prepared_key:          # the weights changed since registration: never serve stale taps
+            self._target_cache = None
+            return None
+        if c.normalize != bool(normalize) or (c.H, c.W) != tuple(in0.shape[2:]) or c.arena.device != in0.device:
+            return None
+        return c
+
     def forward(self, in0, in1, normalize=False):
         if in0.requires_grad:
             raise DbwError('LPIPS: in0 requires a gradient; only in1 (the rendering) is differentiated')
@@ -238,4 +320,5 @@ class LPIPS(nn.Module):
         self._prepare()
         # rec's activations are kept only when a backward can follow (not under no_grad, as in quantitative_eval)
         save = torch.is_grad_enabled() and in1.requires_grad
-        return _LpipsFunction.apply(in0.contiguous(), in1.contiguous(), self, bool(normalize), bool(self.training), save)
+        return _LpipsFunction.apply(in0.contiguous(), in1.contiguous(), self, bool(normalize), bool(self.training), save,
+                                    self._usable_cache(in0, normalize))

@@ -499,7 +499,8 @@ int dbw_knn_backward(const float* p1, const float* p2, const int64_t* lengths1, 
  *  - s0, s1: scratch of B*H*W*64 floats each;
  *  - the head partials: per tap k in order (not padded between taps), B x ceil(H_k W_k / 64) floats, partial[b][c] the sum
  *    of the head over pixels 64c .. 64c + 63 of image b (row-major), as dbw_lpips_head_forward writes it;
- *  - 64 floats whose first holds the uint32 seed the forward used.
+ *  - 64 floats whose first holds the uint32 seed the forward used (dbw_lpips_forward_cached keeps its int32 miss count in
+ *    the second).
  * value[b] is sum_k (sum_c partial[b][c], in c order) * (1 / (H_k W_k) in fp32), summed over k in order.
  *
  * dbw_lpips_head_forward and dbw_lpips_head_backward run one head, as the whole term does, on NHWC features f0 (imgs) and
@@ -539,6 +540,47 @@ int dbw_lpips_head_forward(const float* f0, const float* f1, const float* lin, i
 int dbw_lpips_head_backward(const float* f0, const float* f1, const float* lin, int64_t B, int32_t H, int32_t W, int32_t C,
                             int32_t tap, int32_t train, const uint32_t* seed, const float* grad_value, int32_t accumulate,
                             float* g, void* stream);
+
+/*
+ * LPIPS target cache: the taps of fixed in0 images (a scene's training views) computed once and read by every later call,
+ * with the same results bit for bit.  The caller owns the arena, dbw_lpips_cache_bytes(H, W) per image times N bytes,
+ * device memory with 256-byte alignment, laid out in floats as:
+ *  - tap[k], k = 0..4: the taps relu1_2 .. relu5_3 of the N images, NHWC (N, H_k, W_k, C_k), as tap0[k] of the workspace;
+ *  - N uint64 fingerprints (csrc/dbw_lpips_cache.cuh);
+ *  - a copy of the N images (N, 3, H, W).
+ * The taps are those of the per-call forward to the bit: every convolution row depends only on its own image and the
+ * weights, its tile shape only on C_out and its K order only on C_in, whatever the batch and the image's place in it.
+ *
+ * dbw_lpips_cache_targets fills the arena of `cache` from imgs (N, 3, H, W) for cache->normalize, `chunk` images at a time,
+ * in a workspace of dbw_lpips_workspace_bytes(chunk, H, W, 0) bytes.  It uses the prepared weights: register again (or
+ * drop the cache) whenever the weights change.
+ *
+ * dbw_lpips_forward_cached is dbw_lpips_forward with in0 looked up in the cache: each image's fingerprint selects the
+ * entries with the same fingerprint, and the first whose stored image is equal bit for bit is a hit.  It writes route
+ * (B, 2) int32: route[b][0] = the entry of a hit, or -(s + 1) for miss slot s (misses numbered in b order); route[s][1] =
+ * the image of miss slot s (-1 past the misses).  The conv chain of in0 runs over the misses only (every kernel bounded by
+ * the device miss count, kept in the second float of the workspace's seed region), their taps in the first slots of tap0;
+ * the heads read f0 per route, the dropout keyed on b as always.  n_hits (optional, one int32) receives the hit count.
+ * dbw_lpips_backward_cached is dbw_lpips_backward with the route and cache of that forward.  Both need the cache's H, W and
+ * normalize equal to the call's, run on `stream` only and are capturable: a captured call looks its inputs up on every
+ * replay.  The workspace is that of dbw_lpips_workspace_bytes.
+ */
+typedef struct DbwLpipsTargetCache {
+  void* arena;
+  int64_t N;
+  int32_t H, W;
+  int32_t normalize;
+} DbwLpipsTargetCache;
+
+int dbw_lpips_cache_bytes(int32_t H, int32_t W, size_t* bytes_per_image);
+int dbw_lpips_cache_targets(const DbwLpipsNet* net, const float* imgs, const DbwLpipsTargetCache* cache, int64_t chunk, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int dbw_lpips_forward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const float* in0, const float* in1, int64_t B,
+                             int32_t H, int32_t W, int32_t normalize, int32_t train, int32_t save_for_backward, uint32_t* seed,
+                             float* value, int32_t* route, int32_t* n_hits, void* workspace, size_t workspace_bytes, void* stream);
+int dbw_lpips_backward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const int32_t* route, const float* grad_value,
+                              int64_t B, int32_t H, int32_t W, int32_t normalize, int32_t train, float* grad_in1, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
