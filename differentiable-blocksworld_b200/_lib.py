@@ -7,7 +7,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DBW_RENDER_LIB: explicit path of another build of the same library (kernel experiments); never a fallback
 LIB_PATH = os.environ.get('DBW_RENDER_LIB') or os.path.join(_HERE, 'libdbw_render.so')
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class DbwRenderSettings(ctypes.Structure):
@@ -66,14 +66,11 @@ class DbwMapDesc(ctypes.Structure):
                 ('reserved', ctypes.c_int32)]
 
 
-EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_forward_ex', 'dbw_render_backward',
-           'dbw_render_forward_loss', 'dbw_render_backward_scaled', 'dbw_render_backward_cameras',
-           'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
+EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
+           'dbw_render_forward_loss', 'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_composite_mse', 'dbw_composite_mse_backward', 'dbw_render_forward_host', 'dbw_host_arena_release', 'dbw_launch_count',
-           'dbw_timing_enable', 'dbw_timing_read', 'dbw_timing_reset', 'dbw_scene_geometry_forward',
-           'dbw_scene_geometry_backward', 'dbw_scene_geometry_forward_env', 'dbw_scene_geometry_backward_parts',
-           'dbw_opacity_forward', 'dbw_opacity_backward', 'dbw_texture_prep_forward', 'dbw_texture_prep_backward',
-           'dbw_texture_prep_forward_multi', 'dbw_texture_prep_backward_multi',
+           'dbw_timing_enable', 'dbw_timing_read', 'dbw_timing_reset', 'dbw_scene_geometry_forward', 'dbw_scene_geometry_backward',
+           'dbw_opacity_forward', 'dbw_opacity_backward', 'dbw_texture_prep_forward_multi', 'dbw_texture_prep_backward_multi',
            'dbw_comm_create', 'dbw_comm_buffer', 'dbw_comm_ipc_handle', 'dbw_comm_connect', 'dbw_comm_all_reduce', 'dbw_comm_error', 'dbw_comm_destroy',
            'dbw_eval_sample_setup', 'dbw_eval_sample_count', 'dbw_eval_sample_write', 'dbw_eval_cell_keys',
            'dbw_eval_cell_ranges', 'dbw_eval_downsample_workspace_bytes', 'dbw_eval_radius_downsample', 'dbw_eval_nn_distance',
@@ -103,12 +100,9 @@ def lib():
         L.dbw_last_error.restype = ctypes.c_char_p
         L.dbw_launch_count.restype = ctypes.c_uint64
         L.dbw_workspace_bytes.argtypes = [ctypes.POINTER(DbwRenderSettings), ctypes.POINTER(sz), ctypes.POINTER(sz)]
-        L.dbw_render_forward.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, vp]
-        L.dbw_render_forward_ex.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, vp, vp, vp]
-        L.dbw_render_backward.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [sz] + [vp] * 5 + [sz, vp]
+        L.dbw_render_forward.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, vp, vp, vp]
+        L.dbw_render_backward.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz] + [vp] * 8 + [sz, vp]
         L.dbw_render_forward_loss.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, ctypes.POINTER(DbwLossEpilogue), vp]
-        L.dbw_render_backward_scaled.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [sz] + [vp] * 6 + [sz, vp]
-        L.dbw_render_backward_cameras.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [sz] + [vp] * 8 + [sz, vp]
         L.dbw_render_forward_loss_grad.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz, ctypes.POINTER(DbwLossEpilogue),
                                                                                                ctypes.c_int32, vp, sz, vp]
         L.dbw_render_backward_deferred.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 7 + [sz, vp]
@@ -116,14 +110,10 @@ def lib():
         L.dbw_composite_mse_backward.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
         L.dbw_render_forward_host.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 6
         L.dbw_host_arena_release.restype = None
-        L.dbw_scene_geometry_forward.argtypes = [ctypes.POINTER(DbwSceneGeometry), vp, vp]
-        L.dbw_scene_geometry_backward.argtypes = [ctypes.POINTER(DbwSceneGeometry)] + [vp] * 8
-        L.dbw_scene_geometry_forward_env.argtypes = [ctypes.POINTER(DbwSceneGeometry), vp, ctypes.c_int32, vp, vp]
-        L.dbw_scene_geometry_backward_parts.argtypes = [ctypes.POINTER(DbwSceneGeometry)] + [vp] * 9
+        L.dbw_scene_geometry_forward.argtypes = [ctypes.POINTER(DbwSceneGeometry), vp, ctypes.c_int32, vp, vp]
+        L.dbw_scene_geometry_backward.argtypes = [ctypes.POINTER(DbwSceneGeometry)] + [vp] * 9
         L.dbw_opacity_forward.argtypes = [vp, vp, ctypes.c_float, ctypes.c_float, vp, ctypes.c_int32, ctypes.c_int32, vp, vp, vp, vp]
         L.dbw_opacity_backward.argtypes = [vp, vp, ctypes.c_float, ctypes.c_float, vp, vp, ctypes.c_int32, vp, vp]
-        L.dbw_texture_prep_forward.argtypes = [vp] + [ctypes.c_int32] * 5 + [vp, vp]
-        L.dbw_texture_prep_backward.argtypes = [vp] + [ctypes.c_int32] * 5 + [vp, vp, vp]
         L.dbw_comm_create.argtypes = [ctypes.c_int32, ctypes.c_int32, sz, ctypes.POINTER(vp)]
         L.dbw_comm_buffer.argtypes = [vp, ctypes.POINTER(vp)]
         L.dbw_comm_ipc_handle.argtypes = [vp, vp]

@@ -1074,45 +1074,8 @@ __device__ __forceinline__ float warp_sum_spread(float (&x)[NP], int lane) {
 template <int N> struct Pow2Ceil { static constexpr int v = N <= 1 ? 1 : N <= 2 ? 2 : N <= 4 ? 4 : N <= 8 ? 8 : N <= 16 ? 16 : 32; };
 template <int NP> struct SpreadShift { static constexpr int v = NP == 1 ? 5 : NP == 2 ? 4 : NP == 4 ? 3 : NP == 8 ? 2 : NP == 16 ? 1 : 0; };
 
-// Group sums through the integer reduction unit (REDUX, sm_80+): the members of a group (`grp`, all executing this) scale
-// their N values by a common power of two derived from the group's largest magnitude, round to int32 (|x| < 2^25, so 32
-// addends cannot overflow), add them with one REDUX.SUM per value and scale back.  Quantisation: 2^-25 of the group's largest
-// magnitude per addend -- the size of fp32 summation rounding -- and the sum itself is exact and order-independent.
-// One instruction per value instead of a shuffle butterfly.  Returns the sums to every member.
-template <int N>
-__device__ __forceinline__ void group_sum_redux(unsigned grp, const float (&v)[N], float (&out)[N]) {
-  float mx = 0.f;
-#pragma unroll
-  for (int i = 0; i < N; ++i) mx = fmaxf(mx, fabsf(v[i]));
-  const unsigned gmax = __reduce_max_sync(grp, __float_as_uint(mx));        // non-negative floats order like their bit patterns
-  int ex = (int)(gmax >> 23) - 127;
-  ex = ex < -100 ? -100 : ex;
-  const float scale = __int_as_float((127 + 24 - ex) << 23), inv = __int_as_float((127 - 24 + ex) << 23);
-#pragma unroll
-  for (int i = 0; i < N; ++i) out[i] = (float)__reduce_add_sync(grp, __float2int_rn(v[i] * scale)) * inv;
-}
-
 template <int N>
 __device__ __forceinline__ void warp_agg_add(float* __restrict__ dst, int stride, int key, const float (&v)[N], int lane) {
-#ifdef DBW_AGG_REDUX
-  unsigned todo_r = __ballot_sync(0xffffffffu, key >= 0);
-  while (todo_r) {
-    const int leader = __ffs(todo_r) - 1;
-    const int lk = __shfl_sync(0xffffffffu, key, leader);
-    const bool mine = (key == lk);
-    const unsigned grp = __ballot_sync(0xffffffffu, mine);
-    if (mine) {
-      float r[N];
-      group_sum_redux<N>(grp, v, r);
-      if (lane == leader) {
-#pragma unroll
-        for (int i = 0; i < N; ++i) if (r[i] != 0.f) atomicAdd(dst + (size_t)lk * stride + i, r[i]);
-      }
-    }
-    todo_r &= ~grp;
-  }
-  return;
-#endif
   constexpr int NP = Pow2Ceil<N>::v, SH = SpreadShift<NP>::v;
   unsigned todo = __ballot_sync(0xffffffffu, key >= 0);
   while (todo) {
@@ -1263,29 +1226,6 @@ __device__ __forceinline__ void warp_agg_add1(float* __restrict__ dst, int key, 
 // Distance-path vertex gradient of one layer, keyed by (triangle slot, closest edge): 4 values = (x, y) of the edge's two
 // vertices.  Vertex pair of the edge: 0 = (v0, v1), 1 = (v0, v2), 2 = (v1, v2); vertex j's (x, y) live at floats 3j, 3j+1.
 __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int key, const float (&v)[4], int lane) {
-#ifdef DBW_AGG_REDUX
-  unsigned todo = __ballot_sync(0xffffffffu, key >= 0);
-  while (todo) {
-    const int leader = __ffs(todo) - 1;
-    const int lk = __shfl_sync(0xffffffffu, key, leader);
-    const bool mine = (key == lk);
-    const unsigned grp = __ballot_sync(0xffffffffu, mine);
-    const int edge = lk & 3;
-    const int ia = edge == 2 ? 3 : 0, ib = edge == 0 ? 3 : 6;
-    float* d = g_tri + (size_t)(lk >> 2) * 9;
-    if (mine) {
-      float r[4];
-      group_sum_redux<4>(grp, v, r);
-      if (lane == leader) {
-        if (r[0] != 0.f) atomicAdd(d + ia, r[0]);
-        if (r[1] != 0.f) atomicAdd(d + ia + 1, r[1]);
-        if (r[2] != 0.f) atomicAdd(d + ib, r[2]);
-        if (r[3] != 0.f) atomicAdd(d + ib + 1, r[3]);
-      }
-    }
-    todo &= ~grp;
-  }
-#else
   // A patch's halo fragments of one layer lie along many edges, mostly one or two lanes per (slot, edge): every lane adds
   // its four values with plain atomics, all in the same pass.  Finding the groups first and reducing them one after the
   // other (a ballot, a shuffle and a ballot per group before any atomic) cost more than the atomics it saved: on an H100
@@ -1300,7 +1240,6 @@ __device__ __forceinline__ void warp_agg_add_edge(float* __restrict__ g_tri, int
     if (v[2] != 0.f) atomicAdd(d + ib, v[2]);
     if (v[3] != 0.f) atomicAdd(d + ib + 1, v[3]);
   }
-#endif
 }
 
 // Barycentric-path gradient of one fragment with colour gradient (gcx, gcy, gcz): colour -> (ix, iy) -> (u, v) ->
@@ -1885,14 +1824,6 @@ static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st) {
   return P.ep_target ? go(raster_forward_kernel<NT, true>) : go(raster_forward_kernel<NT, false>);
 }
 
-extern "C" int dbw_render_forward(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
-                                  const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
-                                  const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
-                                  size_t workspace_bytes, void* stream) {
-  return dbw_render_forward_ex(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, out_rgba, topk_ids,
-                               workspace, workspace_bytes, nullptr, nullptr, stream);
-}
-
 // the backward scratch and the gradients a loss-epilogue forward computes itself (dbw_render_forward_loss_grad)
 struct EpilogueGrad { void* scratch; size_t scratch_bytes; int32_t mask; };
 static int render_forward_impl(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
@@ -1901,22 +1832,31 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
                                void* stream, const EpilogueGrad* eg = nullptr);
 
-extern "C" int dbw_render_forward_ex(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
-                                     const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
-                                     const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
-                                     size_t workspace_bytes, const float* face_shade, float* out_dists, void* stream) {
+extern "C" int dbw_render_forward(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
+                                  const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
+                                  const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
+                                  size_t workspace_bytes, const float* face_shade, float* out_dists, void* stream) {
   return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, out_rgba, topk_ids,
                              workspace, workspace_bytes, face_shade, out_dists, nullptr, stream);
+}
+
+// the epilogue arguments both loss-epilogue forwards require; `who` names the entry point in the error message
+static int check_epilogue(const DbwLossEpilogue* ep, const char* who) {
+  const char* why = !ep ? "null epilogue"
+                  : (!ep->env_rgba || !ep->target || !ep->g_env || !ep->loss_partials) ? "env_rgba, target, g_env and loss_partials are required"
+                  : (ep->n_partials < 1 || (ep->n_partials & (ep->n_partials - 1))) ? "n_partials must be a power of two"
+                  : nullptr;
+  if (!why) return 0;
+  char msg[160];
+  snprintf(msg, sizeof(msg), "%s: %s", who, why);
+  return fail(msg);
 }
 
 extern "C" int dbw_render_forward_loss(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                        const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                        const float* T, const float* faces_alpha, float* out_g_rgba, int32_t* topk_ids,
                                        void* workspace, size_t workspace_bytes, const DbwLossEpilogue* ep, void* stream) {
-  if (!ep) return fail("dbw_render_forward_loss: null epilogue");
-  if (!ep->env_rgba || !ep->target || !ep->g_env || !ep->loss_partials)
-    return fail("dbw_render_forward_loss: env_rgba, target, g_env and loss_partials are required");
-  if (ep->n_partials < 1 || (ep->n_partials & (ep->n_partials - 1))) return fail("dbw_render_forward_loss: n_partials must be a power of two");
+  if (check_epilogue(ep, "dbw_render_forward_loss")) return -1;
   return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, out_g_rgba, topk_ids,
                              workspace, workspace_bytes, nullptr, nullptr, ep, stream);
 }
@@ -1926,10 +1866,7 @@ extern "C" int dbw_render_forward_loss_grad(const DbwRenderSettings* s, const fl
                                             const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
                                             void* workspace, size_t workspace_bytes, const DbwLossEpilogue* ep, int32_t grad_mask,
                                             void* bwd_scratch, size_t bwd_scratch_bytes, void* stream) {
-  if (!ep) return fail("dbw_render_forward_loss_grad: null epilogue");
-  if (!ep->env_rgba || !ep->target || !ep->g_env || !ep->loss_partials)
-    return fail("dbw_render_forward_loss_grad: env_rgba, target, g_env and loss_partials are required");
-  if (ep->n_partials < 1 || (ep->n_partials & (ep->n_partials - 1))) return fail("dbw_render_forward_loss_grad: n_partials must be a power of two");
+  if (check_epilogue(ep, "dbw_render_forward_loss_grad")) return -1;
   if (validate(s)) return -1;
   if (!s->detach_bary) return fail("dbw_render_forward_loss_grad: the pass must be detach_bary");
   if (s->maps_are_texels4 != 2) return fail("dbw_render_forward_loss_grad: the maps must be float4 cell maps (maps_are_texels4 = 2)");
@@ -2023,43 +1960,55 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   return 0;
 }
 
-extern "C" int dbw_render_backward(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
+// adds the cell-gradient copies of the backward scratch into g_maps, times *scale (NULL = 1)
+static int fold_gcells(const DbwRenderSettings& s, const BwdScratch& g, float* g_maps, const float* scale, cudaStream_t st) {
+  const int n_entries = s.n_map_floats / 3;
+  const int blocks = stride_grid(n_entries, 8);
+  if (blocks < 0) return fail("fold_gcells_kernel: SM count", cudaGetLastError());
+  fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries, scale);
+  LAUNCH_CK("fold_gcells_kernel");
+  return 0;
+}
+
+// the vertex and camera end of a backward: the triangle-slot gradients of the scratch, times *scale (NULL = 1), through the
+// face setup backward onto the NDC vertices, then through the projection into g_verts and reduced per view into g_R / g_T.
+// Nothing to do when no vertex or camera gradient is wanted.
+static int geometry_backward(const DbwRenderSettings& s, const Workspace& w, const BwdScratch& g, const float* verts,
+                             const int32_t* faces, const float* R, const float* T, const float* scale, float* g_verts,
+                             float* g_R, float* g_T, cudaStream_t st) {
+  if (!g_verts && !g_R && !g_T) return 0;
+  const int B = s.n_views, V = s.n_verts, F = s.n_faces;
+  const float* verts_ndc = s.verts_are_ndc ? verts : w.verts_ndc;
+  float* g_ndc = s.verts_are_ndc ? g_verts : g.g_verts_ndc;
+  face_setup_backward_kernel<<<(B * F + 127) / 128, 128, 0, st>>>(verts_ndc, faces, B, V, F, s.z_clip, s.perspective_correct,
+                                                                  g.g_tri, g.g_conv, scale, g_ndc);
+  LAUNCH_CK("face_setup_backward_kernel");
+  if (!s.verts_are_ndc && g_verts) {
+    project_verts_backward_kernel<<<(V * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, s.fx, s.fy, s.px, s.py, s.proj_eps, B, V,
+                                                                   g.g_verts_ndc, g_verts);
+    LAUNCH_CK("project_verts_backward_kernel");
+  }
+  if (g_R || g_T) {
+    camera_grad_kernel<<<B, DBW_CAM_NT, 0, st>>>(verts, R, T, s.fx, s.fy, s.px, s.py, s.proj_eps, V, g.g_verts_ndc, g_R, g_T);
+    LAUNCH_CK("camera_grad_kernel");
+  }
+  return 0;
+}
+
+extern "C" int dbw_render_backward(const DbwRenderSettings* s_in, const float* verts, const int32_t* faces, const float* faces_uvs,
                                    const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
-                                   const float* T, const float* faces_alpha, const int32_t* topk_ids, const void* workspace,
-                                   size_t workspace_bytes, const float* grad_rgba, float* g_verts, float* g_faces_alpha,
-                                   float* g_maps, void* bwd_scratch, size_t bwd_scratch_bytes, void* stream) {
-  return dbw_render_backward_scaled(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, topk_ids, workspace,
-                                    workspace_bytes, grad_rgba, nullptr, g_verts, g_faces_alpha, g_maps, bwd_scratch,
-                                    bwd_scratch_bytes, stream);
-}
-
-extern "C" int dbw_render_backward_scaled(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
-                                          const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
-                                          const float* T, const float* faces_alpha, const int32_t* topk_ids, const void* workspace,
-                                          size_t workspace_bytes, const float* grad_rgba, const float* grad_scale, float* g_verts,
-                                          float* g_faces_alpha, float* g_maps, void* bwd_scratch, size_t bwd_scratch_bytes,
-                                          void* stream) {
-  return dbw_render_backward_cameras(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, topk_ids, workspace,
-                                     workspace_bytes, grad_rgba, grad_scale, g_verts, g_faces_alpha, g_maps, nullptr, nullptr,
-                                     bwd_scratch, bwd_scratch_bytes, stream);
-}
-
-extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const float* verts, const int32_t* faces,
-                                           const float* faces_uvs, const int32_t* face_map, const float* maps,
-                                           const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
-                                           const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
-                                           const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
-                                           float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
-                                           void* stream) {
+                                   const float* T, const float* faces_alpha, const void* workspace, size_t workspace_bytes,
+                                   const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
+                                   float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
+                                   void* stream) {
   if (validate(s_in)) return -1;
-  (void)topk_ids;          // kept in the signature for ABI continuity: the backward streams the workspace's fragment records
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || !workspace || !grad_rgba || !bwd_scratch)
     return fail("dbw_render_backward: null pointer argument");
   if (!s_in->save_fragment_state) return fail("dbw_render_backward: the forward must run with save_fragment_state = 1 or 2");
   if (s_in->save_fragment_state == 2 && faces_alpha) return fail("dbw_render_backward: save_fragment_state = 2 declares a pass without faces_alpha");
   const bool cams = g_R != nullptr || g_T != nullptr;
-  if (cams && s_in->verts_are_ndc) return fail("dbw_render_backward_cameras: no camera gradient when verts_are_ndc (R and T are not used)");
-  if (cams && (!R || !T)) return fail("dbw_render_backward_cameras: camera gradients need R and T");
+  if (cams && s_in->verts_are_ndc) return fail("dbw_render_backward: no camera gradient when verts_are_ndc (R and T are not used)");
+  if ((cams || (g_verts && !s_in->verts_are_ndc)) && (!R || !T)) return fail("dbw_render_backward: R and T are required unless verts_are_ndc");
   // every face moves in the image when the camera moves: a call with camera gradients differentiates the static faces too
   DbwRenderSettings s_local = *s_in;
   if (cams) s_local.n_static_faces = 0;
@@ -2068,7 +2017,6 @@ extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const 
   BwdScratch g = carve_bwd(*s, bwd_scratch);
   if (workspace_bytes < w.total || bwd_scratch_bytes < g.total) return fail("dbw_render_backward: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  const int B = s->n_views, V = s->n_verts, F = s->n_faces;
   const bool need_geom = g_verts != nullptr || cams;     // both are reductions of the per-view NDC vertex gradient
   CK(cudaMemsetAsync(bwd_scratch, 0, g.total, st));
   RasterParams P = make_params(*s, w, faces_alpha);
@@ -2109,12 +2057,7 @@ extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const 
       LAUNCH_CK("raster_bary_backward_kernel");
     }
   }
-  if (P.g_cells) {
-    const int blocks = stride_grid(n_entries, 8);
-    if (blocks < 0) return fail("fold_gcells_kernel: SM count", cudaGetLastError());
-    fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries, nullptr);
-    LAUNCH_CK("fold_gcells_kernel");
-  }
+  if (P.g_cells && fold_gcells(*s, g, g_maps, nullptr, st)) return -1;
   if (g_maps && !s->maps_are_texels4) {
     const int n_texels = s->n_map_floats / 3;
     const int blocks = stride_grid(n_texels, 8);
@@ -2122,24 +2065,7 @@ extern "C" int dbw_render_backward_cameras(const DbwRenderSettings* s_in, const 
     fold_gmaps_kernel<<<blocks, 256, 0, st>>>(g.g_maps4, g_maps, n_texels);
     LAUNCH_CK("fold_gmaps_kernel");
   }
-  if (need_geom) {
-    const float* verts_ndc = s->verts_are_ndc ? verts : w.verts_ndc;
-    float* g_ndc = s->verts_are_ndc ? g_verts : g.g_verts_ndc;
-    face_setup_backward_kernel<<<(B * F + 127) / 128, 128, 0, st>>>(verts_ndc, faces, B, V, F, s->z_clip, s->perspective_correct,
-                                                                    g.g_tri, g.g_conv, nullptr, g_ndc);
-    LAUNCH_CK("face_setup_backward_kernel");
-    if (!s->verts_are_ndc && g_verts) {
-      if (!R || !T) return fail("dbw_render_backward: R and T are required unless verts_are_ndc");
-      project_verts_backward_kernel<<<(V * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, B, V,
-                                                                     g.g_verts_ndc, g_verts);
-      LAUNCH_CK("project_verts_backward_kernel");
-    }
-    if (cams) {
-      camera_grad_kernel<<<B, DBW_CAM_NT, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, V, g.g_verts_ndc, g_R, g_T);
-      LAUNCH_CK("camera_grad_kernel");
-    }
-  }
-  return 0;
+  return geometry_backward(*s, w, g, verts, faces, R, T, nullptr, g_verts, g_R, g_T, st);
 }
 
 extern "C" int dbw_render_backward_deferred(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* R,
@@ -2156,39 +2082,16 @@ extern "C" int dbw_render_backward_deferred(const DbwRenderSettings* s, const fl
   const BwdScratch g = carve_bwd(*s, bwd_scratch);
   if (workspace_bytes < w.total || bwd_scratch_bytes < g.total) return fail("dbw_render_backward_deferred: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  const int B = s->n_views, V = s->n_verts, F = s->n_faces;
   // the differentiation itself ran inside raster_forward_kernel<NT, true>: this is the blocks backward a caller times
   ScopedTimer timer(1, s->faces_per_pixel, st);
-  if (g_maps) {
-    const int n_entries = s->n_map_floats / 3;
-    const int blocks = stride_grid(n_entries, 8);
-    if (blocks < 0) return fail("fold_gcells_kernel: SM count", cudaGetLastError());
-    fold_gcells_kernel<<<blocks, 256, 0, st>>>(g.g_cells, (float4*)g_maps, n_entries, grad_scale);
-    LAUNCH_CK("fold_gcells_kernel");
-  }
+  if (g_maps && fold_gcells(*s, g, g_maps, grad_scale, st)) return -1;
   if (g_faces_alpha) {
     const int n_alpha = s->n_faces / (s->alpha_group > 0 ? s->alpha_group : 1);
-    const int n = s->alpha_view_stride ? B * n_alpha : n_alpha;
+    const int n = s->alpha_view_stride ? s->n_views * n_alpha : n_alpha;
     scale_add_kernel<<<(n + 255) / 256, 256, 0, st>>>(g_faces_alpha, g.g_alpha, n, grad_scale);
     LAUNCH_CK("scale_add_kernel");
   }
-  if (g_verts || cams) {
-    const float* verts_ndc = s->verts_are_ndc ? verts : w.verts_ndc;
-    float* g_ndc = s->verts_are_ndc ? g_verts : g.g_verts_ndc;
-    face_setup_backward_kernel<<<(B * F + 127) / 128, 128, 0, st>>>(verts_ndc, faces, B, V, F, s->z_clip, s->perspective_correct,
-                                                                    g.g_tri, g.g_conv, grad_scale, g_ndc);
-    LAUNCH_CK("face_setup_backward_kernel");
-    if (!s->verts_are_ndc && g_verts) {
-      project_verts_backward_kernel<<<(V * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, B, V,
-                                                                     g.g_verts_ndc, g_verts);
-      LAUNCH_CK("project_verts_backward_kernel");
-    }
-    if (cams) {
-      camera_grad_kernel<<<B, DBW_CAM_NT, 0, st>>>(verts, R, T, s->fx, s->fy, s->px, s->py, s->proj_eps, V, g.g_verts_ndc, g_R, g_T);
-      LAUNCH_CK("camera_grad_kernel");
-    }
-  }
-  return 0;
+  return geometry_backward(*s, w, g, verts, faces, R, T, grad_scale, g_verts, g_R, g_T, st);
 }
 
 extern "C" int dbw_composite_mse(int32_t n_views, int32_t height, int32_t width, const float* fg, const float* env,
@@ -2266,7 +2169,7 @@ extern "C" int dbw_render_forward_host(const DbwRenderSettings* s, const float* 
   const int rc = dbw_render_forward(s, (float*)(d + o_verts), (int32_t*)(d + o_faces), (float*)(d + o_fuv), (int32_t*)(d + o_fmap),
                                     (float*)(d + o_maps), (DbwMapDesc*)(d + o_tab), R ? (float*)(d + o_R) : nullptr,
                                     T ? (float*)(d + o_T) : nullptr, faces_alpha ? (float*)(d + o_alpha) : nullptr,
-                                    (float*)(d + o_out), (int32_t*)(d + o_ids), d + o_ws, fwd, stream);
+                                    (float*)(d + o_out), (int32_t*)(d + o_ids), d + o_ws, fwd, nullptr, nullptr, stream);
   if (rc) return rc;
   CK(cudaMemcpyAsync(out_rgba, d + o_out, B * 4 * HW * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));

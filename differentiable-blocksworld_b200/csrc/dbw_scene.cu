@@ -22,15 +22,15 @@ extern void dbw_count_launch_(void);
 // ------------------------------------------------------------------------------------------------ geometry
 #include "dbw_scene_math.cuh"
 
-// out: (N*Vb + Vg, 3) world-space vertices, blocks first then the ground; with env_layout it is (n_static + Vg + N*Vb, 3): the
-// static environment vertices (copied; there may be none), the ground, then the blocks
+// out: (n_static + Vg + N*Vb, 3) world-space vertices: the static environment vertices (copied; there may be none), the
+// ground, then the blocks
 __global__ void scene_geometry_forward_kernel(const GeomParams P, float* __restrict__ out, const float* __restrict__ env_static,
-                                              int n_static, bool env_layout) {
+                                              int n_static) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int nb = P.n_blocks * P.verts_per_block;
   if (i < n_static * 3) out[i] = env_static[i];
   if (i >= nb + P.n_ground_verts) return;
-  if (env_layout) out += (ptrdiff_t)(n_static + (i < nb ? P.n_ground_verts : -nb)) * 3;      // blocks move behind the ground
+  out += (ptrdiff_t)(n_static + (i < nb ? P.n_ground_verts : -nb)) * 3;      // blocks move behind the ground
   const int prim = i < nb ? i / P.verts_per_block : P.n_blocks;
   const int v = i < nb ? i - prim * P.verts_per_block : i - nb;
   float u[3], aux[6], R[9], sc[3] = {1.f, 1.f, 1.f};
@@ -140,34 +140,23 @@ static GeomParams make_geom(const DbwSceneGeometry* g) {
   return P;
 }
 
-extern "C" int dbw_scene_geometry_forward(const DbwSceneGeometry* g, float* verts_out, void* stream) {
-  if (!g || !verts_out) return dbw_fail_("dbw_scene_geometry_forward: null pointer argument", cudaSuccess);
-  if (g->n_blocks < 0 || g->verts_per_block <= 0 || g->n_ground_verts < 0 || g->verts_per_block > 4096)
-    return dbw_fail_("dbw_scene_geometry_forward: bad sizes", cudaSuccess);
-  const int n = g->n_blocks * g->verts_per_block + g->n_ground_verts;
-  if (n == 0) return 0;
-  scene_geometry_forward_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(make_geom(g), verts_out, nullptr, 0, false);
-  SCENE_LAUNCH_CK("scene_geometry_forward_kernel");
-  return 0;
-}
-
-extern "C" int dbw_scene_geometry_forward_env(const DbwSceneGeometry* g, const float* env_static_verts, int32_t n_env_static,
-                                              float* verts_out, void* stream) {
-  if (!g || !verts_out || (n_env_static > 0 && !env_static_verts)) return dbw_fail_("dbw_scene_geometry_forward_env: null pointer argument", cudaSuccess);
+extern "C" int dbw_scene_geometry_forward(const DbwSceneGeometry* g, const float* env_static_verts, int32_t n_env_static,
+                                          float* verts_out, void* stream) {
+  if (!g || !verts_out || (n_env_static > 0 && !env_static_verts)) return dbw_fail_("dbw_scene_geometry_forward: null pointer argument", cudaSuccess);
   if (g->n_blocks < 0 || g->verts_per_block <= 0 || g->n_ground_verts < 0 || g->verts_per_block > 4096 || n_env_static < 0)
-    return dbw_fail_("dbw_scene_geometry_forward_env: bad sizes", cudaSuccess);
+    return dbw_fail_("dbw_scene_geometry_forward: bad sizes", cudaSuccess);
   const int n = g->n_blocks * g->verts_per_block + g->n_ground_verts;
   const int threads = n > n_env_static * 3 ? n : n_env_static * 3;
   if (threads == 0) return 0;
   scene_geometry_forward_kernel<<<(threads + 127) / 128, 128, 0, (cudaStream_t)stream>>>(make_geom(g), verts_out, env_static_verts,
-                                                                                         n_env_static, true);
+                                                                                         n_env_static);
   SCENE_LAUNCH_CK("scene_geometry_forward_kernel");
   return 0;
 }
 
-extern "C" int dbw_scene_geometry_backward_parts(const DbwSceneGeometry* g, const float* g_block_verts, const float* g_ground_verts,
-                                                 float* g_sq_eps, float* g_S, float* g_R_6d, float* g_T, float* g_R_6d_ground,
-                                                 float* g_T_ground, void* stream) {
+extern "C" int dbw_scene_geometry_backward(const DbwSceneGeometry* g, const float* g_block_verts, const float* g_ground_verts,
+                                           float* g_sq_eps, float* g_S, float* g_R_6d, float* g_T, float* g_R_6d_ground,
+                                           float* g_T_ground, void* stream) {
   if (!g || (g->n_blocks > 0 && !g_block_verts) || (g->n_ground_verts > 0 && !g_ground_verts))
     return dbw_fail_("dbw_scene_geometry_backward: null pointer argument", cudaSuccess);
   const int prims = g->n_blocks + (g->n_ground_verts > 0 ? 1 : 0);
@@ -176,13 +165,6 @@ extern "C" int dbw_scene_geometry_backward_parts(const DbwSceneGeometry* g, cons
                                                                          g_R_6d, g_T, g_R_6d_ground, g_T_ground);
   SCENE_LAUNCH_CK("scene_geometry_backward_kernel");
   return 0;
-}
-
-extern "C" int dbw_scene_geometry_backward(const DbwSceneGeometry* g, const float* g_verts, float* g_sq_eps, float* g_S,
-                                           float* g_R_6d, float* g_T, float* g_R_6d_ground, float* g_T_ground, void* stream) {
-  if (!g || !g_verts) return dbw_fail_("dbw_scene_geometry_backward: null pointer argument", cudaSuccess);
-  return dbw_scene_geometry_backward_parts(g, g_verts, g_verts + (size_t)g->n_blocks * g->verts_per_block * 3, g_sq_eps, g_S, g_R_6d,
-                                           g_T, g_R_6d_ground, g_T_ground, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ opacities
@@ -384,7 +366,7 @@ static int check_tex(const char* who, int M, int TS, int p_left, int p_right, in
 }
 
 static int launch_tex(const DbwTexJob* jobs, int n_jobs, bool backward, void* stream) {
-  const char* who = backward ? "dbw_texture_prep_backward" : "dbw_texture_prep_forward";
+  const char* who = backward ? "dbw_texture_prep_backward_multi" : "dbw_texture_prep_forward_multi";
   if (!jobs || n_jobs < 1 || n_jobs > DBW_MAX_TEX_JOBS) return dbw_fail_("texture prep: 1 .. DBW_MAX_TEX_JOBS jobs", cudaSuccess);
   TexJobs J;
   memset(&J, 0, sizeof(J));
@@ -409,15 +391,3 @@ static int launch_tex(const DbwTexJob* jobs, int n_jobs, bool backward, void* st
 
 extern "C" int dbw_texture_prep_forward_multi(const DbwTexJob* jobs, int32_t n_jobs, void* stream) { return launch_tex(jobs, n_jobs, false, stream); }
 extern "C" int dbw_texture_prep_backward_multi(const DbwTexJob* jobs, int32_t n_jobs, void* stream) { return launch_tex(jobs, n_jobs, true, stream); }
-
-extern "C" int dbw_texture_prep_forward(const float* textures, int32_t n_maps, int32_t txt_size, int32_t p_left, int32_t p_right,
-                                        int32_t decimate, float* atlas_out, void* stream) {
-  DbwTexJob j = {textures, atlas_out, nullptr, n_maps, txt_size, p_left, p_right, decimate, 0};
-  return launch_tex(&j, 1, false, stream);
-}
-
-extern "C" int dbw_texture_prep_backward(const float* textures, int32_t n_maps, int32_t txt_size, int32_t p_left, int32_t p_right,
-                                         int32_t decimate, const float* g_atlas, float* g_textures, void* stream) {
-  DbwTexJob j = {textures, const_cast<float*>(g_atlas), g_textures, n_maps, txt_size, p_left, p_right, decimate, 0};
-  return launch_tex(&j, 1, true, stream);
-}

@@ -9,7 +9,7 @@ The blocks pass runs with the loss epilogue of include/dbw_render.h (dbw_render_
 and the MSE gradients w.r.t. both layers happen per pixel inside the rasterizer while the blended colour is in registers.
 Neither `fg` nor `rec` nor the two image-sized gradient round trips of a separate composite kernel ever touch HBM; the
 backward is the two raster backward kernels reading those gradients, scaled on the fly by the upstream gradient of the loss
-(dbw_render_backward_scaled).  When the blocks pass is detach_bary over cell maps (the coarse phase) and a gradient is wanted,
+(dbw_render_backward's grad_scale).  When the blocks pass is detach_bary over cell maps (the coarse phase) and a gradient is wanted,
 it goes further: the blocks forward kernel also runs the pass's backward while the per-pixel fragment lists are still on chip
 (dbw_render_forward_loss_grad), so neither its fragment records nor d loss / d blocks RGBA are written, and the backward only
 folds the accumulated gradients, times the upstream gradient (dbw_render_backward_deferred).  Not usable when another loss consumes `rec` with gradient (LPIPS): the model then keeps
@@ -79,9 +79,9 @@ class _SceneMSEFn(torch.autograd.Function):
         ws_e, bwd_e = _workspace(cfg_e, dev)
         ws_b, bwd_b = _workspace(cfg_b, dev)
         env_rgba = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)
-        _lib.check(L.dbw_render_forward_ex(ctypes.byref(cfg_e), _c(env_verts), _c(env_pass.faces), _c(env_pass.faces_uvs),
-                                           _c(env_pass.face_map), _c(env_maps), _c(table_e), _c(R), _c(T), None, _c(env_rgba),
-                                           None, _c(ws_e), ws_e.numel(), None, None, _stream()), 'dbw_render_forward_ex')
+        _lib.check(L.dbw_render_forward(ctypes.byref(cfg_e), _c(env_verts), _c(env_pass.faces), _c(env_pass.faces_uvs),
+                                        _c(env_pass.face_map), _c(env_maps), _c(table_e), _c(R), _c(T), None, _c(env_rgba),
+                                        None, _c(ws_e), ws_e.numel(), None, None, _stream()), 'dbw_render_forward')
         g_env = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)      # d loss / d env RGBA (unscaled)
         partials = torch.empty(N_PARTIALS, dtype=torch.float32, device=dev)
         rec = torch.empty(B, 3, H, W, dtype=torch.float32, device=dev) if want_rec else None
@@ -143,16 +143,10 @@ class _SceneMSEFn(torch.autograd.Function):
             if g_verts is None and g_maps is None and g_alpha is None and g_R is None and g_T is None:
                 return
             scratch = torch.empty(bwd_bytes, dtype=torch.uint8, device=dev)
-            if g_R is None and g_T is None:
-                _lib.check(L.dbw_render_backward_scaled(ctypes.byref(cfg), _c(verts), _c(p.faces), _c(p.faces_uvs), _c(fmap), _c(maps),
-                                                        _c(table), _c(R), _c(T), _c(alpha), None, _c(ws), ws.numel(), _c(grad),
-                                                        _c(gl), _c(g_verts), _c(g_alpha), _c(g_maps), _c(scratch), scratch.numel(),
-                                                        _stream()), 'dbw_render_backward_scaled')
-                return
-            _lib.check(L.dbw_render_backward_cameras(ctypes.byref(cfg), _c(verts), _c(p.faces), _c(p.faces_uvs), _c(fmap), _c(maps),
-                                                     _c(table), _c(R), _c(T), _c(alpha), None, _c(ws), ws.numel(), _c(grad),
-                                                     _c(gl), _c(g_verts), _c(g_alpha), _c(g_maps), _c(g_R), _c(g_T), _c(scratch),
-                                                     scratch.numel(), _stream()), 'dbw_render_backward_cameras')
+            _lib.check(L.dbw_render_backward(ctypes.byref(cfg), _c(verts), _c(p.faces), _c(p.faces_uvs), _c(fmap), _c(maps), _c(table),
+                                             _c(R), _c(T), _c(alpha), _c(ws), ws.numel(), _c(grad), _c(gl), _c(g_verts), _c(g_alpha),
+                                             _c(g_maps), _c(g_R), _c(g_T), _c(scratch), scratch.numel(), _stream()),
+                       'dbw_render_backward')
 
         def run_blocks():
             if scratch_b is None:
@@ -184,7 +178,7 @@ class _SceneMSEFn(torch.autograd.Function):
 def scene_mse(env_verts, env_atlas, blk_verts, blk_atlas, blk_alpha, R, T, imgs, env_pass, blk_pass, blk_face_map,
               n_total_views=None, return_rec=False, view_rows=None):
     """MSE between `imgs` (B,3,H,W) and the blocks composited over the environment, both rendered from raw scene tensors
-    (float4 texel atlases from scene_ops.texture_atlas).  `n_total_views`: size of the GLOBAL batch the mean runs over
+    (float4 texel atlases from scene_ops.scene_atlases).  `n_total_views`: size of the GLOBAL batch the mean runs over
     (view-sharded data parallelism); `view_rows` (B,2) int32: the [row_begin, row_end) of each view this rank owns.  Returns the loss, or (loss, rec) with a non-differentiable `rec`."""
     B, _, H, W = imgs.shape
     inv = 1.0 / (float(n_total_views or B) * 3 * H * W)

@@ -77,9 +77,9 @@ class _RenderFn(torch.autograd.Function):
         ids = torch.empty(B, K, H, W, dtype=torch.int32, device=verts.device) if (want_ids or want_dists) else None
         dists = torch.empty(B, K, H, W, dtype=torch.float32, device=verts.device) if want_dists else None
         shade = face_shade.detach().contiguous().float() if face_shade is not None else None
-        _lib.check(L.dbw_render_forward_ex(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
-                                           _c(map_table), _c(R), _c(T), _c(fa), _c(out), _c(ids), _c(ws), fwd.value,
-                                           _c(shade), _c(dists), _stream()), 'dbw_render_forward_ex')
+        _lib.check(L.dbw_render_forward(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
+                                        _c(map_table), _c(R), _c(T), _c(fa), _c(out), _c(ids), _c(ws), fwd.value,
+                                        _c(shade), _c(dists), _stream()), 'dbw_render_forward')
         ctx.save_for_backward(verts, maps, fa, R, T, faces, faces_uvs, face_map, map_table, ws)
         ctx.cfg, ctx.bwd_bytes, ctx.lit = s, bwd.value, shade is not None
         if want_dists:
@@ -112,25 +112,20 @@ class _RenderFn(torch.autograd.Function):
         g_maps = torch.zeros_like(maps) if need_m else None
         scratch = torch.empty(ctx.bwd_bytes, dtype=torch.uint8, device=verts.device)
         need_R, need_T = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
-        if not (need_R or need_T):
-            _lib.check(L.dbw_render_backward(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
-                                             _c(map_table), _c(R), _c(T), _c(fa), None, _c(ws), ws.numel(), _c(g_out),
-                                             _c(g_verts), _c(g_fa), _c(g_maps), _c(scratch), scratch.numel(), _stream()),
-                       'dbw_render_backward')
-            return g_verts, g_maps, g_fa, None, None, None, None, None, None, None, None, None, None
-        if s.verts_are_ndc:
-            raise DbwError('R and T are not part of a render from NDC vertices (verts_are_ndc): they have no gradient')
-        # the camera gradients share one zero-fill; a call with camera gradients also differentiates the static faces
-        # (include/dbw_render.h), so g_verts then holds their vertices' rows too
-        cam = torch.zeros(R.shape[0] * 12, device=verts.device, dtype=torch.float32)
-        g_R, g_T = cam[:R.numel()].view_as(R), cam[R.numel():].view_as(T)
-        _lib.check(L.dbw_render_backward_cameras(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
-                                                 _c(map_table), _c(R), _c(T), _c(fa), None, _c(ws), ws.numel(), _c(g_out), None,
-                                                 _c(g_verts), _c(g_fa), _c(g_maps), _c(g_R if need_R else None),
-                                                 _c(g_T if need_T else None), _c(scratch), scratch.numel(), _stream()),
-                   'dbw_render_backward_cameras')
-        return (g_verts, g_maps, g_fa, g_R if need_R else None, g_T if need_T else None, None, None, None, None, None, None,
-                None, None)
+        g_R = g_T = None
+        if need_R or need_T:
+            if s.verts_are_ndc:
+                raise DbwError('R and T are not part of a render from NDC vertices (verts_are_ndc): they have no gradient')
+            # the camera gradients share one zero-fill; a call with camera gradients also differentiates the static faces
+            # (include/dbw_render.h), so g_verts then holds their vertices' rows too
+            cam = torch.zeros(R.shape[0] * 12, device=verts.device, dtype=torch.float32)
+            g_R = cam[:R.numel()].view_as(R) if need_R else None
+            g_T = cam[R.numel():].view_as(T) if need_T else None
+        _lib.check(L.dbw_render_backward(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
+                                         _c(map_table), _c(R), _c(T), _c(fa), _c(ws), ws.numel(), _c(g_out), None,
+                                         _c(g_verts), _c(g_fa), _c(g_maps), _c(g_R), _c(g_T), _c(scratch), scratch.numel(),
+                                         _stream()), 'dbw_render_backward')
+        return g_verts, g_maps, g_fa, g_R, g_T, None, None, None, None, None, None, None, None
 
 
 _TABLE_CACHE = {}
@@ -224,7 +219,7 @@ def render_scene(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, 
     """Functional form over raw tensors (used by Renderer.forward and by the parity tests).
     verts (V,3) [or (B,V,3) NDC], faces (F,3) int32, faces_uvs (F,3,2), face_map (F) int32, maps flat float buffer,
     map_table_host [(offset,H,W)], R (B,3,3), T (B,3), faces_alpha None | (F,) | (B*F,).
-    maps_are_texels4: `maps` is a float4 (RGB+pad) texel atlas from scene_ops.texture_atlas (offsets stay 3*texel)."""
+    maps_are_texels4: `maps` is a float4 (RGB+pad) texel atlas from scene_ops.scene_atlases (offsets stay 3*texel)."""
     dev = verts.device
     B = R.shape[0] if R is not None else verts.shape[0]
     cfg, map_table = scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigma, faces_per_pixel, z_clip,

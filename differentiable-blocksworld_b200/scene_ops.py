@@ -23,39 +23,8 @@ def _geom_struct(static, sq_eps, S, R6, T, R6g, Tg):
     return g
 
 
-class _SceneGeometryFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, sq_eps, S, R6, T, R6g, Tg, static):
-        args = [t.detach().contiguous().float() for t in (sq_eps, S, R6, T, R6g, Tg)]
-        g = _geom_struct(static, *args)
-        n = static['n_blocks'] * static['verts_per_block'] + static['n_ground_verts']
-        out = torch.empty(n, 3, device=sq_eps.device, dtype=torch.float32)
-        _lib.check(_lib.lib().dbw_scene_geometry_forward(ctypes.byref(g), _c(out), _stream()), 'dbw_scene_geometry_forward')
-        ctx.save_for_backward(*args)
-        ctx.static = static
-        nb = static['n_blocks'] * static['verts_per_block']
-        # two outputs (views of the one buffer the kernel wrote): the blocks pass and the environment pass each take theirs,
-        # and the backward receives their gradients directly -- no slice-backward zero-fills / copies / adds
-        return out[:nb], out[nb:]
-
-    @staticmethod
-    def backward(ctx, g_blocks, g_ground):
-        args = ctx.saved_tensors
-        g = _geom_struct(ctx.static, *args)
-        g_out = torch.cat([g_blocks.reshape(-1, 3).float(), g_ground.reshape(-1, 3).float()])
-        # one zero-fill for all six gradients (views of a flat buffer) instead of six launches
-        flat = torch.zeros(sum(t.numel() for t in args), device=g_out.device, dtype=torch.float32)
-        grads, o = [], 0
-        for t in args:
-            grads.append(flat[o:o + t.numel()].view_as(t))
-            o += t.numel()
-        _lib.check(_lib.lib().dbw_scene_geometry_backward(ctypes.byref(g), _c(g_out), *[_c(t) for t in grads],
-                                                          _stream()), 'dbw_scene_geometry_backward')
-        return (*grads, None)
-
-
 class _SceneGeometryEnvFn(torch.autograd.Function):
-    """dbw_scene_geometry_forward_env / _backward_parts: both passes' vertex arrays out of one launch and one buffer
+    """dbw_scene_geometry_forward / _backward: both passes' vertex arrays out of one launch and one buffer
     (static environment vertices | ground | blocks), their gradients taken where autograd hands them over -- no
     concatenation either way, no zero-fill (the backward kernel writes every leaf gradient)."""
 
@@ -66,8 +35,8 @@ class _SceneGeometryEnvFn(torch.autograd.Function):
         n_static, n_ground = env_static.shape[0], static['n_ground_verts']
         nb = static['n_blocks'] * static['verts_per_block']
         out = torch.empty(n_static + n_ground + nb, 3, device=sq_eps.device, dtype=torch.float32)
-        _lib.check(_lib.lib().dbw_scene_geometry_forward_env(ctypes.byref(g), _c(env_static), n_static, _c(out), _stream()),
-                   'dbw_scene_geometry_forward_env')
+        _lib.check(_lib.lib().dbw_scene_geometry_forward(ctypes.byref(g), _c(env_static), n_static, _c(out), _stream()),
+                   'dbw_scene_geometry_forward')
         ctx.save_for_backward(*args)
         ctx.static, ctx.n_static = static, n_static
         return out[n_static + n_ground:], out[:n_static + n_ground]
@@ -84,8 +53,8 @@ class _SceneGeometryEnvFn(torch.autograd.Function):
         for t in args:
             grads.append(flat[o:o + t.numel()].view_as(t))
             o += t.numel()
-        _lib.check(_lib.lib().dbw_scene_geometry_backward_parts(ctypes.byref(g), _c(g_blocks), _c(g_ground), *[_c(t) for t in grads],
-                                                                _stream()), 'dbw_scene_geometry_backward_parts')
+        _lib.check(_lib.lib().dbw_scene_geometry_backward(ctypes.byref(g), _c(g_blocks), _c(g_ground), *[_c(t) for t in grads],
+                                                          _stream()), 'dbw_scene_geometry_backward')
         return (*grads, None, None)
 
 
@@ -132,45 +101,6 @@ def block_opacities(alpha_logit, noise, noise_scale, keep_threshold, face_map, f
     above it are zeroed in alpha_kept and disabled (-1) in the returned face map (keep_threshold < 0: nothing is filtered and
     `face_map` is returned as it is)."""
     return _OpacityFn.apply(alpha_logit, noise, noise_scale, keep_threshold, face_map, faces_per_block)
-
-
-def scene_geometry_parts(sq_eps, S, R_6d, T, R_6d_ground, T_ground, static):
-    """(block vertices (N*Vb, 3), ground vertices (Vg, 3)) in world space, from one kernel launch."""
-    return _SceneGeometryFn.apply(sq_eps, S, R_6d, T, R_6d_ground, T_ground, static)
-
-
-def scene_geometry(sq_eps, S, R_6d, T, R_6d_ground, T_ground, static):
-    """World-space vertices (N*Vb + Vg, 3): the N superquadric blocks, then the ground plane.  `static` holds the
-    buffers / constants of the scene template (see DifferentiableBlocksWorld._geometry_static)."""
-    return torch.cat(_SceneGeometryFn.apply(sq_eps, S, R_6d, T, R_6d_ground, T_ground, static))
-
-
-class _TextureAtlasFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, textures, p_left, p_right, decimate):
-        tex = textures.detach().contiguous().float()
-        M, TS = tex.shape[0], tex.shape[1]
-        atlas = torch.empty(M, TS, TS + p_left + p_right, 4, device=tex.device, dtype=torch.float32)
-        _lib.check(_lib.lib().dbw_texture_prep_forward(_c(tex), M, TS, p_left, p_right, decimate, _c(atlas), _stream()),
-                   'dbw_texture_prep_forward')
-        ctx.save_for_backward(tex)
-        ctx.cfg = (M, TS, p_left, p_right, decimate)
-        return atlas
-
-    @staticmethod
-    def backward(ctx, g_atlas):
-        (tex,) = ctx.saved_tensors
-        M, TS, p_left, p_right, decimate = ctx.cfg
-        g_tex = torch.empty_like(tex)
-        _lib.check(_lib.lib().dbw_texture_prep_backward(_c(tex), M, TS, p_left, p_right, decimate, _c(g_atlas.contiguous().float()),
-                                                        _c(g_tex), _stream()), 'dbw_texture_prep_backward')
-        return g_tex, None, None, None
-
-
-def texture_atlas(textures, p_left=0, p_right=0, decimate=1):
-    """(M,TS,TS,3) logits -> (M, TS, p_left+TS+p_right, 4) float4 texels: sigmoid, optional 8x8 box decimation, circular
-    padding along u -- the layout the rasterizer samples directly (render_scene(..., maps_are_texels4=True))."""
-    return _TextureAtlasFn.apply(textures, int(p_left), int(p_right), int(decimate))
 
 
 class _SceneAtlasesFn(torch.autograd.Function):
@@ -301,5 +231,6 @@ def atlases_from_cells(cells_env, cells_blk, pad, decim_env=1, decim_blocks=1):
 
 def scene_atlases(texture_bkg, texture_ground, textures, pad, decim_env=1, decim_blocks=1):
     """(env atlas (2, S, S, 4): background then ground; blocks atlas (N, TS, p_left + TS + p_right, 4)) from the three texture
-    parameters in one launch (and one for all three gradients)"""
+    parameters in one launch (and one for all three gradients): sigmoid, optional 8x8 box decimation, circular padding along
+    u, as float4 texels -- the layout the rasterizer samples directly (render_scene(..., maps_are_texels4=True))"""
     return _SceneAtlasesFn.apply(texture_bkg, texture_ground, textures, (int(pad[0]), int(pad[1])), int(decim_env), int(decim_blocks))

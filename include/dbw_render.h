@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DBW_ABI_VERSION 7
+#define DBW_ABI_VERSION 8
 #define DBW_MAX_FACES_PER_PIXEL 64
 
 /*
@@ -62,7 +62,7 @@ typedef struct DbwRenderSettings {
                                  every warp that covers it)                                                               */
   int32_t save_fragment_state;/* 1: the forward also keeps one 16 B record {triangle slot | closest edge, u, v, signed squared
                                  distance} and one 16 B colour {r, g, b, -} per kept fragment (+ a per-pixel count byte) in its
-                                 workspace; dbw_render_backward* streams these instead of re-deriving geometry and REQUIRES
+                                 workspace; dbw_render_backward streams these instead of re-deriving geometry and REQUIRES
                                  them.  Costs B*H*W*(32 K + 1) bytes of workspace ADDRESS space (only fragments that exist are
                                  touched).  2: the same for a pass without opacities (faces_alpha must then be NULL in the
                                  forward and the backward); when it is also hard and single-layer (sigma = 0, K = 1) its
@@ -72,7 +72,7 @@ typedef struct DbwRenderSettings {
                                  (src/model/dbw.py:219 repeat_interleave's it per face; that is alpha_group = 1)            */
   int32_t n_static_faces;     /* faces [0, n_static_faces) have constant vertices (the background sphere of the environment,
                                  src/model/dbw.py:267-280): the backward skips their vertex gradient.  Ignored (0) by a
-                                 dbw_render_backward_cameras call that asks for camera gradients                            */
+                                 dbw_render_backward call that asks for camera gradients                                    */
   const int32_t* view_rows;   /* DEVICE (B,2) int32 or NULL: [row_begin, row_end) of each view that this call renders / differentiates.
                                  Rows outside are left untouched in every output (and contribute nothing to a fused loss):
                                  a data-parallel step shards at (view, row band) granularity, so 49 views split evenly
@@ -123,39 +123,44 @@ int dbw_workspace_bytes(const DbwRenderSettings* settings, size_t* fwd_bytes, si
  *   topk_ids     (B,K,H,W) int32 or NULL: z-sorted face slots kept per pixel (-1 = empty) = fragments.pix_to_face modulo
  *                the slot convention; a diagnostic / visualisation output (render_edges), NOT what the backward reads --
  *                that is the workspace's fragment records (settings->save_fragment_state)
+ * and the two optional extras the reference's visualisation paths need (SURVEY 8f ranks 2 and 4):
+ *   face_shade   (B,F,3) or NULL: per-view per-face colour multiplier = PyTorch3D flat shading with ambient + directional
+ *                diffuse light, as configured for renderer_light (src/model/dbw.py:139-143, renderer.py:87-97,195-205)
+ *   out_dists    (B,K,H,W) or NULL: signed squared NDC distance of each kept fragment to its face's nearest edge
+ *                (< 0 inside, -1 for empty slots) = fragments.dists, what render_edges thresholds (renderer.py:134-146)
  */
 int dbw_render_forward(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
                        const float* faces_uvs, const int32_t* face_map, const float* maps,
                        const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
-                       float* out_rgba, int32_t* topk_ids, void* workspace, size_t workspace_bytes, void* stream);
-
-/*
- * Same, with the two optional extras the reference's visualisation paths need (SURVEY 8f ranks 2 and 4):
- *   face_shade  (B,F,3) or NULL: per-view per-face colour multiplier = PyTorch3D flat shading with ambient + directional
- *               diffuse light, as configured for renderer_light (src/model/dbw.py:139-143, renderer.py:87-97,195-205)
- *   out_dists   (B,K,H,W) or NULL: signed squared NDC distance of each kept fragment to its face's nearest edge
- *               (< 0 inside, -1 for empty slots) = fragments.dists, what render_edges thresholds (renderer.py:134-146)
- */
-int dbw_render_forward_ex(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
-                          const float* faces_uvs, const int32_t* face_map, const float* maps,
-                          const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
-                          float* out_rgba, int32_t* topk_ids, void* workspace, size_t workspace_bytes,
-                          const float* face_shade, float* out_dists, void* stream);
+                       float* out_rgba, int32_t* topk_ids, void* workspace, size_t workspace_bytes,
+                       const float* face_shade, float* out_dists, void* stream);
 
 /*
  * Backward of the same (replaces autograd through layered_rgb_blend, grid_sample, interpolate_face_attributes
- * and _C.rasterize_meshes_backward).  grad_rgba (B,4,H,W).  Outputs accumulate:
+ * and _C.rasterize_meshes_backward).  grad_rgba (B,4,H,W), multiplied by the device scalar *grad_scale (NULL = 1) as it is
+ * read.  Outputs accumulate:
  *   g_verts        (V,3)  [or (B,V,3) when verts_are_ndc]
  *   g_faces_alpha  same shape as faces_alpha (may be NULL when faces_alpha is NULL)
  *   g_maps         same packing as maps (may be NULL: no texture gradient)
- * Requires the forward to have run with save_fragment_state = 1 on the same workspace; `topk_ids` is ignored (may be
- * NULL; kept in the signature since ABI 1).
+ * and the gradient of the camera poses (PyTorch3D keeps the camera transform inside autograd behind the reference's
+ * renderer, src/model/renderer.py:94, so a loss on the image differentiates R and T):
+ *   g_R (B,3,3), g_T (B,3)  accumulate (the caller zero-fills); either may be NULL.  Row-vector convention
+ *                           X_view = X_world @ R + T:  g_T[b] = sum_v g_view[b,v],  g_R[b][i][j] = sum_v X_world[v][i] g_view[b,v][j],
+ *                           g_view the NDC vertex gradient pulled back through the projection (|z| < proj_eps: no z term).
+ * Requires the forward to have run with save_fragment_state = 1 or 2 on the same workspace.  With g_R or g_T set:
+ *  - n_static_faces is treated as 0: every face moves in the image when the camera does, so the static faces are
+ *    differentiated too (the background sphere of the environment pass), and g_verts, when not NULL, then also receives the
+ *    rows of the static faces' vertices;
+ *  - the per-view sums run in a fixed order (one CTA per view) and each element of g_R / g_T receives one atomic add per call;
+ *  - with view_rows, the result is the gradient of the rows this call owns: the calls over a partition of the rows sum to
+ *    the gradient of the whole image;
+ *  - verts_are_ndc is an error (R and T are not part of such a render).
  */
 int dbw_render_backward(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
                         const float* faces_uvs, const int32_t* face_map, const float* maps,
                         const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
-                        const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
-                        const float* grad_rgba, float* g_verts, float* g_faces_alpha, float* g_maps,
+                        const void* workspace, size_t workspace_bytes, const float* grad_rgba, const float* grad_scale,
+                        float* g_verts, float* g_faces_alpha, float* g_maps, float* g_R, float* g_T,
                         void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
 
 /*
@@ -195,7 +200,7 @@ typedef struct DbwLossEpilogue {
   float inv_count;            /* weight / (B_total * 3 * H * W): the mean of nn.MSELoss over the GLOBAL batch              */
   int32_t env_alpha_unread;   /* 1: nothing reads the alpha plane of g_env and it is left unwritten -- the environment's
                                  backward has no opacity and no distance path (sigma = 0, faces_alpha NULL), and such a
-                                 dbw_render_backward* never reads grad_rgba's alpha plane.  0: the plane is written (zeros) */
+                                 dbw_render_backward never reads grad_rgba's alpha plane.  0: the plane is written (zeros)  */
 } DbwLossEpilogue;
 
 int dbw_render_forward_loss(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
@@ -226,43 +231,12 @@ int dbw_render_forward_loss_grad(const DbwRenderSettings* settings, const float*
  * The rest of the backward of a dbw_render_forward_loss_grad call (same settings, workspace and scratch): adds
  * *grad_scale (device scalar, required) times the scratch into g_maps (the cell-gradient copies), g_faces_alpha and, through
  * the face setup and projection backward, g_verts, g_R and g_T (any may be NULL; camera gradients as in
- * dbw_render_backward_cameras).  A gradient whose grad_mask bit the forward did not set comes out unchanged.
+ * dbw_render_backward).  A gradient whose grad_mask bit the forward did not set comes out unchanged.
  */
 int dbw_render_backward_deferred(const DbwRenderSettings* settings, const float* verts, const int32_t* faces, const float* R,
                                  const float* T, const void* workspace, size_t workspace_bytes, const float* grad_scale,
                                  float* g_verts, float* g_faces_alpha, float* g_maps, float* g_R, float* g_T,
                                  void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
-
-/* dbw_render_backward with grad_rgba multiplied by the device scalar *grad_scale (NULL = 1) as it is read. */
-int dbw_render_backward_scaled(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
-                               const float* faces_uvs, const int32_t* face_map, const float* maps,
-                               const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
-                               const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
-                               const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
-                               float* g_maps, void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
-
-/*
- * dbw_render_backward_scaled plus the gradient of the camera poses (PyTorch3D keeps the camera transform inside autograd
- * behind the reference's renderer, src/model/renderer.py:94, so a loss on the image differentiates R and T):
- *   g_R (B,3,3), g_T (B,3)  accumulate (the caller zero-fills); either may be NULL.  Row-vector convention
- *                           X_view = X_world @ R + T:  g_T[b] = sum_v g_view[b,v],  g_R[b][i][j] = sum_v X_world[v][i] g_view[b,v][j],
- *                           g_view the NDC vertex gradient pulled back through the projection (|z| < proj_eps: no z term).
- * With both NULL this IS dbw_render_backward_scaled.  With either set:
- *  - n_static_faces is treated as 0: every face moves in the image when the camera does, so the static faces are
- *    differentiated too (the background sphere of the environment pass), and g_verts, when not NULL, then also receives the
- *    rows of the static faces' vertices;
- *  - the per-view sums run in a fixed order (one CTA per view) and each element of g_R / g_T receives one atomic add per call;
- *  - with view_rows, the result is the gradient of the rows this call owns: the calls over a partition of the rows sum to
- *    the gradient of the whole image;
- *  - verts_are_ndc is an error (R and T are not part of such a render).
- */
-int dbw_render_backward_cameras(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
-                                const float* faces_uvs, const int32_t* face_map, const float* maps,
-                                const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
-                                const int32_t* topk_ids, const void* workspace, size_t workspace_bytes,
-                                const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
-                                float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
-                                void* stream);
 
 /*
  * Fused scene construction (src/model/dbw.py:267-352), so that a training step needs no eager tensor ops between the
@@ -283,20 +257,17 @@ typedef struct DbwSceneGeometry {
   float R_world[9], T_world[3];   /* world transform (v * S_world) @ R_world + T_world (dbw.py:264,344)                    */
 } DbwSceneGeometry;
 
-/* verts_out (N*Vb + Vg, 3): world-space vertices of the N superquadric blocks, then of the ground plane. */
-int dbw_scene_geometry_forward(const DbwSceneGeometry* g, float* verts_out, void* stream);
-/* g_verts (N*Vb + Vg, 3) -> gradients of the leaf parameters (written, not accumulated). */
-int dbw_scene_geometry_backward(const DbwSceneGeometry* g, const float* g_verts, float* g_sq_eps, float* g_S, float* g_R_6d,
-                                float* g_T, float* g_R_6d_ground, float* g_T_ground, void* stream);
-/* The layout the two render passes consume without a concatenation: verts_out (n_env_static + Vg + N*Vb, 3) = the static
- * environment vertices (the background sphere in world space, dbw.py:271-274; copied), the ground, then the blocks -- the
- * environment pass takes the first n_env_static + Vg rows, the blocks pass the rest.  The backward takes the two gradient
- * blocks where they lie (any two device pointers: no gather). */
-int dbw_scene_geometry_forward_env(const DbwSceneGeometry* g, const float* env_static_verts, int32_t n_env_static,
-                                   float* verts_out, void* stream);
-int dbw_scene_geometry_backward_parts(const DbwSceneGeometry* g, const float* g_block_verts, const float* g_ground_verts,
-                                      float* g_sq_eps, float* g_S, float* g_R_6d, float* g_T, float* g_R_6d_ground,
-                                      float* g_T_ground, void* stream);
+/* World-space vertices of the N superquadric blocks and of the ground plane, in the layout the two render passes consume
+ * without a concatenation: verts_out (n_env_static + Vg + N*Vb, 3) = the static environment vertices (the background sphere
+ * in world space, dbw.py:271-274; copied; there may be none), the ground, then the blocks -- the environment pass takes the
+ * first n_env_static + Vg rows, the blocks pass the rest.  The backward takes the two gradient blocks where they lie (any
+ * two device pointers: no gather; each may be NULL when it has no rows) and writes the gradients of the leaf parameters
+ * (written, not accumulated). */
+int dbw_scene_geometry_forward(const DbwSceneGeometry* g, const float* env_static_verts, int32_t n_env_static,
+                               float* verts_out, void* stream);
+int dbw_scene_geometry_backward(const DbwSceneGeometry* g, const float* g_block_verts, const float* g_ground_verts,
+                                float* g_sq_eps, float* g_S, float* g_R_6d, float* g_T, float* g_R_6d_ground,
+                                float* g_T_ground, void* stream);
 
 /* Block opacities of a step (src/model/dbw.py:300-316 with static shapes), one launch each way:
  *   alpha[k]      = sigmoid(alpha_logit[k] + noise_scale * noise[k])      (noise may be NULL)
@@ -338,10 +309,6 @@ typedef struct DbwTexJob {
 /* Several stacks in ONE launch (the step's three: background, ground, blocks; `jobs` is a HOST array of n_jobs <= 4). */
 int dbw_texture_prep_forward_multi(const DbwTexJob* jobs, int32_t n_jobs, void* stream);
 int dbw_texture_prep_backward_multi(const DbwTexJob* jobs, int32_t n_jobs, void* stream);
-int dbw_texture_prep_forward(const float* textures, int32_t n_maps, int32_t txt_size, int32_t p_left, int32_t p_right,
-                             int32_t decimate, float* atlas_out, void* stream);
-int dbw_texture_prep_backward(const float* textures, int32_t n_maps, int32_t txt_size, int32_t p_left, int32_t p_right,
-                              int32_t decimate, const float* g_atlas, float* g_textures, void* stream);
 
 /*
  * Host-buffer variants (the end-to-end call a reference-side binding makes with numpy / CPU tensors): every

@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(L, n), f'{n} declared in include/dbw_render.h but not exported'
     assert set(_lib.EXPORTS) == set(names)
-    assert L.dbw_abi_version() == _lib.ABI_VERSION == 7
+    assert L.dbw_abi_version() == _lib.ABI_VERSION == 8
 
 
 def test_settings_struct_layout_and_workspace_query():
@@ -45,10 +45,10 @@ def test_invalid_arguments_fail_loudly_without_a_gpu():
     from dbw_b200.renderer import make_settings
     L = _lib.lib()
     s = make_settings(1, 8, 8, 100, 3, 1, 1, 0, (1, 1, 0, 0), 0., 0., None, (0, 0, 0))      # K = 100 > 64
-    rc = L.dbw_render_forward(ctypes.byref(s), *([None] * 12), 0, None)
+    rc = L.dbw_render_forward(ctypes.byref(s), *([None] * 12), 0, None, None, None)
     assert rc != 0 and b'faces_per_pixel' in L.dbw_last_error()
     s = make_settings(1, 8, 8, 4, 3, 1, 1, 0, (1, 1, 0, 0), 0., 0., None, (0, 0, 0), n_map_floats=12)
-    rc = L.dbw_render_forward(ctypes.byref(s), *([None] * 12), 0, None)
+    rc = L.dbw_render_forward(ctypes.byref(s), *([None] * 12), 0, None, None, None)
     assert rc != 0 and b'null pointer' in L.dbw_last_error()
 
 

@@ -1,10 +1,10 @@
-"""GPU: gradients of the camera poses R and T (dbw_render_backward_cameras, include/dbw_render.h).
+"""GPU: gradients of the camera poses R and T (dbw_render_backward's g_R / g_T, include/dbw_render.h).
 
 Parity with the float64 oracle, whose d/dR and d/dT are torch autograd through oracle.pt3d.world_to_ndc and the rasterizer
 (itself checked against central differences in tests/test_camera_grad_host.py).  Tolerances are those of
 tests/test_raster_matrix_gpu.py: pixels whose kept faces differ between fp32 and fp64 are excluded on both sides; the pose
 gradients must then agree to 1e-3 relative L2 plus an element-wise bound of 2e-3 of the largest magnitude.  Then the C-ABI
-contract (no camera gradient = dbw_render_backward_scaled; the other gradients do not move; row bands sum), the model's
+contract (a camera gradient adds one launch; the other gradients do not move; row bands sum), the model's
 paths, the refusals, the launch count, and a pose recovery."""
 import ctypes
 
@@ -145,7 +145,7 @@ def test_environment_soft_camera_gradients_match_oracle():
 
 # ------------------------------------------------------------------------------------------------ the C-ABI contract
 def _abi(d, R, T, K, size, sigma, Kf, fa=None, group=1, n_static_faces=0, detach=False):
-    """forward once through the C-ABI; returns backward(entry, want_cams) -> (g_verts, g_maps, g_fa, g_R, g_T)"""
+    """forward once through the C-ABI; returns backward(want_cams) -> (g_verts, g_maps, g_fa, g_R, g_T)"""
     from dbw_b200 import _lib
     from dbw_b200.renderer import _c, _stream, scene_settings
     dev = _dev()
@@ -162,19 +162,17 @@ def _abi(d, R, T, K, size, sigma, Kf, fa=None, group=1, n_static_faces=0, detach
     ws = torch.empty(fwd.value, dtype=torch.uint8, device=dev)
     out = torch.empty(B, 4, *size, device=dev)
     _lib.check(L.dbw_render_forward(ctypes.byref(cfg), _c(verts), _c(d['faces']), _c(d['fvu']), _c(d['fmap']), _c(maps), _c(table),
-                                    _c(R), _c(T), _c(fa), _c(out), None, _c(ws), ws.numel(), _stream()), 'dbw_render_forward')
+                                    _c(R), _c(T), _c(fa), _c(out), None, _c(ws), ws.numel(), None, None, _stream()),
+               'dbw_render_forward')
     grad = torch.rand(B, 4, *size, generator=torch.Generator().manual_seed(4)).to(dev)
 
-    def backward(entry, cams):
+    def backward(cams):
         g = [torch.zeros_like(verts), torch.zeros_like(maps), torch.zeros_like(fa) if fa is not None else None,
              torch.zeros(B, 3, 3, device=dev) if cams else None, torch.zeros(B, 3, device=dev) if cams else None]
         scratch = torch.empty(bwd.value, dtype=torch.uint8, device=dev)
-        head = (ctypes.byref(cfg), _c(verts), _c(d['faces']), _c(d['fvu']), _c(d['fmap']), _c(maps), _c(table), _c(R), _c(T), _c(fa),
-                None, _c(ws), ws.numel(), _c(grad), None, _c(g[0]), _c(g[2]), _c(g[1]))
-        if entry == 'scaled':
-            _lib.check(L.dbw_render_backward_scaled(*head, _c(scratch), scratch.numel(), _stream()), entry)
-        else:
-            _lib.check(L.dbw_render_backward_cameras(*head, _c(g[3]), _c(g[4]), _c(scratch), scratch.numel(), _stream()), entry)
+        _lib.check(L.dbw_render_backward(ctypes.byref(cfg), _c(verts), _c(d['faces']), _c(d['fvu']), _c(d['fmap']), _c(maps), _c(table),
+                                         _c(R), _c(T), _c(fa), _c(ws), ws.numel(), _c(grad), None, _c(g[0]), _c(g[2]), _c(g[1]),
+                                         _c(g[3]), _c(g[4]), _c(scratch), scratch.numel(), _stream()), 'dbw_render_backward')
         torch.cuda.synchronize()
         return g
     return backward
@@ -191,37 +189,17 @@ def _abi_cases():
     yield 'env', _abi(_dev_scene(env, dev, texels4=True), R, T, K, (40, 48), 0.0, 1, n_static_faces=n_bkg), env['faces'][:n_bkg]
 
 
-def test_without_camera_gradients_the_entry_is_backward_scaled():
-    """g_R = g_T = NULL: the same launches and the same bits as dbw_render_backward_scaled.  Where the atomics' order differs
-    between two identical calls (the run below says so), the results must lie within that spread"""
-    from dbw_b200 import _lib
-    for name, backward, _ in _abi_cases():
-        n0 = _lib.launch_count()
-        a = backward('scaled', False)
-        n1 = _lib.launch_count()
-        b = backward('cameras', False)
-        n2 = _lib.launch_count()
-        a2 = backward('scaled', False)
-        assert n2 - n1 == n1 - n0, name
-        for x, y, x2, what in zip(a[:3], b[:3], a2[:3], ('verts', 'maps', 'alpha')):
-            if x is None:
-                continue
-            if torch.equal(x, x2):
-                assert torch.equal(x, y), f'{name} {what}: not bit-identical'
-            else:
-                _close_to_cuda(y, x, x2, f'{name} {what}', floor=0.0)
-
-
 def test_camera_gradients_leave_the_other_gradients_alone():
     """with cameras on, g_maps, g_faces_alpha and the rows of g_verts that no static face touches are those of the camera-less
-    call (to the atomics' order); the static faces' vertices now get gradient too, and one reduction launch is added"""
+    call (g_R = g_T = NULL; to the atomics' order); the static faces' vertices now get gradient too, and one reduction launch
+    is added"""
     from dbw_b200 import _lib
     for name, backward, static_faces in _abi_cases():
-        ref = backward('scaled', False)
+        ref = backward(False)
         n0 = _lib.launch_count()
-        got = backward('cameras', True)
+        got = backward(True)
         n1 = _lib.launch_count()
-        backward('scaled', False)
+        backward(False)
         assert (n1 - n0) - (_lib.launch_count() - n1) == 1, name
         V = ref[0].shape[0]
         static_v = torch.zeros(V, dtype=torch.bool)

@@ -93,10 +93,10 @@ def test_camera_gradients_of_an_ndc_render_fail_loudly():
     s = make_settings(1, 8, 8, 1, 3, 1, 1, 0, (1, 1, 0, 0), 0., 0., None, (0, 0, 0), n_map_floats=12, verts_are_ndc=True,
                       save_fragment_state=True)
     fake = ctypes.c_void_p(16)          # never dereferenced: the call fails on its arguments
-    args = [ctypes.byref(s)] + [fake] * 9 + [None, fake, 1 << 20, fake, None, fake, None, None]
-    assert L.dbw_render_backward_cameras(*args, fake, None, fake, 1 << 20, None) != 0
+    args = [ctypes.byref(s)] + [fake] * 9 + [fake, 1 << 20, fake, None, fake, None, None]
+    assert L.dbw_render_backward(*args, fake, None, fake, 1 << 20, None) != 0
     assert b'verts_are_ndc' in L.dbw_last_error()
-    assert L.dbw_render_backward_cameras(*args, None, None, None, 1 << 20, None) != 0      # no scratch: the null check
+    assert L.dbw_render_backward(*args, None, None, None, 1 << 20, None) != 0      # no scratch: the null check
     assert b'null pointer' in L.dbw_last_error()
 
 

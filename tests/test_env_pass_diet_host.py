@@ -64,10 +64,10 @@ def test_opacities_are_refused_in_a_pass_declared_without_them():
     L = _lib.lib()
     s = _settings(1, 0., 2)
     p = ctypes.c_void_p(256)                  # never dereferenced: the call fails on the settings first
-    rc = L.dbw_render_forward(ctypes.byref(s), *([p] * 8), p, p, None, p, 1 << 30, None)
+    rc = L.dbw_render_forward(ctypes.byref(s), *([p] * 8), p, p, None, p, 1 << 30, None, None, None)
     assert rc != 0 and b'faces_alpha' in L.dbw_last_error()
-    rc = L.dbw_render_backward(ctypes.byref(s), *([p] * 8), p, None, p, 1 << 30, p, p, p, p, p, 1 << 30, None)
+    rc = L.dbw_render_backward(ctypes.byref(s), *([p] * 8), p, p, 1 << 30, p, None, p, p, p, None, None, p, 1 << 30, None)
     assert rc != 0 and b'faces_alpha' in L.dbw_last_error()
     s.save_fragment_state = 3
-    rc = L.dbw_render_forward(ctypes.byref(s), *([p] * 8), None, p, None, p, 1 << 30, None)
+    rc = L.dbw_render_forward(ctypes.byref(s), *([p] * 8), None, p, None, p, 1 << 30, None, None, None)
     assert rc != 0 and b'save_fragment_state' in L.dbw_last_error()

@@ -144,16 +144,19 @@ def test_cuda_graph_step_equals_eager_step():
 
 
 def test_fused_scene_geometry_matches_torch_path():
-    """dbw_scene_geometry_* (one kernel each way) vs the eager restatement of dbw.py:299-311,344,348-352."""
+    """dbw_scene_geometry_* (one kernel each way) with an empty static environment vs the eager restatement of
+    dbw.py:299-311,344,348-352; with the background sphere's vertices ahead of the ground, the ground, the blocks and the
+    leaf gradients are the same bits"""
     from dbw_b200 import geometry as G
-    from dbw_b200.scene_ops import scene_geometry
+    from dbw_b200.scene_ops import scene_geometry_passes
     model, tpl, p, dev = _model_and_oracle()
     with torch.no_grad():
         model.sq_eps.copy_(torch.randn_like(model.sq_eps))
         model.R_6d_ground.add_(0.1 * torch.randn_like(model.R_6d_ground))
     st = model._fused_arrays()
     leaves = [model.sq_eps, model.S, model.R_6d, model.T, model.R_6d_ground, model.T_ground]
-    out = scene_geometry(*leaves, st['geom'])
+    blk, ground = scene_geometry_passes(*leaves, st['geom'], torch.zeros(0, 3, device=dev))
+    out = torch.cat([blk, ground])
     # eager
     S, R, T = model.S.exp() + model.scale_min, G.rotation_6d_to_matrix(model.R_6d), model.T
     vb = model._to_world((model.get_blocks_verts() * S[:, None]) @ R + T[:, None]).reshape(-1, 3)
@@ -166,28 +169,45 @@ def test_fused_scene_geometry_matches_torch_path():
     g_r = torch.autograd.grad((ref * w).sum(), leaves)
     for a, b, n in zip(g_f, g_r, ['sq_eps', 'S', 'R_6d', 'T', 'R_6d_ground', 'T_ground']):
         assert (a - b).norm() <= 2e-5 * b.norm() + 1e-7, (n, (a - b).norm().item(), b.norm().item())
+    bkg = st['bkg_world']
+    blk_s, env_s = scene_geometry_passes(*leaves, st['geom'], bkg)
+    assert torch.equal(blk_s, blk) and torch.equal(env_s, torch.cat([bkg, ground]))
+    w_env = torch.cat([torch.randn_like(bkg), w[blk.shape[0]:]])
+    g_s = torch.autograd.grad((blk_s * w[:blk.shape[0]]).sum() + (env_s * w_env).sum(), leaves)
+    for a, b in zip(g_s, g_f):
+        assert torch.equal(a, b)
 
 
 @pytest.mark.parametrize('decim', [1, 8])
 @pytest.mark.parametrize('pad', [(0, 0), (0, 5), (3, 2)])
 def test_fused_texture_atlas_matches_torch_path(decim, pad):
+    """scene_atlases (background, ground and blocks in one launch each way) vs the eager restatement of dbw.py:331-341: the
+    environment maps decimated by `decim`, the blocks' maps by 1 and by 8 and padded by `pad`"""
     import torch.nn.functional as F
-    from dbw_b200.scene_ops import texture_atlas
+    from dbw_b200.scene_ops import scene_atlases
     dev = torch.device('cuda:0')
     g = torch.Generator().manual_seed(3)
-    tex = torch.randn(3, 32, 32, 3, generator=g).to(dev).requires_grad_(True)
-    atlas = texture_atlas(tex, pad[0], pad[1], decim)
-    maps = torch.sigmoid(tex)
-    if decim > 1:
-        sub = F.avg_pool2d(maps.permute(0, 3, 1, 2), kernel_size=decim, stride=decim)
-        maps = F.interpolate(sub, scale_factor=decim).permute(0, 2, 3, 1)
-    ref = F.pad(maps.permute(0, 3, 1, 2), pad=(pad[0], pad[1], 0, 0), mode='circular').permute(0, 2, 3, 1)
-    assert atlas.shape == (3, 32, 32 + sum(pad), 4)
-    assert (atlas[..., :3] - ref).abs().max().item() < 1e-6 and (atlas[..., 3] == 0).all()
-    w = torch.randn(3, 32, 32 + sum(pad), 4, generator=g).to(dev)
-    (ga,) = torch.autograd.grad((atlas * w).sum(), tex)
-    (gr,) = torch.autograd.grad((ref * w[..., :3]).sum(), tex)
-    assert (ga - gr).norm() <= 1e-5 * gr.norm()
+
+    def eager(tex, f, pad):
+        maps = torch.sigmoid(tex)
+        if f > 1:
+            sub = F.avg_pool2d(maps.permute(0, 3, 1, 2), kernel_size=f, stride=f)
+            maps = F.interpolate(sub, scale_factor=f).permute(0, 2, 3, 1)
+        return F.pad(maps.permute(0, 3, 1, 2), pad=(pad[0], pad[1], 0, 0), mode='circular').permute(0, 2, 3, 1)
+
+    tb, tg = (torch.randn(1, 64, 64, 3, generator=g).to(dev).requires_grad_(True) for _ in range(2))
+    tk = torch.randn(3, 32, 32, 3, generator=g).to(dev).requires_grad_(True)
+    for decim_blocks in (1, 8):
+        env, blk = scene_atlases(tb, tg, tk, pad, decim, decim_blocks)
+        ref_env, ref_blk = torch.cat([eager(tb, decim, (0, 0)), eager(tg, decim, (0, 0))]), eager(tk, decim_blocks, pad)
+        assert env.shape == (2, 64, 64, 4) and blk.shape == (3, 32, 32 + sum(pad), 4)
+        for atlas, ref in ((env, ref_env), (blk, ref_blk)):
+            assert (atlas[..., :3] - ref).abs().max().item() < 1e-6 and (atlas[..., 3] == 0).all()
+        we, wb = torch.randn(env.shape, generator=g).to(dev), torch.randn(blk.shape, generator=g).to(dev)
+        ga = torch.autograd.grad((env * we).sum() + (blk * wb).sum(), [tb, tg, tk])
+        gr = torch.autograd.grad((ref_env * we[..., :3]).sum() + (ref_blk * wb[..., :3]).sum(), [tb, tg, tk])
+        for a, b in zip(ga, gr):
+            assert (a - b).norm() <= 1e-5 * b.norm()
 
 
 @pytest.mark.parametrize('fine', [False, True])
@@ -212,7 +232,7 @@ def test_fused_scene_path_equals_eager_path(fine):
 @pytest.mark.parametrize('fine', [False, True])
 def test_loss_epilogue_in_the_rasterizer_equals_composite_kernel(fine):
     """fused_loss.scene_mse (compositing + MSE + their gradients in the blocks pass' epilogue, dbw_render_forward_loss /
-    dbw_render_backward_scaled) against the separate render -> dbw_composite_mse path, incl. a non-unit upstream gradient
+    dbw_render_backward) against the separate render -> dbw_composite_mse path, incl. a non-unit upstream gradient
     and the global-batch normalisation of a view shard."""
     model, tpl, p, dev = _model_and_oracle(fine=fine)
     inp, *_ = _inputs(dev)
@@ -564,40 +584,25 @@ def test_quantitative_and_qualitative_eval(tmp_path):
 
 @pytest.mark.parametrize('decim', [(1, 1), (8, 8), (8, 1)])
 def test_scene_atlases_one_launch_equals_three(decim):
-    """dbw_texture_prep_*_multi (background + ground + blocks in one launch each way) == the three single-stack calls"""
-    from dbw_b200.scene_ops import texture_atlas, scene_atlases
+    """dbw_texture_prep_*_multi: background + ground + blocks in one launch each way (scene_atlases) == one launch per
+    stack, values and gradients bit for bit"""
+    from dbw_b200._lib import DbwTexJob
+    from dbw_b200.scene_ops import scene_atlases, _tex_launch
     dev = torch.device('cuda:0')
     g = torch.Generator().manual_seed(4)
     tb, tg = (torch.randn(1, 64, 64, 3, generator=g).to(dev).requires_grad_(True) for _ in range(2))
     tk = torch.randn(3, 32, 32, 3, generator=g).to(dev).requires_grad_(True)
     env, blk = scene_atlases(tb, tg, tk, (3, 5), decim[0], decim[1])
-    ref_env = torch.stack([texture_atlas(tb, 0, 0, decim[0])[0], texture_atlas(tg, 0, 0, decim[0])[0]])
-    ref_blk = texture_atlas(tk, 3, 5, decim[1])
-    assert torch.equal(env, ref_env) and torch.equal(blk, ref_blk)
     we, wb = torch.randn_like(env), torch.randn_like(blk)
     ga = torch.autograd.grad((env * we).sum() + (blk * wb).sum(), [tb, tg, tk])
-    gr = torch.autograd.grad((ref_env * we).sum() + (ref_blk * wb).sum(), [tb, tg, tk])
-    for a, b in zip(ga, gr):
-        assert torch.equal(a, b)
-
-
-def test_scene_geometry_passes_equals_parts_plus_concatenation():
-    """dbw_scene_geometry_forward_env / _backward_parts: (static environment | ground | blocks) out of one launch ==
-    dbw_scene_geometry_forward + torch.cat, values and leaf gradients bit for bit"""
-    from dbw_b200.scene_ops import scene_geometry_parts, scene_geometry_passes
-    model, tpl, p, dev = _model_and_oracle()
-    with torch.no_grad():
-        model.sq_eps.copy_(torch.randn_like(model.sq_eps))
-        model.R_6d_ground.add_(0.1 * torch.randn_like(model.R_6d_ground))
-    st = model._fused_arrays()
-    leaves = [model.sq_eps, model.S, model.R_6d, model.T, model.R_6d_ground, model.T_ground]
-    blk, env = scene_geometry_passes(*leaves, st['geom'], st['bkg_world'])
-    blk_ref, ground_ref = scene_geometry_parts(*leaves, st['geom'])
-    env_ref = torch.cat([st['bkg_world'], ground_ref])
-    assert torch.equal(blk, blk_ref) and torch.equal(env, env_ref)
-    wb, we = torch.randn_like(blk), torch.randn_like(env)
-    ga = torch.autograd.grad((blk * wb).sum() + (env * we).sum(), leaves)
-    gr = torch.autograd.grad((blk_ref * wb).sum() + (env_ref * we).sum(), leaves)
+    ref_env, ref_blk = torch.empty_like(env), torch.empty_like(blk)
+    gr = [torch.empty_like(t) for t in (tb, tg, tk)]
+    stacks = ((tb, ref_env[0], we[0], 0, 0, decim[0]), (tg, ref_env[1], we[1], 0, 0, decim[0]), (tk, ref_blk, wb, 3, 5, decim[1]))
+    for (t, out, w, pl, pr, f), gt in zip(stacks, gr):
+        t = t.detach()
+        _tex_launch([DbwTexJob(t.data_ptr(), out.data_ptr(), None, t.shape[0], t.shape[1], pl, pr, f, 0)], False)
+        _tex_launch([DbwTexJob(t.data_ptr(), w.data_ptr(), gt.data_ptr(), t.shape[0], t.shape[1], pl, pr, f, 0)], True)
+    assert torch.equal(env, ref_env) and torch.equal(blk, ref_blk)
     for a, b in zip(ga, gr):
         assert torch.equal(a, b)
 

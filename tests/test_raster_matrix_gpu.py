@@ -1,6 +1,6 @@
 """GPU: every raster kernel variant and render option of the C-ABI against the float64 oracle.
 
-`render_forward_impl` / `dbw_render_backward_scaled` (csrc/dbw_render.cu) choose among two forward block sizes with and
+`render_forward_impl` / `dbw_render_backward` (csrc/dbw_render.cu) choose among two forward block sizes with and
 without the loss epilogue, a hard single-layer forward, six `raster_backward_kernel<DETACH, ALPHA, K1>` and two
 `raster_bary_backward_kernel<ALPHA>`.  The cases below are covering sets over that dispatch and over the options of
 `render_scene` (opacity layouts, map layouts, row bands, partial gradients, background, sigmoid opacity, affine

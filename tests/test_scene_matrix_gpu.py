@@ -3,7 +3,7 @@
 The oracle evaluates the same float32 inputs in float64 with oracle/dbw_path.py's pieces (parametric_sq, the 6D rotation,
 SceneTemplate.to_world / _decimate / build_env / build_blocks, circular F.pad, sigmoid).  Every output gets random cotangents
 and every leaf gradient is compared element by element:
-  * geometry -- scene_geometry_parts / scene_geometry_passes and the raw C-ABI entries: icosphere levels 1-3 and one vertex per
+  * geometry -- scene_geometry_passes and the raw C-ABI entries: icosphere levels 1-3 and one vertex per
     block (the backward's 64-thread stride loop), 0 .. 300 blocks with and without a ground, exponents from cube-like to
     pinched (the ln|x| terms at the poles), log-scales -5 .. 3, unnormalised 6D vectors of magnitude 1e-3 .. 1e3, a posed world;
   * opacities -- block_opacities and the raw entries: up to 1000 blocks x 300 faces, saturating logits, each upstream gradient
@@ -219,8 +219,8 @@ def _check_geom(case, tag, blk, gr, grads, want_blk, want_gr, want_grads):
 
 @pytest.mark.parametrize('case', GEOM_CASES, ids=[c[0] for c in GEOM_CASES])
 def test_geometry_seams_match_the_float64_oracle(case):
-    """scene_geometry_parts and scene_geometry_passes (no static environment, and 37 static vertices ahead of the ground)"""
-    from dbw_b200.scene_ops import scene_geometry_parts, scene_geometry_passes
+    """scene_geometry_passes (no static environment, and 37 static vertices ahead of the ground)"""
+    from dbw_b200.scene_ops import scene_geometry_passes
     dev = torch.device('cuda:0')
     x = geom_inputs(case)
     wb, wg = geom_cotangents(x)
@@ -228,9 +228,6 @@ def test_geometry_seams_match_the_float64_oracle(case):
     static = _geom_static(x, dev)
     leaves = [x[k].to(dev).requires_grad_(True) for k in GEOM_LEAVES]
     wb_d, wg_d = wb.float().to(dev), wg.float().to(dev)
-    blk, gr = scene_geometry_parts(*leaves, static)
-    grads = torch.autograd.grad((blk * wb_d).sum() + (gr * wg_d).sum(), leaves)
-    _check_geom(case, 'parts', blk, gr, grads, want_blk, want_gr, want_grads)
     for n_static in (0, 37):
         env_static = torch.randn(n_static, 3, generator=_gen(n_static)).to(dev)
         blk, env = scene_geometry_passes(*leaves, static, env_static)
@@ -246,8 +243,10 @@ def _nan(n, dev):
 
 @pytest.mark.parametrize('case', GEOM_CASES, ids=[c[0] for c in GEOM_CASES])
 def test_geometry_cabi_writes_every_output_and_leaves_the_absent_ground_alone(case):
-    """the raw entries on NaN-prefilled outputs: forward, forward_env, backward, backward_parts.  Without a ground its two
-    gradients keep whatever the caller left there; with neither blocks nor a ground nothing is written at all"""
+    """the raw entries on NaN-prefilled outputs: the forward without and with static environment vertices (nothing written
+    past the end), the backward from two separate gradient blocks and from the two halves of one (ground | blocks) buffer.
+    Without a ground its two gradients keep whatever the caller left there; with neither blocks nor a ground nothing is
+    written at all"""
     from dbw_b200 import _lib
     from dbw_b200.scene_ops import _geom_struct
     from dbw_b200.renderer import _stream
@@ -262,35 +261,32 @@ def test_geometry_cabi_writes_every_output_and_leaves_the_absent_ground_alone(ca
     N, Vb = x['eta'].shape
     Vg, nb = x['ground'].shape[0], N * x['eta'].shape[1]
     p = lambda t: ctypes.c_void_p(t.data_ptr())
-    out = _nan((nb + Vg) * 3 + 1, dev)
-    _lib.check(L.dbw_scene_geometry_forward(ctypes.byref(g), p(out), _stream()), 'dbw_scene_geometry_forward')
-    assert torch.isnan(out[-1])
-    check('geom.verts', out[:-1].view(-1, 3)[:nb], want_blk, 'forward blocks')
-    check('geom.verts', out[:-1].view(-1, 3)[nb:], want_gr, 'forward ground')
-    n_static = 5
-    env_static = torch.randn(n_static, 3, generator=_gen(9)).to(dev)
-    out = _nan((n_static + nb + Vg) * 3, dev)
-    _lib.check(L.dbw_scene_geometry_forward_env(ctypes.byref(g), p(env_static), n_static, p(out), _stream()),
-               'dbw_scene_geometry_forward_env')
-    o = out.view(-1, 3)
-    assert torch.equal(o[:n_static], env_static)
-    check('geom.verts', o[n_static:n_static + Vg], want_gr, 'forward_env ground')
-    check('geom.verts', o[n_static + Vg:], want_blk, 'forward_env blocks')
-    g_verts = torch.cat([wb, wg]).float().to(dev).contiguous()
+    for n_static in (0, 5):
+        env_static = torch.randn(n_static, 3, generator=_gen(9)).to(dev)
+        out = _nan((n_static + Vg + nb) * 3 + 1, dev)
+        _lib.check(L.dbw_scene_geometry_forward(ctypes.byref(g), p(env_static) if n_static else None, n_static, p(out), _stream()),
+                   'dbw_scene_geometry_forward')
+        assert torch.isnan(out[-1])
+        o = out[:-1].view(-1, 3)
+        assert torch.equal(o[:n_static], env_static)
+        check('geom.verts', o[n_static:n_static + Vg], want_gr, f'forward n_static={n_static} ground')
+        check('geom.verts', o[n_static + Vg:], want_blk, f'forward n_static={n_static} blocks')
+    g_env_blocks = torch.cat([wg, wb]).float().to(dev).contiguous()         # the forward's (ground | blocks) layout
     sentinel = 12345.
-    for parts in (False, True):
+    for separate in (False, True):
         grads = [_nan(t.numel(), dev).view_as(t) for t in leaves[:4]] + [torch.full_like(t, sentinel) for t in leaves[4:]]
         if Vg:
             for t in grads[4:]:
                 t.fill_(float('nan'))
-        if parts:
-            gb, gg = g_verts[:nb].clone(), g_verts[nb:].clone()          # two separate allocations
-            rc = L.dbw_scene_geometry_backward_parts(ctypes.byref(g), p(gb) if nb else None, p(gg) if Vg else None,
-                                                     *[p(t) for t in grads], _stream())
+        if separate:
+            gb, gg = wb.float().to(dev), wg.float().to(dev)                   # two separate allocations
+            rc = L.dbw_scene_geometry_backward(ctypes.byref(g), p(gb) if nb else None, p(gg) if Vg else None,
+                                               *[p(t) for t in grads], _stream())
         else:
-            rc = L.dbw_scene_geometry_backward(ctypes.byref(g), p(g_verts), *[p(t) for t in grads], _stream())
+            rc = L.dbw_scene_geometry_backward(ctypes.byref(g), p(g_env_blocks[Vg:]), p(g_env_blocks[:Vg]), *[p(t) for t in grads],
+                                               _stream())
         _lib.check(rc, 'dbw_scene_geometry_backward')
-        tag = 'backward_parts' if parts else 'backward'
+        tag = 'backward separate' if separate else 'backward one buffer'
         for n, a, b in zip(GEOM_LEAVES[:4], grads[:4], want_grads[:4]):
             check(geom_bar(n, case), a, b, tag)
         for n, a, b in zip(GEOM_LEAVES[4:], grads[4:], want_grads[4:]):
@@ -312,13 +308,15 @@ def test_geometry_cabi_with_nothing_to_build_writes_nothing():
     g = _geom_struct(static, *leaves)
     p = lambda t: ctypes.c_void_p(t.data_ptr())
     out = torch.full((12,), 7., device=dev)
-    _lib.check(L.dbw_scene_geometry_forward(ctypes.byref(g), p(out), _stream()), 'forward')
+    _lib.check(L.dbw_scene_geometry_forward(ctypes.byref(g), None, 0, p(out), _stream()), 'forward without static vertices')
+    torch.cuda.synchronize()
+    assert (out == 7.).all()
     env_static = torch.randn(3, 3, generator=_gen(1)).to(dev)
-    _lib.check(L.dbw_scene_geometry_forward_env(ctypes.byref(g), p(env_static), 3, p(out), _stream()), 'forward_env')
+    _lib.check(L.dbw_scene_geometry_forward(ctypes.byref(g), p(env_static), 3, p(out), _stream()), 'forward with static vertices')
     assert torch.equal(out[:9], env_static.reshape(-1)) and (out[9:] == 7.).all()
     grads = [torch.full((6,), 7., device=dev) for _ in range(6)]
-    _lib.check(L.dbw_scene_geometry_backward(ctypes.byref(g), p(out), *[p(t) for t in grads], _stream()), 'backward')
-    _lib.check(L.dbw_scene_geometry_backward_parts(ctypes.byref(g), None, None, *[p(t) for t in grads], _stream()), 'backward_parts')
+    _lib.check(L.dbw_scene_geometry_backward(ctypes.byref(g), p(out), p(out), *[p(t) for t in grads], _stream()), 'backward')
+    _lib.check(L.dbw_scene_geometry_backward(ctypes.byref(g), None, None, *[p(t) for t in grads], _stream()), 'backward, no pointers')
     torch.cuda.synchronize()
     assert all((t == 7.).all() for t in grads)
 
