@@ -8,9 +8,21 @@
 //     A[k] = (pz, bits, signed squared distance, u)      V[k] = v
 //     bits = triangle slot (20 bits) | closest edge (2 bits: 0 = v0v1, 1 = v0v2, 2 = v1v2) << 20 | outside (sd >= 0) << 22
 //            | texture map of the face (9 bits) << 23
-// Order = the tuple order of PyTorch3D's CPU rasterizer queue (depth, then face index; SURVEY.md Appendix A5); the two
-// halves of a z-clipped quad exclude each other (Appendix A3).  Plain C++ apart from the __device__ markers:
-// tests/host_math compiles it for the CPU and checks it against the oracle's queue.
+// Order = (depth, slot): the tuple order of PyTorch3D's CPU rasterizer queue (depth, then face index in the clipped mesh;
+// SURVEY.md Appendix A5) up to the exact depth ties named at frag_key_less; the two halves of a z-clipped quad exclude each
+// other (Appendix A3).
+//
+// The result depends on the order in which a pixel's candidates are OFFERED, through the quad rule alone: a half only
+// yields to, or evicts, its other half while that one is in the list, and a half that was rejected or evicted earlier no
+// longer excludes it (K = 1, halves A and B, a face C with pz_A < pz_C < pz_B and dist_B < |d_A|: offered A, B, C the list
+// ends with C; C, A, B: with B; B, C, A: with A).  The reference offers faces in the clipped mesh's index order, where a
+// quad's two halves are adjacent; the kernel's slots put the second half of face f at F + f.  So every view with z-clipped
+// slots offers them in frag_order_key order, which is that index order: raster_forward_kernel sorts its tile list by it
+// (frag_order_rank) or scans its slots in it (frag_order_slot, coarse_bin_kernel), and compacts in order.  Views without
+// z-clipped slots cannot depend on the order and skip the sort and the ordered bin compaction.
+//
+// Plain C++ apart from the __device__ markers: tests/host_math compiles it for the CPU and checks it against the oracle's
+// queue under every offer order.
 #pragma once
 #include "dbw_math.cuh"
 
@@ -20,7 +32,25 @@
 #define DBW_FRAG_MAP_SHIFT 23
 #define DBW_FRAG_MAX_MAPS 512
 
-// (pz, slot) < key of entry e ?   depths are >= 0, so their bit patterns order like the values
+// Position of slot s of a view with F faces in the clipped mesh's face order: face s's first triangle (s < F), or the
+// second triangle of face s - F right after it.  Strictly monotone in the clipped index (culled faces only leave gaps).
+__device__ __forceinline__ int frag_order_key(int slot, int F) { return slot < F ? 2 * slot : 2 * (slot - F) + 1; }
+
+// The slot at position i of that order (inverse of frag_order_key over the 2F slots of a view)
+__device__ __forceinline__ int frag_order_slot(int i, int F) { return (i & 1) ? F + (i >> 1) : i >> 1; }
+
+// Where entry j of n distinct listed slots goes when the list is sorted by frag_order_key: the number of entries before it
+__device__ __forceinline__ int frag_order_rank(const int* slots, int n, int j, int F) {
+  const int kj = frag_order_key(slots[j], F);
+  int r = 0;
+  for (int i = 0; i < n; ++i) r += frag_order_key(slots[i], F) < kj ? 1 : 0;
+  return r;
+}
+
+// (pz, slot) < key of entry e ?   depths are >= 0, so their bit patterns order like the values.  Exact depth ties go by slot,
+// which is the clipped index order except between the second half of a quad (slot F + f) and a face g > f.  Such a tie needs
+// a clipped triangle, whose clipped vertex is interpolated, and another face to give bit-equal depths at a pixel centre; the
+// (F-dependent) clipped-order comparison here cost 0.8 % of the dtu step, so ties keep the slot order.
 __device__ __forceinline__ bool frag_key_less(unsigned pz_bits, int slot, float4 e) {
   const unsigned eb = __float_as_uint(e.x);
   return pz_bits < eb || (pz_bits == eb && slot < (__float_as_int(e.y) & DBW_FRAG_SLOT_MASK));

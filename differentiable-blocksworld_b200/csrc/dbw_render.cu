@@ -423,34 +423,49 @@ __global__ void face_setup_kernel(const float* __restrict__ verts_ndc, const int
 // ------------------------------------------------------------------------------------------------ coarse binning
 // One CTA per (view, 64 x 64 pixel bin): the slots whose blur-expanded box reaches the bin, compacted into the bin's list.
 // A raster tile then scans its bin's list (tens of slots) instead of the view's 2F (800 - 8000): at the stress shape the
-// per-tile scan of all 8000 slots was half of the forward's instructions.
+// per-tile scan of all 8000 slots was half of the forward's instructions.  A view with z-clipped slots lists them in
+// frag_order_key order (the clipped mesh's face order, dbw_fraglist.cuh): slots are scanned in that order and compacted in
+// order (a block prefix over the warps' counts per batch), so that the raster kernel's chunked path offers them in it.  Other
+// views cannot depend on the order: one shared atomic per warp and batch, no barrier.
 __global__ void coarse_bin_kernel(const float4* __restrict__ bbox, const int* __restrict__ view_flags, int F, int H, int W,
                                   int nbx, int nby, int* __restrict__ cbin_count, int* __restrict__ cbin_list) {
   __shared__ int s_n;
+  __shared__ int s_wn[32];
   const int view = blockIdx.x, bin = blockIdx.y, bx = bin % nbx, by = bin / nbx;
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n_warps = blockDim.x >> 5;
   if (tid == 0) s_n = 0;
   __syncthreads();
   const int x0 = bx * DBW_CBIN, x1 = min(x0 + DBW_CBIN, W) - 1, y0 = by * DBW_CBIN, y1 = min(y0 + DBW_CBIN, H) - 1;
   // NDC extents of the bin's pixel centres (+X is left, +Y is up: the last column / row has the smallest coordinate)
   const float xmin = pix_to_ndc(W - 1 - x1, W, H), xmax = pix_to_ndc(W - 1 - x0, W, H);
   const float ymin = pix_to_ndc(H - 1 - y1, H, W), ymax = pix_to_ndc(H - 1 - y0, H, W);
-  const int nslots = (view_flags[view] & 1) ? 2 * F : F;
+  const bool split = view_flags[view] & 1;
+  const int nslots = split ? 2 * F : F;
   const float4* bb = bbox + (size_t)view * 2 * F;
   int* list = cbin_list + ((size_t)view * gridDim.y + bin) * 2 * F;
+  int n = 0;                        // entries listed so far in order (the same in every thread)
   for (int base = 0; base < nslots; base += blockDim.x) {
-    const int sl = base + tid;
+    const int i = base + tid;
+    const int sl = split ? frag_order_slot(i, F) : i;
     bool hit = false;
-    if (sl < nslots) { const float4 b = __ldg(&bb[sl]); hit = !(b.x > xmax || b.y < xmin || b.z > ymax || b.w < ymin); }
+    if (i < nslots) { const float4 b = __ldg(&bb[sl]); hit = !(b.x > xmax || b.y < xmin || b.z > ymax || b.w < ymin); }
     const unsigned m = __ballot_sync(0xffffffffu, hit);
-    if (m == 0u) continue;
-    int wbase = 0;
-    if (lane == 0) wbase = atomicAdd(&s_n, __popc(m));
-    wbase = __shfl_sync(0xffffffffu, wbase, 0);
-    if (hit) list[wbase + __popc(m & ((1u << lane) - 1u))] = sl;
+    if (split) {
+      if (lane == 0) s_wn[warp] = __popc(m);
+      __syncthreads();
+      int pos = n;
+      for (int w = 0; w < n_warps; ++w) { const int c = s_wn[w]; pos += w < warp ? c : 0; n += c; }
+      if (hit) list[pos + __popc(m & ((1u << lane) - 1u))] = sl;
+      __syncthreads();              // s_wn is read before the next batch writes it
+    } else if (m) {
+      int wbase = 0;
+      if (lane == 0) wbase = atomicAdd(&s_n, __popc(m));
+      wbase = __shfl_sync(0xffffffffu, wbase, 0);
+      if (hit) list[wbase + __popc(m & ((1u << lane) - 1u))] = sl;
+    }
   }
   __syncthreads();
-  if (tid == 0) cbin_count[(size_t)view * gridDim.y + bin] = s_n;
+  if (tid == 0) cbin_count[(size_t)view * gridDim.y + bin] = split ? n : s_n;
 }
 
 // ------------------------------------------------------------------------------------------------ raster + shade + blend, forward
@@ -734,9 +749,12 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   // slots is tested and compacted with NO block barrier in between (ballot + one shared atomic per warp); hits beyond the
   // list capacity are counted but not stored, and only then the chunked path below (barrier per batch) is taken.
   const float rx0 = t_xmin - P.sqrt_blur, rx1 = t_xmax + P.sqrt_blur, ry0 = t_ymin - P.sqrt_blur, ry1 = t_ymax + P.sqrt_blur;
+  // (the chunked path scans in frag_order_key order: the coarse bin's list is in it, the view's 2F slots are mapped to it)
+  const bool split = vflags & 1;
   auto scan_hit = [&](int& s, float4& bb) -> bool {
     if (s >= nslots) return false;
     if (clist) s = __ldg(clist + s);
+    else if (split) s = frag_order_slot(s, P.F);
     bb = __ldg(&bbox[s]);
     if (bb.x > t_xmax || bb.y < t_xmin || bb.z > t_ymax || bb.w < t_ymin) return false;
     const float4 r0 = __ldg(&rec[(size_t)s * 4]);
@@ -776,33 +794,50 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   __syncthreads();
   const int total = s_count;
   if (total <= CAP) {
+    // the warps above listed their hits in the order they won the atomic; where the offer order can matter (a view with
+    // z-clipped slots, dbw_fraglist.cuh), the list is sorted into frag_order_key order first: each entry moves to its rank.
+    // (Flagging the tiles that list a second half instead costs all views a shared store per hit in the scan: slower.)
+    if (split && total > 1) {
+      constexpr int PER = (CAP + NT - 1) / NT;
+      int sl[PER], rk[PER]; float4 bx[PER];
+#pragma unroll
+      for (int r = 0; r < PER; ++r) {
+        const int j = tid + r * NT;
+        if (j < total) { sl[r] = s_slot[j]; bx[r] = s_bbox[j]; rk[r] = frag_order_rank(s_slot, total, j, P.F); }
+      }
+      __syncthreads();
+#pragma unroll
+      for (int r = 0; r < PER; ++r)
+        if (tid + r * NT < total) { s_slot[rk[r]] = sl[r]; s_bbox[rk[r]] = bx[r]; }
+      __syncthreads();
+    }
     if (total > 0) raster_list(total);
   } else {
-    // chunked path (more than CAP faces touch this tile): re-scan, flushing the list whenever it may overflow
-    __syncthreads();
-    if (tid == 0) s_count = 0;
-    __syncthreads();
+    // chunked path (more than CAP faces touch this tile): re-scan in frag_order_key order, compacting each batch in order (a
+    // block prefix over the warps' counts), and flush the list whenever it may overflow
+    __shared__ int s_wcount[NT / 32];
     constexpr int BS = NT < CAP ? NT : CAP;          // slots scanned per batch: a batch never overflows an empty list
+    int cnt = 0;                                     // entries listed (the same in every thread)
     for (int base = 0; base < nslots; base += BS) {
       float4 bb = make_float4(0, 0, 0, 0);
       int sl = base + tid;
       const bool hit = tid < BS && scan_hit(sl, bb);
       const unsigned m = __ballot_sync(0xffffffffu, hit);
-      int wbase = 0;
-      if (lane == 0 && m) wbase = atomicAdd(&s_count, __popc(m));
-      wbase = __shfl_sync(0xffffffffu, wbase, 0);
+      if (lane == 0) s_wcount[warp] = __popc(m);
+      __syncthreads();
+      int pos = cnt;
+#pragma unroll
+      for (int w = 0; w < NT / 32; ++w) { const int c = s_wcount[w]; pos += w < warp ? c : 0; cnt += c; }
       if (hit) {
-        const int pos = wbase + __popc(m & ((1u << lane) - 1u));
+        pos += __popc(m & ((1u << lane) - 1u));
         s_slot[pos] = sl; s_bbox[pos] = bb;
       }
-      __syncthreads();
-      const int cnt = s_count;
+      __syncthreads();                // the batch is listed; s_wcount is read before the next batch writes it
       const bool last = base + BS >= nslots;
       if (cnt > CAP - BS || last) {
         raster_list(cnt);
-        __syncthreads();              // every warp is done with the list before it is reset and refilled
-        if (tid == 0) s_count = 0;
-        __syncthreads();
+        __syncthreads();              // every warp is done with the list before it is refilled
+        cnt = 0;
       }
     }
   }

@@ -153,7 +153,7 @@ def _close_to_cuda(a, b, spread_ref, what, floor=1e-5):
     assert torch.isfinite(a).all() and err <= max(floor, 4 * spread), f'{what}: {err:.3e} (spread {spread:.3e})'
 
 
-def _parity(tag, scene, ref, frags, out, ids, pairs, seed, max_ambiguous=2e-3, rel=GRAD_REL, elem=GRAD_ELEM):
+def _parity(tag, scene, ref, frags, out, ids, pairs, seed, max_ambiguous=2e-3, rel=GRAD_REL, elem=GRAD_ELEM, img_tol=IMG_TOL):
     """image + top-K ids + gradients of one CUDA render against its oracle render.  pairs: (name, oracle leaves, CUDA leaf,
     CUDA gradient -> list of tensors shaped like the oracle leaves)"""
     B, _, H, W = ref.shape
@@ -162,7 +162,7 @@ def _parity(tag, scene, ref, frags, out, ids, pairs, seed, max_ambiguous=2e-3, r
     print(f'\n{tag}: ambiguous pixels {amb * 100:.3f}%')
     assert amb <= max(max_ambiguous, 1.5 / (B * H * W)), f'{amb * 100:.3f}% of pixels take a different discrete decision'
     err = (out.detach().cpu().double() - ref.detach()).abs() * mask
-    assert err.max().item() <= IMG_TOL, f'image max err {err.max().item():.3e}'
+    assert err.max().item() <= img_tol, f'image max err {err.max().item():.3e}'
     wgt = torch.rand(B, 4, H, W, generator=torch.Generator().manual_seed(seed), dtype=torch.float64) * mask
     ref_leaves = [t for _, leaves, _, _ in pairs for t in leaves]
     ref_g = torch.autograd.grad((ref * wgt).sum(), ref_leaves, allow_unused=True)
