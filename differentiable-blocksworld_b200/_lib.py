@@ -61,6 +61,11 @@ class DbwLpipsTargetCache(ctypes.Structure):
                 ('normalize', ctypes.c_int32)]
 
 
+class DbwVggLossOptions(ctypes.Structure):
+    _fields_ = [('levels', ctypes.c_int32), ('normalize_input', ctypes.c_int32), ('normalize_features', ctypes.c_int32),
+                ('sum_channels', ctypes.c_int32)]
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -78,7 +83,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_u
            'dbw_lpips_workspace_bytes', 'dbw_lpips_prepare_weights', 'dbw_lpips_forward', 'dbw_lpips_backward',
            'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward',
            'dbw_lpips_head_forward', 'dbw_lpips_head_backward',
-           'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached']
+           'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached',
+           'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward']
 
 _lib = None
 
@@ -159,6 +165,10 @@ def lib():
         L.dbw_lpips_cache_targets.argtypes = [np_, vp, cp, i64, vp, sz, vp]
         L.dbw_lpips_forward_cached.argtypes = [np_, cp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, sz, vp]
         L.dbw_lpips_backward_cached.argtypes = [np_, cp, vp, vp, i64, i32, i32, i32, i32, vp, vp, sz, vp]
+        op = ctypes.POINTER(DbwVggLossOptions)
+        L.dbw_vgg_loss_workspace_bytes.argtypes = [i64, i32, i32, op, i32, ctypes.POINTER(sz)]
+        L.dbw_vgg_loss_forward.argtypes = [np_, op, vp, vp, i64, i32, i32, i32, vp, vp, sz, vp]
+        L.dbw_vgg_loss_backward.argtypes = [np_, op, vp, i64, i32, i32, vp, vp, sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

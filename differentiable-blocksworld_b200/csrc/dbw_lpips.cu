@@ -523,6 +523,102 @@ __global__ void lpips_prepare_kernel(const float* __restrict__ w, float* __restr
   bwd[((int64_t)ci * 9 + (8 - tap)) * Cout + co] = v;           // (2-ky)*3 + (2-kx) = 8 - tap
 }
 
+// ------------------------------------------------------------------------------------------------ VGG feature loss
+// the constants of a dbw_vgg_loss_forward, written by it into the workspace: the head weight of each level (the first C_k
+// of 512 floats: 1 with sum_channels, else 1 / C_k, exact for C_k = 64..512), then the identity input transform (shift
+// 0, scale 1, 4 floats each)
+constexpr int VGG_CONSTS = 5 * 512 + 8;
+
+__global__ void vgg_consts_kernel(float* __restrict__ c, int sum_channels) {
+  for (int i = threadIdx.x; i < VGG_CONSTS; i += blockDim.x) {
+    const int k = i / 512;
+    float v;
+    if (k < 5) v = sum_channels ? 1.f : __fdiv_rn(1.f, (float)(k < 3 ? 64 << k : 512));
+    else v = i < 5 * 512 + 4 ? 0.f : 1.f;
+    c[i] = v;
+  }
+}
+
+// the un-normalised head: per pixel w * sum_c (f0 - f1)^2, one warp per pixel; partials as lpips_head_forward_kernel
+// writes them
+template <int C>
+__global__ void __launch_bounds__(256) vgg_head_plain_forward_kernel(const float* __restrict__ f0, const float* __restrict__ f1,
+                                                                     float w, int HW, float* __restrict__ partials, int n_chunks) {
+  constexpr int NPL = C / 32;
+  __shared__ float wsum[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, b = blockIdx.y;
+  float acc = 0.f;
+  for (int s = 0; s < HEAD_PIX / 8; ++s) {
+    const int p = blockIdx.x * HEAD_PIX + warp * (HEAD_PIX / 8) + s;
+    if (p >= HW) break;
+    const int64_t base = ((int64_t)b * HW + p) * C;
+    float v = 0.f;
+#pragma unroll
+    for (int j = 0; j < NPL; ++j) {
+      const float e = f0[base + lane + 32 * j] - f1[base + lane + 32 * j];
+      v = fmaf(w, e * e, v);
+    }
+    acc += warp_sum0(v);
+  }
+  if (lane == 0) wsum[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+#pragma unroll
+    for (int w8 = 0; w8 < 8; ++w8) s += wsum[w8];
+    partials[(int64_t)b * n_chunks + blockIdx.x] = s;
+  }
+}
+
+// g <- (d value / d f1 + (accumulate ? g : 0)) * [f1 > 0]; d value / d f1 = 2 w (f1 - f0) grad_value[b] / HW
+template <int C>
+__global__ void __launch_bounds__(256) vgg_head_plain_backward_kernel(const float* __restrict__ f0, const float* __restrict__ f1,
+                                                                      float w, int HW, const float* __restrict__ grad_value,
+                                                                      int accumulate, float* __restrict__ g) {
+  constexpr int NPL = C / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, b = blockIdx.y;
+  const float k = 2.f * w * __fdiv_rn(grad_value[b], (float)HW);
+  for (int s = 0; s < HEAD_PIX / 8; ++s) {
+    const int p = blockIdx.x * HEAD_PIX + warp * (HEAD_PIX / 8) + s;
+    if (p >= HW) break;
+    const int64_t base = ((int64_t)b * HW + p) * C;
+#pragma unroll
+    for (int j = 0; j < NPL; ++j) {
+      const int64_t o = base + lane + 32 * j;
+      const float u1 = f1[o];
+      float v = k * (u1 - f0[o]);
+      if (accumulate) v += g[o];
+      g[o] = u1 > 0.f ? v : 0.f;
+    }
+  }
+}
+
+// g *= [act > 0]: the ReLU of a tap whose level is not requested, between its pool's backward and its input gradient
+__global__ void vgg_relu_mask_kernel(const float4* __restrict__ act, float4* __restrict__ g, int64_t n4) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n4) return;
+  const float4 a = act[i];
+  float4 v = g[i];
+  v.x = a.x > 0.f ? v.x : 0.f; v.y = a.y > 0.f ? v.y : 0.f; v.z = a.z > 0.f ? v.z : 0.f; v.w = a.w > 0.f ? v.w : 0.f;
+  g[i] = v;
+}
+
+// value[b] = sum over the requested levels k, in order, of (sum of the level's partials, in chunk order) / (H_k W_k); the
+// levels not requested have no chunks
+__global__ void vgg_reduce_kernel(const float* __restrict__ partials, PartDesc pd, int B, float* __restrict__ value) {
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    float v = 0.f;
+    for (int k = 0; k < 5; ++k) {
+      if (pd.chunks[k] == 0) continue;
+      const float* p = partials + pd.off[k] + (int64_t)b * pd.chunks[k];
+      float s = 0.f;
+      for (int64_t c = 0; c < pd.chunks[k]; ++c) s += p[c];
+      v += s * pd.inv_hw[k];
+    }
+    value[b] = v;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ target cache
 constexpr int FP_CHUNKS = 32;                // fingerprint partials per image
 constexpr int LOOKUP_THREADS = 512;
@@ -746,28 +842,36 @@ int check_dims(const char* what, int64_t B, int H, int W) {
   return 0;
 }
 
-bool net_ok(const DbwLpipsNet* net) {
+// the conv weights, the input transform and the prepared copies (all dbw_lpips_prepare_weights needs)
+bool trunk_ok(const DbwLpipsNet* net) {
   if (!net || !net->shift || !net->scale || !net->prepared) return false;
   for (int l = 0; l < LP_LAYERS; ++l) if (!net->conv_w[l] || !net->conv_b[l]) return false;
+  return true;
+}
+
+bool net_ok(const DbwLpipsNet* net) {
+  if (!trunk_ok(net)) return false;
   for (int k = 0; k < 5; ++k) if (!net->lin_w[k]) return false;
   return true;
 }
 
-// the 13 layers of one image batch x: out[l] receives layer l's activation (pool outputs go to S0).  With route and count
-// (the miss chain), only the images of route[s][1] for slots s < *count, compacted in slot order.
+// layers 0..last of one image batch x: out[l] receives layer l's activation, the pool before level k writes pool_out[k]
+// (S0 without pool_out).  With route and count (the miss chain), only the images of route[s][1] for slots s < *count,
+// compacted in slot order.
 int trunk(const DbwLpipsNet* net, const float* x, float* const* out, float* S0, const Dims& d, int normalize, cudaStream_t st,
-          const int32_t* route = nullptr, const int* count = nullptr) {
+          const int32_t* route = nullptr, const int* count = nullptr, int last = LP_LAYERS - 1, float* const* pool_out = nullptr) {
   const float* prep = (const float*)net->prepared;
   const int64_t B = d.B;
   if (const int rc = conv_first(x, net->conv_w[0], net->conv_b[0], net->shift, net->scale, normalize, out[0], B, d.H[0], d.W[0], st,
                                 route, count))
     return rc;
   const float* cur = out[0];
-  for (int l = 1; l < LP_LAYERS; ++l) {
+  for (int l = 1; l <= last; ++l) {
     const int lv = LP_LEVEL[l];
     if (lv != LP_LEVEL[l - 1]) {
-      if (const int rc = pool(cur, S0, B, d.H[lv - 1], d.W[lv - 1], LP_CIN[l], st, count)) return rc;
-      cur = S0;
+      float* po = pool_out ? pool_out[lv] : S0;
+      if (const int rc = pool(cur, po, B, d.H[lv - 1], d.W[lv - 1], LP_CIN[l], st, count)) return rc;
+      cur = po;
     }
     if (const int rc = conv3x3(cur, prep + wfwd_off(l), net->conv_b[l], nullptr, out[l], B, d.H[lv], d.W[lv], LP_CIN[l], LP_COUT[l], 1,
                                st, count))
@@ -878,6 +982,188 @@ int check_cache(const char* what, const DbwLpipsTargetCache* cache, int H, int W
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ VGG feature loss (host)
+bool vgg_wants(int levels, int k) { return (levels >> k) & 1; }
+int vgg_deepest(int levels) { int L = 0; for (int k = 0; k < 5; ++k) if (vgg_wants(levels, k)) L = k; return L; }   // 0-based
+
+// workspace layout, in floats (stated in include/dbw_render.h): rec's activations through the deepest level (only its
+// requested taps when no backward follows), imgs' requested taps, two scratch tensors of B*H*W*64, the head partials of the
+// requested levels, the constants of vgg_consts_kernel
+struct VggLayout {
+  int64_t act[LP_LAYERS], tap0[5], s0, s1, partials, consts, total;
+  int64_t chunks[5], part_off[5];
+};
+
+VggLayout vgg_layout_of(const Dims& d, int levels, bool save) {
+  VggLayout L; int64_t o = 0;
+  const int last = LP_TAP_LAYER[vgg_deepest(levels)];
+  for (int l = 0; l < LP_LAYERS; ++l) {
+    L.act[l] = -1;
+    const int lv = LP_LEVEL[l];
+    if (l > last || (!save && !(LP_TAP_LAYER[lv] == l && vgg_wants(levels, lv)))) continue;
+    L.act[l] = o; o += align64(d.B * d.H[lv] * d.W[lv] * LP_COUT[l]);
+  }
+  for (int k = 0; k < 5; ++k) {
+    L.tap0[k] = -1;
+    if (vgg_wants(levels, k)) { L.tap0[k] = o; o += align64(d.B * d.H[k] * d.W[k] * LP_TAP_C[k]); }
+  }
+  const int64_t big = align64(d.B * d.H[0] * d.W[0] * 64);
+  L.s0 = o; o += big;
+  L.s1 = o; o += big;
+  L.partials = o;
+  int64_t p = 0;
+  for (int k = 0; k < 5; ++k) {
+    L.chunks[k] = vgg_wants(levels, k) ? head_chunks(d.H[k], d.W[k]) : 0;
+    L.part_off[k] = p; p += d.B * L.chunks[k];
+  }
+  o += align64(p);
+  L.consts = o; o += align64(VGG_CONSTS);
+  L.total = o;
+  return L;
+}
+
+int check_vgg_args(const char* what, int64_t B, int H, int W, const DbwVggLossOptions* opt) {
+  if (!opt || opt->levels < 1 || opt->levels > 31) return dbw_fail_(what, cudaSuccess);
+  const int min_hw = 1 << vgg_deepest(opt->levels);
+  if (B < 1 || B > 65535 || H < min_hw || W < min_hw || H > 32767 || W > 32767 || B * H * W * 64 >= ((int64_t)1 << 40) ||
+      B * H * W >= ((int64_t)1 << 31) - CV_BM)
+    return dbw_fail_(what, cudaSuccess);
+  return 0;
+}
+
+bool vgg_net_ok(const DbwLpipsNet* net, const DbwVggLossOptions* opt) {
+  if (!net || !net->prepared || (opt->normalize_input && (!net->shift || !net->scale))) return false;
+  for (int l = 0; l < LP_LAYERS; ++l) if (!net->conv_w[l] || !net->conv_b[l]) return false;
+  return true;
+}
+
+// the outputs of one chain through layer `last`: keep[l] where given, else (as for the pools) whichever scratch tensor the
+// layer does not read
+void vgg_chain_outputs(float* const* keep, int last, float* S0, float* S1, float** out, float** pool_out) {
+  const float* cur = nullptr;
+  for (int l = 0; l <= last; ++l) {
+    if (l > 0 && LP_LEVEL[l] != LP_LEVEL[l - 1]) {
+      pool_out[LP_LEVEL[l]] = cur == S0 ? S1 : S0;
+      cur = pool_out[LP_LEVEL[l]];
+    }
+    out[l] = keep[l] ? keep[l] : (cur == S0 ? S1 : S0);
+    cur = out[l];
+  }
+}
+
+int vgg_head_forward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
+                     float* part, cudaStream_t st) {
+  if (normalized) return head_forward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, part, st);
+  const int n = (int)head_chunks(H, W), HW = H * W;
+  const dim3 grid((unsigned)n, (unsigned)B);
+  switch (LP_TAP_C[k]) {
+    case 64: vgg_head_plain_forward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
+    case 128: vgg_head_plain_forward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
+    case 256: vgg_head_plain_forward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
+    default: vgg_head_plain_forward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
+  }
+  LP_LAUNCH_CK("vgg_head_plain_forward_kernel");
+  return 0;
+}
+
+int vgg_head_backward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
+                      const float* grad_value, int accumulate, float* g, cudaStream_t st) {
+  if (normalized) return head_backward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, grad_value, accumulate, g, st);
+  const dim3 grid((unsigned)head_chunks(H, W), (unsigned)B);
+  const int HW = H * W;
+  switch (LP_TAP_C[k]) {
+    case 64: vgg_head_plain_backward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
+    case 128: vgg_head_plain_backward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
+    case 256: vgg_head_plain_backward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
+    default: vgg_head_plain_backward_kernel<512><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
+  }
+  LP_LAUNCH_CK("vgg_head_plain_backward_kernel");
+  return 0;
+}
+
+float vgg_head_weight(const DbwVggLossOptions* opt, int k) { return opt->sum_channels ? 1.f : 1.f / (float)LP_TAP_C[k]; }
+
+int vgg_forward_impl(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* in0, const float* in1, int64_t B, int H, int W,
+                     int save_for_backward, float* value, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const Dims d = dims_of(B, H, W);
+  const int levels = opt->levels, last = LP_TAP_LAYER[vgg_deepest(levels)];
+  const VggLayout L = vgg_layout_of(d, levels, save_for_backward != 0);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_vgg_loss_forward: workspace too small", cudaSuccess);
+  float* ws = (float*)workspace;
+  float *S0 = ws + L.s0, *S1 = ws + L.s1, *consts = ws + L.consts;
+  vgg_consts_kernel<<<1, 256, 0, st>>>(consts, opt->sum_channels);
+  LP_LAUNCH_CK("vgg_consts_kernel");
+  // the first layer applies (x - shift) / scale: the ImageNet statistics, or the identity of the constants
+  DbwLpipsNet n = *net;
+  if (!opt->normalize_input) { n.shift = consts + 5 * 512; n.scale = consts + 5 * 512 + 4; }
+  float* keep0[LP_LAYERS] = {};
+  float* keep1[LP_LAYERS] = {};
+  for (int l = 0; l <= last; ++l) {
+    const int lv = LP_LEVEL[l];
+    if (LP_TAP_LAYER[lv] == l && vgg_wants(levels, lv)) keep0[l] = ws + L.tap0[lv];
+    if (L.act[l] >= 0) keep1[l] = ws + L.act[l];
+  }
+  float *out0[LP_LAYERS], *out1[LP_LAYERS], *pool0[5], *pool1[5];
+  vgg_chain_outputs(keep0, last, S0, S1, out0, pool0);
+  vgg_chain_outputs(keep1, last, S0, S1, out1, pool1);
+  if (const int rc = trunk(&n, in0, out0, S0, d, 0, st, nullptr, nullptr, last, pool0)) return rc;
+  if (const int rc = trunk(&n, in1, out1, S0, d, 0, st, nullptr, nullptr, last, pool1)) return rc;
+  PartDesc pd;
+  for (int k = 0; k < 5; ++k) {
+    pd.off[k] = L.part_off[k]; pd.chunks[k] = L.chunks[k]; pd.inv_hw[k] = 1.f / (float)(d.H[k] * d.W[k]);
+    if (!vgg_wants(levels, k)) continue;
+    if (const int rc = vgg_head_forward(ws + L.tap0[k], out1[LP_TAP_LAYER[k]], consts + 512 * k, vgg_head_weight(opt, k),
+                                        opt->normalize_features != 0, B, d.H[k], d.W[k], k, ws + L.partials + L.part_off[k], st))
+      return rc;
+  }
+  vgg_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value);
+  LP_LAUNCH_CK("vgg_reduce_kernel");
+  return 0;
+}
+
+int vgg_backward_impl(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B, int H, int W,
+                      float* grad_in1, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const Dims d = dims_of(B, H, W);
+  const int levels = opt->levels, last = LP_TAP_LAYER[vgg_deepest(levels)];
+  const VggLayout L = vgg_layout_of(d, levels, true);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_vgg_loss_backward: workspace too small", cudaSuccess);
+  float* ws = (float*)workspace;
+  const float* prep = (const float*)net->prepared;
+  const float* consts = ws + L.consts;
+  float* G[2] = {ws + L.s0, ws + L.s1};
+  int cur = 0;                        // G[cur] holds the gradient at the pre-activation of layer l
+  for (int l = last; l >= 1; --l) {
+    const int lv = LP_LEVEL[l];
+    const float* act = ws + L.act[l];
+    if (l == LP_TAP_LAYER[lv]) {
+      const bool deepest = l == last;
+      if (!deepest) {                 // G[cur] holds the gradient at the next pool's output: route it back to this tap
+        if (const int rc = pool_backward(act, G[cur], G[cur ^ 1], B, d.H[lv], d.W[lv], LP_COUT[l], st)) return rc;
+        cur ^= 1;
+      }
+      if (vgg_wants(levels, lv)) {
+        if (const int rc = vgg_head_backward(ws + L.tap0[lv], act, consts + 512 * lv, vgg_head_weight(opt, lv),
+                                             opt->normalize_features != 0, B, d.H[lv], d.W[lv], lv, grad_value, !deepest, G[cur], st))
+          return rc;
+      } else {                        // the deepest level is always requested
+        const int64_t n4 = B * d.H[lv] * d.W[lv] * LP_COUT[l] / 4;
+        if (n4 > 0) {
+          vgg_relu_mask_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>((const float4*)act, (float4*)G[cur], n4);
+          LP_LAUNCH_CK("vgg_relu_mask_kernel");
+        }
+      }
+    }
+    // input gradient of layer l; masked by the ReLU below unless a pool sits in between
+    const bool after_pool = LP_LEVEL[l - 1] != lv;
+    if (const int rc = conv3x3(G[cur], prep + wbwd_off(l), nullptr, after_pool ? nullptr : ws + L.act[l - 1], G[cur ^ 1], B,
+                               d.H[lv], d.W[lv], LP_COUT[l], LP_CIN[l], 0, st))
+      return rc;
+    cur ^= 1;
+  }
+  const float* scale = opt->normalize_input ? net->scale : consts + 5 * 512 + 4;
+  return dgrad_last(G[cur], net->conv_w[0], scale, 0, grad_in1, B, H, W, st);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ C-ABI
@@ -892,7 +1178,7 @@ extern "C" int dbw_lpips_workspace_bytes(int64_t B, int32_t H, int32_t W, int32_
 }
 
 extern "C" int dbw_lpips_prepare_weights(const DbwLpipsNet* net, void* stream) {
-  if (!net_ok(net)) return dbw_fail_("dbw_lpips_prepare_weights: null pointer argument", cudaSuccess);
+  if (!trunk_ok(net)) return dbw_fail_("dbw_lpips_prepare_weights: null pointer argument", cudaSuccess);
   cudaStream_t st = (cudaStream_t)stream;
   float* p = (float*)net->prepared;
   for (int l = 1; l < LP_LAYERS; ++l) {
@@ -1058,4 +1344,32 @@ extern "C" int dbw_lpips_head_backward(const float* f0, const float* f1, const f
   if (!f0 || !f1 || !lin || (train && !seed) || !grad_value || !g)
     return dbw_fail_("dbw_lpips_head_backward: null pointer argument", cudaSuccess);
   return head_backward(f0, f1, lin, B, H, W, C, tap, train, seed, grad_value, accumulate, g, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------ VGG feature loss (C-ABI)
+#define VGG_SIZES "(levels: bits 0..4, not 0; 1 <= B <= 65535, 2^(deepest level - 1) <= H, W <= 32767, B*H*W < 2^31 - 128)"
+
+extern "C" int dbw_vgg_loss_workspace_bytes(int64_t B, int32_t H, int32_t W, const DbwVggLossOptions* opt, int32_t save_for_backward,
+                                            size_t* workspace_bytes) {
+  if (const int rc = check_vgg_args("dbw_vgg_loss_workspace_bytes: bad options or sizes " VGG_SIZES, B, H, W, opt)) return rc;
+  if (!workspace_bytes) return dbw_fail_("dbw_vgg_loss_workspace_bytes: null pointer argument", cudaSuccess);
+  *workspace_bytes = (size_t)vgg_layout_of(dims_of(B, H, W), opt->levels, save_for_backward != 0).total * 4;
+  return 0;
+}
+
+extern "C" int dbw_vgg_loss_forward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* in0, const float* in1, int64_t B,
+                                    int32_t H, int32_t W, int32_t save_for_backward, float* value, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  if (const int rc = check_vgg_args("dbw_vgg_loss_forward: bad options or sizes " VGG_SIZES, B, H, W, opt)) return rc;
+  if (!vgg_net_ok(net, opt) || !in0 || !in1 || !value || !workspace)
+    return dbw_fail_("dbw_vgg_loss_forward: null pointer argument", cudaSuccess);
+  return vgg_forward_impl(net, opt, in0, in1, B, H, W, save_for_backward, value, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int dbw_vgg_loss_backward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B,
+                                     int32_t H, int32_t W, float* grad_in1, void* workspace, size_t workspace_bytes, void* stream) {
+  if (const int rc = check_vgg_args("dbw_vgg_loss_backward: bad options or sizes " VGG_SIZES, B, H, W, opt)) return rc;
+  if (!vgg_net_ok(net, opt) || !grad_value || !grad_in1 || !workspace)
+    return dbw_fail_("dbw_vgg_loss_backward: null pointer argument", cudaSuccess);
+  return vgg_backward_impl(net, opt, grad_value, B, H, W, grad_in1, workspace, workspace_bytes, (cudaStream_t)stream);
 }

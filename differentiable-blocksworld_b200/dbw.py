@@ -667,11 +667,15 @@ class DifferentiableBlocksWorld(nn.Module):
     @torch.no_grad()
     def quantitative_eval(self, loader, device, hard_inference=True):
         """the columns of final_scores.tsv (dbw.py:464-493): n_blocks, L_tot, L_rec, PSNR, SSIM, LPIPS, alpha_k -- hard 4x
-        supersampled renders of the opaque blocks over a loader.  LPIPS is NaN when no perceptual network is installed."""
+        supersampled renders of the opaque blocks over a loader.  LPIPS is NaN when no perceptual network is installed, or
+        when the installed term is the VGG feature loss (perceptual.PerceptualLoss), which is not an LPIPS score."""
+        from .perceptual import PerceptualLoss
         self.eval()
         opacities = self.get_opacities()
         scene = self.build_scene(filter_transparent=True)
         perceptual = getattr(self, 'perceptual_loss', None)
+        if isinstance(perceptual, PerceptualLoss):
+            perceptual = None
         sums, count = dict(L_tot=0.0, L_rec=0.0, PSNR=0.0, SSIM=0.0, LPIPS=0.0), 0
         for inp, labels in loader:
             inp = {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in inp.items()}
@@ -766,7 +770,20 @@ class PerceptualTerm(nn.Module):
 
 def _make_perceptual(name):
     """the perceptual term's network, or None (with a LOUD warning: every shipped config weighs it 0.1) when `lpips` and its
-    VGG weights are not available -- set_perceptual_loss() installs any callable / module instead"""
+    VGG weights are not available -- set_perceptual_loss() installs any callable / module instead.  'perceptual' builds
+    perceptual.PerceptualLoss from torchvision's hub cache file (the file the reference's vgg16(weights=IMAGENET1K_V1)
+    loads); it never downloads.  It is called as perceptual_loss(imgs, rec), as in the reference, so it is not wrapped."""
+    if name == 'perceptual':
+        import os
+        from .perceptual import PerceptualLoss
+        path = os.path.join(torch.hub.get_dir(), 'checkpoints', 'vgg16-397923af.pth')
+        if os.path.exists(path):
+            return PerceptualLoss.from_files(path)
+        import warnings
+        warnings.warn(f'[dbw_b200] perceptual_weight > 0 but the VGG16 weights are unavailable ({path} not found; nothing is '
+                      f'downloaded): the perceptual term is DROPPED from the objective (reported as 0) until '
+                      f'set_perceptual_loss() installs one', RuntimeWarning)
+        return None
     if name != 'lpips':
         raise NotImplementedError(name)
     try:

@@ -20,7 +20,10 @@ Target cache (opt in): `cache_targets(imgs)` computes the taps of fixed `in0` im
 every later forward looks each `in0` image up on the device (a fingerprint, confirmed by comparing the whole image bit for
 bit) and runs the VGG16 trunk of `in0` over the misses only.  Results are the uncached ones bit for bit, hits or not; the
 caller never says which view is which.  A forward uses the cache when its `normalize` and (H, W) are the cache's; any
-change of the weights drops it."""
+change of the weights drops it.
+
+`PerceptualLoss` is the reference's other perceptual term, the VGG16 feature-reconstruction loss (`perceptual_name:
+perceptual`), on the same trunk kernels (dbw_vgg_loss_* in csrc/dbw_lpips.cu)."""
 import ctypes
 from collections import OrderedDict
 
@@ -322,3 +325,178 @@ class LPIPS(nn.Module):
         save = torch.is_grad_enabled() and in1.requires_grad
         return _LpipsFunction.apply(in0.contiguous(), in1.contiguous(), self, bool(normalize), bool(self.training), save,
                                     self._usable_cache(in0, normalize))
+
+
+# ------------------------------------------------------------------------------------------------ VGG feature loss
+MEAN_RGB = (0.485, 0.456, 0.406)
+STD_RGB = (0.229, 0.224, 0.225)
+
+
+def vgg_loss_state_dict_shapes():
+    """{key: shape} of the reference's PerceptualLoss state dict: the ImageNet statistics, then the 13 convolutions under
+    their torchvision indices in the slices relu1_2 .. relu5_3 (all of them, whatever feature_levels is)"""
+    shapes = OrderedDict([('mean_rgb', (3,)), ('std_rgb', (3,))])
+    for s, i, ci, co in CONVS:
+        shapes[f'slice{s}.{i}.weight'] = (co, ci, 3, 3)
+        shapes[f'slice{s}.{i}.bias'] = (co,)
+    return shapes
+
+
+class _VggLossFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, imgs, rec, mod, save):
+        B, _, H, W = rec.shape
+        net, opt = mod._net_struct(), mod._options()
+        ws_bytes = mod._bytes(B, H, W, save)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=rec.device)
+        value = torch.empty(B, dtype=torch.float32, device=rec.device)
+        check(_lib.lib().dbw_vgg_loss_forward(ctypes.byref(net), ctypes.byref(opt), _vp(imgs), _vp(rec), B, H, W, int(save), _vp(value),
+                                              _vp(ws), ws_bytes, _stream(rec.device)), 'dbw_vgg_loss_forward')
+        ctx.mod, ctx.opt, ctx.shape = mod, opt, rec.shape
+        ctx.save_for_backward(ws)
+        return value
+
+    @staticmethod
+    def backward(ctx, grad_value):
+        (ws,) = ctx.saved_tensors
+        B, _, H, W = ctx.shape
+        g = grad_value.reshape(B).to(torch.float32).contiguous()
+        grad = torch.empty(ctx.shape, dtype=torch.float32, device=ws.device)
+        net = ctx.mod._net_struct()
+        check(_lib.lib().dbw_vgg_loss_backward(ctypes.byref(net), ctypes.byref(ctx.opt), _vp(g), B, H, W, _vp(grad), _vp(ws), ws.numel(),
+                                               _stream(ws.device)), 'dbw_vgg_loss_backward')
+        return None, grad, None, None
+
+
+class PerceptualLoss(nn.Module):
+    """The reference's VGG16 feature-reconstruction loss (`PerceptualLoss`, src/model/loss.py:66-111; `perceptual_name:
+    perceptual`) on the sm_90a kernels of csrc/dbw_lpips.cu.  forward(imgs, rec) -> scalar, differentiable in `rec` only:
+    with `normalize_input`, (x - mean_rgb) / std_rgb; torchvision's VGG16 features only through the deepest of
+    `feature_levels` (default [3], relu3_3; a level listed twice counts once); per requested level, optionally
+    f / (||f||_2 over channels + 1e-10), the squared difference averaged over C*H*W (or, with `sum_channels`, summed over
+    channels and averaged over pixels); the levels summed and the batch averaged.  The 64..512-channel convolutions take
+    TF32 operands, as for LPIPS.  CUDA float32 tensors only (no CPU fallback).
+
+    Its buffers and parameters carry the reference's names (`mean_rgb`, `std_rgb`, `slice{s}.{i}.weight` / `.bias`, all 13
+    convolutions), so a reference checkpoint's `perceptual_loss.*` entries load into it.  Build it with `from_files`
+    (torchvision's vgg16-397923af.pth) or `from_state_dict`; a bare PerceptualLoss() has torchvision's default random
+    initialisation (tests only).  With several levels and `sum_channels` the reference's own forward fails to broadcast
+    its per-row means; here the levels' values are summed as for the other options."""
+
+    def __init__(self, normalize_input=True, normalize_features=True, feature_levels=None, sum_channels=False, requires_grad=False):
+        super().__init__()
+        if requires_grad:
+            raise NotImplementedError('PerceptualLoss(requires_grad=True): the kernels give no gradient to the VGG weights')
+        self.normalize_input = normalize_input
+        self.normalize_features = normalize_features
+        self.sum_channels = sum_channels
+        self.feature_levels = feature_levels if feature_levels is not None else [3]
+        if not isinstance(self.feature_levels, (list, tuple)) or not self.feature_levels \
+                or any(k not in (1, 2, 3, 4, 5) for k in self.feature_levels):
+            raise DbwError(f'PerceptualLoss: feature_levels must be a non-empty list of levels 1..5, got {feature_levels!r}')
+        self.max_level = max(self.feature_levels)
+        self.register_buffer('mean_rgb', torch.tensor(MEAN_RGB))
+        self.register_buffer('std_rgb', torch.tensor(STD_RGB))
+        vgg = _Vgg()
+        for s in range(1, 6):
+            self.add_module(f'slice{s}', getattr(vgg, f'slice{s}'))
+        for p in self.parameters():
+            p.requires_grad_(False)
+        self.register_buffer('prepared', torch.zeros(0), persistent=False)
+        self._prepared_key = None
+
+    # ------------------------------------------------------------------ construction
+    @classmethod
+    def from_state_dict(cls, sd, **options):
+        """from a state dict with the reference's names; a `perceptual_loss.` or `module.` prefix is stripped.  Raises on a
+        missing or misshapen key."""
+        sd = dict(sd)
+        for prefix in ('module.', 'perceptual_loss.'):
+            if any(k.startswith(prefix) for k in sd):
+                sd = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
+        shapes = vgg_loss_state_dict_shapes()
+        missing = [k for k in shapes if k not in sd]
+        if missing:
+            raise KeyError(f'PerceptualLoss.from_state_dict: missing keys {missing}')
+        bad = [(k, tuple(sd[k].shape), s) for k, s in shapes.items() if tuple(sd[k].shape) != s]
+        if bad:
+            raise ValueError(f'PerceptualLoss.from_state_dict: misshapen keys (key, got, want) {bad}')
+        m = cls(**options)
+        m.load_state_dict({k: sd[k] for k in shapes}, strict=True)
+        return m
+
+    @classmethod
+    def from_files(cls, vgg16_pth, **options):
+        """from torchvision's vgg16 state dict (`features.N.weight` / `.bias`), the file LPIPS.from_files also reads"""
+        vgg = torch.load(vgg16_pth, map_location='cpu', weights_only=True)
+        sd = {'mean_rgb': torch.tensor(MEAN_RGB), 'std_rgb': torch.tensor(STD_RGB)}
+        for s, i, _, _ in CONVS:
+            for n in ('weight', 'bias'):
+                if f'features.{i}.{n}' not in vgg:
+                    raise KeyError(f'PerceptualLoss.from_files: {vgg16_pth} lacks features.{i}.{n}')
+                sd[f'slice{s}.{i}.{n}'] = vgg[f'features.{i}.{n}']
+        return cls.from_state_dict(sd, **options)
+
+    # ------------------------------------------------------------------ device plumbing
+    def _options(self):
+        levels = 0
+        for k in self.feature_levels:
+            levels |= 1 << (k - 1)
+        return _lib.DbwVggLossOptions(levels, int(bool(self.normalize_input)), int(bool(self.normalize_features)),
+                                      int(bool(self.sum_channels)))
+
+    def _bytes(self, B, H, W, save=True):
+        ws = ctypes.c_size_t(0)
+        check(_lib.lib().dbw_vgg_loss_workspace_bytes(B, H, W, ctypes.byref(self._options()), int(save), ctypes.byref(ws)),
+              'dbw_vgg_loss_workspace_bytes')
+        return ws.value
+
+    def _convs(self):
+        return [getattr(getattr(self, f'slice{s}'), str(i)) for s, i, _, _ in CONVS]
+
+    def _net_struct(self):
+        net = _lib.DbwLpipsNet()
+        for i, c in enumerate(self._convs()):
+            net.conv_w[i], net.conv_b[i] = c.weight.data_ptr(), c.bias.data_ptr()
+        net.shift, net.scale = self.mean_rgb.data_ptr(), self.std_rgb.data_ptr()
+        net.prepared = self.prepared.data_ptr()
+        return net
+
+    def _prepare(self):
+        """(re)write the TF32 forward and input-gradient weight copies when a weight tensor was replaced or modified"""
+        convs = self._convs()
+        params = [c.weight for c in convs] + [c.bias for c in convs] + [self.mean_rgb, self.std_rgb]
+        key = tuple((p.data_ptr(), p._version) for p in params)
+        if key == self._prepared_key:
+            return
+        for p in params:
+            if not (p.is_cuda and p.dtype == torch.float32 and p.is_contiguous()):
+                raise DbwError('PerceptualLoss: weights must be contiguous CUDA float32 tensors (call .cuda() on the module)')
+        ws, prep = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        check(_lib.lib().dbw_lpips_workspace_bytes(1, 16, 16, 0, ctypes.byref(ws), ctypes.byref(prep)), 'dbw_lpips_workspace_bytes')
+        dev = params[0].device
+        if self.prepared.numel() * 4 != prep.value or self.prepared.device != dev:
+            self.prepared = torch.empty(prep.value // 4, dtype=torch.float32, device=dev)
+        check(_lib.lib().dbw_lpips_prepare_weights(ctypes.byref(self._net_struct()), _stream(dev)), 'dbw_lpips_prepare_weights')
+        self._prepared_key = key
+
+    def per_image(self, imgs, rec):
+        """(B,) float32: each image's value, whose batch mean forward() returns"""
+        if imgs.requires_grad:
+            raise DbwError('PerceptualLoss: imgs requires a gradient; only rec (the rendering) is differentiated')
+        if not (torch.is_tensor(imgs) and torch.is_tensor(rec) and imgs.is_cuda and rec.is_cuda):
+            raise DbwError('PerceptualLoss: expected CUDA tensors (there is no CPU fallback)')
+        if imgs.dtype != torch.float32 or rec.dtype != torch.float32:
+            raise DbwError(f'PerceptualLoss: expected float32 images, got {imgs.dtype} / {rec.dtype}')
+        if imgs.shape != rec.shape or rec.dim() != 4 or rec.shape[1] != 3:
+            raise DbwError(f'PerceptualLoss: expected two (B,3,H,W) images of one shape, got {tuple(imgs.shape)} / {tuple(rec.shape)}')
+        if min(rec.shape[2:]) < 2 ** (self.max_level - 1):
+            raise DbwError(f'PerceptualLoss: H and W must be >= {2 ** (self.max_level - 1)} for level {self.max_level}, '
+                           f'got {tuple(rec.shape[2:])}')
+        self._prepare()
+        # rec's activations are kept only when a backward can follow (not under no_grad)
+        save = torch.is_grad_enabled() and rec.requires_grad
+        return _VggLossFunction.apply(imgs.contiguous(), rec.contiguous(), self, save)
+
+    def forward(self, imgs, rec):
+        return self.per_image(imgs, rec).mean()

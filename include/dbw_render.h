@@ -549,6 +549,53 @@ int dbw_lpips_backward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache*
                               int64_t B, int32_t H, int32_t W, int32_t normalize, int32_t train, float* grad_in1, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/*
+ * VGG16 feature-reconstruction loss: the reference's PerceptualLoss (src/model/loss.py:66-111, `perceptual_name:
+ * perceptual`), on the LPIPS kernels above.  in0 (imgs), in1 (rec): (B,3,H,W) fp32 NCHW, 1 <= B <= 65535,
+ * B*H*W < 2^31 - 128, 2^(L-1) <= H, W <= 32767 for the deepest requested level L (its tap is then at least 1x1).
+ *   levels              bit k-1 set: level k used, k = 1..5 (relu1_2, relu2_2, relu3_3, relu4_3, relu5_3); 1..31.
+ *   normalize_input     the first layer reads (x - shift) / scale, shift = mean_rgb, scale = std_rgb (net->shift, ->scale);
+ *                       0: x as is (shift and scale may then be NULL).  LPIPS's 2x - 1 is never applied.
+ *   normalize_features  f / (||f||_2 over channels + 1e-10) before the difference (the LPIPS head with weight w and no
+ *                       dropout; an all-zero feature vector gets no normalisation gradient); 0: f as is.
+ *   sum_channels        w = 1: the squared difference summed over channels, averaged over pixels; 0: w = 1 / C_k, the
+ *                       average over C_k*H_k*W_k.
+ * value[b] = sum over the requested levels k, in increasing order, of (sum_c partial[b][c], in c order) * (1 / (H_k W_k)
+ * in fp32), partial[b][c] the sum of w * (f0 - f1)^2 over channels and pixels 64c .. 64c + 63 of image b's level k.  The
+ * trunk runs only through the deepest requested level (level 3: convolutions 0..6 and two pools), in the arithmetic of the
+ * LPIPS trunk.  conv_w, conv_b and `prepared` of `net` as for LPIPS (dbw_lpips_prepare_weights; lin_w is not read and may
+ * be NULL).
+ *
+ * dbw_vgg_loss_forward writes value (B); with save_for_backward it keeps what dbw_vgg_loss_backward needs.
+ * dbw_vgg_loss_backward writes grad_in1 (B,3,H,W) = sum_b grad_value[b] d value[b] / d in1 from the workspace of a
+ * save_for_backward forward with the same options (the workspace untouched in between).  Both run on `stream` only: no
+ * allocation, no synchronisation (capturable).
+ *
+ * The workspace (dbw_vgg_loss_workspace_bytes for the same B, H, W, options and save_for_backward), in floats, every region
+ * starting at a multiple of 64 floats (its length rounded up to a multiple of 64), in this order:
+ *  - act[l], l = 0..last (last = 1, 3, 6, 9, 12 for L = 1..5): rec's activation after layer l's ReLU, NHWC, as for LPIPS.
+ *    Without save_for_backward only the taps of the requested levels have a region;
+ *  - tap0[k] for the requested levels k, in order: imgs' tap, NHWC (B, H_k, W_k, C_k);
+ *  - s0, s1: scratch of B*H*W*64 floats each;
+ *  - the head partials: per requested level in order (not padded between levels), B x ceil(H_k W_k / 64) floats;
+ *  - 2568 constants the forward writes: per level k, 512 floats whose first C_k hold w; then shift 0 and scale 1 (4 floats
+ *    each), the identity transform used without normalize_input.
+ */
+typedef struct DbwVggLossOptions {
+  int32_t levels;
+  int32_t normalize_input;
+  int32_t normalize_features;
+  int32_t sum_channels;
+} DbwVggLossOptions;
+
+int dbw_vgg_loss_workspace_bytes(int64_t B, int32_t H, int32_t W, const DbwVggLossOptions* opt, int32_t save_for_backward,
+                                 size_t* workspace_bytes);
+int dbw_vgg_loss_forward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* in0, const float* in1, int64_t B,
+                         int32_t H, int32_t W, int32_t save_for_backward, float* value, void* workspace, size_t workspace_bytes,
+                         void* stream);
+int dbw_vgg_loss_backward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B, int32_t H,
+                          int32_t W, float* grad_in1, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
