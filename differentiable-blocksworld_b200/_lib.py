@@ -66,6 +66,18 @@ class DbwVggLossOptions(ctypes.Structure):
                 ('sum_channels', ctypes.c_int32)]
 
 
+class DbwAdamSegment(ctypes.Structure):
+    _fields_ = [('param', ctypes.c_void_p), ('grad', ctypes.c_void_p), ('exp_avg', ctypes.c_void_p), ('exp_avg_sq', ctypes.c_void_p),
+                ('n', ctypes.c_int64), ('group', ctypes.c_int32), ('active', ctypes.c_int32)]
+
+
+class DbwAdamGroup(ctypes.Structure):
+    _fields_ = [('beta1', ctypes.c_double), ('beta2', ctypes.c_double), ('eps', ctypes.c_double), ('weight_decay', ctypes.c_double)]
+
+
+ADAM_MAX_SEGMENTS, ADAM_MAX_GROUPS = 64, 8
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -84,7 +96,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_u
            'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward',
            'dbw_lpips_head_forward', 'dbw_lpips_head_backward',
            'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached',
-           'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward']
+           'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward',
+           'dbw_adam_step']
 
 _lib = None
 
@@ -169,6 +182,7 @@ def lib():
         L.dbw_vgg_loss_workspace_bytes.argtypes = [i64, i32, i32, op, i32, ctypes.POINTER(sz)]
         L.dbw_vgg_loss_forward.argtypes = [np_, op, vp, vp, i64, i32, i32, i32, vp, vp, sz, vp]
         L.dbw_vgg_loss_backward.argtypes = [np_, op, vp, i64, i32, i32, vp, vp, sz, vp]
+        L.dbw_adam_step.argtypes = [vp, i32, i64, ctypes.POINTER(DbwAdamGroup), i32, vp, vp, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

@@ -8,15 +8,24 @@ shape that depends on parameter values inside forward().
 Camera-pose gradients (a ViewParallel built with max_pose_views > 0, and poses that require grad in example_inp): the inputs
 are the full batch; the step keeps this rank's slice of the per-view inputs and the full-batch poses as static LEAF buffers
 that require grad, renders from their slices inside the graph, and after each replay back-propagates the (summed) pose
-gradient into the caller's graph behind run()'s inp['R'] / inp['T'] -- a small eager backward outside the graph."""
+gradient into the caller's graph behind run()'s inp['R'] / inp['T'] -- a small eager backward outside the graph.
+
+The parameter update (GraphedStep(optimizer=BucketAdam)): the optimiser's one launch (optim.py) is captured after the point
+where the gradients are final -- the captured all-reduce, or the backward when the sum happens inside it or there is one rank
+-- so one replay is one training iteration.  Every rank applies the same elementwise update to the same summed gradients.  The
+learning rates are read on the device: a scheduler changes them between replays without a new capture."""
 import torch
 
+from .optim import BucketAdam
 from .parallel import pose_backward, refuse_camera_gradients, wants_pose_gradients
 
 
 class GraphedStep:
-    def __init__(self, view_parallel, example_inp, n_total_views, warmup=3, capture_all_reduce=None, generator=None):
+    def __init__(self, view_parallel, example_inp, n_total_views, warmup=3, capture_all_reduce=None, generator=None, optimizer=None):
         self.vp, self.model = view_parallel, view_parallel.model
+        if optimizer is not None and not isinstance(optimizer, BucketAdam):
+            raise TypeError('GraphedStep: only an optim.BucketAdam can be captured (its launch reads rates and counters on the device)')
+        self.optimizer = optimizer
         self.pose = None                   # (R, T, views): static full-batch pose leaves and this rank's views of them
         if wants_pose_gradients(example_inp):
             view_parallel.check_pose_views(example_inp, 'GraphedStep')
@@ -29,6 +38,9 @@ class GraphedStep:
         if capture_all_reduce is None:
             capture_all_reduce = view_parallel.graph_capturable_collective
         self.capture_all_reduce = capture_all_reduce and view_parallel.world_size > 1
+        if optimizer is not None and view_parallel.world_size > 1 and not self.capture_all_reduce:
+            raise RuntimeError('GraphedStep: with an optimizer the gradient sum must be captured too (capture_all_reduce=True, the '
+                               'peer-memory collective): a collective issued after the replay would come after the update')
         self.n_total = n_total_views
         dev = example_inp['imgs'].device
         self.static_inp = {k: v.clone() for k, v in example_inp.items()}
@@ -45,12 +57,14 @@ class GraphedStep:
             self.gen = torch.Generator(device=dev)
             self.gen.manual_seed(self.vp.seed)
         self.model._install_cameras(self.static_inp)          # the one-off host read of the intrinsics happens here
+        self.segment_table = optimizer.new_segment_table() if optimizer is not None else None
         self._capture(warmup=warmup)
 
     def _phase(self):
         """what the captured control flow depends on: the training-schedule switches of dbw.py:210-212,276,331-334"""
         m = self.model
-        return (m.training, m.is_live('coarse_learning'), m.is_live('decimate_txt'), m.is_live('kill_blocks'))
+        frozen = self.optimizer.captured_constants() if self.optimizer is not None else ()      # a capture holds them by value
+        return (m.training, m.is_live('coarse_learning'), m.is_live('decimate_txt'), m.is_live('kill_blocks'), *frozen)
 
     def _bind_buffers(self):
         self.model.opacity_noise_buffer, self.model.overlap_samples_buffer = self.noise_buf, self.overlap_buf
@@ -76,6 +90,13 @@ class GraphedStep:
         # the gradient tensors THIS capture writes (bucket views when the gradients are gathered, else tensors of the graph's
         # private pool): another GraphedStep on the same model (PipelinedGraphedStep) leaves its own in the .grad attributes
         self.grads = [p.grad for p in self.vp.bucket.params]
+        if self.optimizer is not None:
+            # the records the captured launch reads, written now that the capture has fixed the gradients' addresses; a parameter
+            # is active when this phase's backward gave it a gradient (torch.optim skips a .grad that is None: hard opacities
+            # leave alpha_logit alone, whereas the bucket's zeros would keep moving it on old momentum)
+            got = {id(p) for p, r in zip(self.vp.bucket.params, self.vp.bucket.received) if r}
+            self.optimizer.write_segments(self.segment_table, [p.grad for p in self.optimizer.params],
+                                          active=[id(p) in got for p in self.optimizer.params])
         self.pose_grads = self.vp.pose_grads(self.pose) if self.pose is not None else None
 
     def _body(self):
@@ -83,6 +104,8 @@ class GraphedStep:
         self.inside = self.vp.reduces_inside_backward(self.static_inp)      # the collective sits INSIDE the backward (parallel.GradSumPoint)
         if self.capture_all_reduce and not reduced:
             self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views)
+        if self.optimizer is not None and torch.cuda.is_current_stream_capturing():      # the warm-up runs must not train
+            self.optimizer.launch(self.segment_table)
         return losses
 
     @property
@@ -118,9 +141,12 @@ class GraphedStep:
     def run(self, inp=None, non_blocking=True, all_reduce=True):
         """inp: optional dict of (host or device) tensors for this step, copied into the static buffers.
         all_reduce=False skips the collective when it is issued after the replay (a captured one always runs).
+        With an optimizer the replay also applies the update, at the learning rates param_groups hold now.
         With pose gradients, inp holds the full batch, and the summed pose gradient is back-propagated into the graph
         behind inp['R'] / inp['T'] (without them, it stays in the static leaves' .grad)."""
         self.check_poses(inp)
+        if self.optimizer is not None and not all_reduce and self.vp.world_size > 1:
+            raise RuntimeError('GraphedStep: run(all_reduce=False) with an optimizer would update from gradients that are not summed')
         if inp is not None:
             if self.pose is not None:
                 self.load_poses(inp, non_blocking)
@@ -132,6 +158,8 @@ class GraphedStep:
         self.noise_buf.normal_(generator=self.gen)                      # identical on every rank (same seed, same count)
         if self.overlap_buf is not None:
             self.overlap_buf.uniform_(generator=self.gen)
+        if self.optimizer is not None:
+            self.optimizer.prepare_replay()
         self.graph.replay()
         for p, g in zip(self.vp.bucket.params, self.grads):
             p.grad = g
@@ -155,12 +183,13 @@ class PipelinedGraphedStep:
     change them between the prefetch and the step that consumes them, so they are copied into that step's static leaves on
     the current stream right before its replay."""
 
-    def __init__(self, view_parallel, example_inp, n_total_views, capture_all_reduce=None):
+    def __init__(self, view_parallel, example_inp, n_total_views, capture_all_reduce=None, optimizer=None):
         if wants_pose_gradients(example_inp):
             view_parallel.check_pose_views(example_inp, 'PipelinedGraphedStep')
         gen = torch.Generator(device=example_inp['imgs'].device)
         gen.manual_seed(view_parallel.seed)
-        self.steps = [GraphedStep(view_parallel, example_inp, n_total_views, capture_all_reduce=capture_all_reduce, generator=gen)
+        self.steps = [GraphedStep(view_parallel, example_inp, n_total_views, capture_all_reduce=capture_all_reduce, generator=gen,
+                                  optimizer=optimizer)
                       for _ in range(2)]
         self.copy_stream = torch.cuda.Stream()
         self.ready = [torch.cuda.Event(), torch.cuda.Event()]      # inputs of buffer b have landed
@@ -198,4 +227,34 @@ class PipelinedGraphedStep:
         losses = self.steps[b].run(poses, all_reduce=all_reduce)
         self.free[b].record(cur)
         self.i += 1
+        return losses
+
+
+class GraphedModel:
+    """A captured step with its optimiser, behind the call sequence of the reference's training loop (src/trainer.py:137-147:
+    `optimizer.zero_grad(); loss = model(inp, labels); loss['total'].backward(); optimizer.step()`), which cannot call
+    step.run().  The call replays the step, update included; the `total` it returns back-propagates into nothing, and the
+    BucketAdam skips the step() call that follows.  Everything else (train(), step(), predict(), state_dict(), ...) is the
+    wrapped model's."""
+
+    def __init__(self, step):
+        if step.optimizer is None:
+            raise ValueError('GraphedModel: the step must be built with an optimizer')
+        self.graphed_step, self.model = step, step.model
+
+    def __getattr__(self, name):
+        if name in ('model', 'graphed_step'):          # not set yet (copying, unpickling): no delegation to a missing model
+            raise AttributeError(name)
+        return getattr(self.model, name)
+
+    def __call__(self, inp, labels=None):
+        step = self.graphed_step
+        if not self.model.training:
+            raise RuntimeError('GraphedModel: the captured step is a training iteration; call the model itself to evaluate')
+        if len(inp['imgs']) != len(step.static_inp['imgs']):
+            raise ValueError(f"GraphedModel: a batch of {len(inp['imgs'])} views, but the step was captured for "
+                             f"{len(step.static_inp['imgs'])} (drop the last, smaller batch of an epoch)")
+        losses = dict(step.run(inp))
+        step.optimizer.skip_next_step()
+        losses['total'] = losses['total'].detach().clone().requires_grad_(True)      # a leaf: backward() reaches no parameter
         return losses

@@ -206,6 +206,7 @@ class GradBucket:
             self._all = torch.zeros(n_all, dtype=ref.dtype, device=ref.device)
         self.flat = self._all[:n_pad]               # the parameter gradients; the pose region follows it
         self._zeros = {}
+        self.received = None                         # per parameter: the last backward() produced a gradient for it
         off, self.views = 0, []
         for p in self.params:
             self.views.append(self.flat[off:off + p.numel()].view_as(p))
@@ -229,6 +230,7 @@ class GradBucket:
         for p in (*self.params, *poses):
             p.grad = None
         total.backward()
+        self.received = [p.grad is not None for p in self.params]      # before the gather gives every parameter a bucket view
         if not gather:
             return
         pieces = [(p.grad if p.grad is not None else self._zero(p.numel())).reshape(-1) for p in self.params]

@@ -596,6 +596,43 @@ int dbw_vgg_loss_forward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, c
 int dbw_vgg_loss_backward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B, int32_t H,
                           int32_t W, float* grad_in1, void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Optimiser: one Adam step over every parameter tensor of a model in ONE launch -- torch.optim.Adam's single-tensor path
+ * with amsgrad=False, maximize=False:
+ *   g = grad + weight_decay p (when weight_decay != 0);  m = m + (1 - beta1)(g - m);  v = beta2 v + (1 - beta2) g g;
+ *   t = ++step;  p -= (lr / (1 - beta1^t)) m / (sqrt(v) / sqrt(1 - beta2^t) + eps),
+ * the bias corrections in double from the device counter.  The learning rates and the counters are read on the device, so a
+ * captured launch replays with whatever they hold then.  No allocation, no synchronisation, no host read (capturable).
+ *
+ *   segments  DEVICE, n_segments <= DBW_ADAM_MAX_SEGMENTS records, one per parameter tensor: param, grad, exp_avg, exp_avg_sq
+ *             of n fp32 each (float4 accesses where param, exp_avg and exp_avg_sq are 16-byte aligned; grad may sit anywhere),
+ *             its group in [0, n_groups), and active.  active = 0 -- the tensor received no gradient this step, torch's
+ *             "p.grad is None" -- leaves the parameter, both moments and the counter untouched; so does a record with a null
+ *             pointer, n <= 0 or a group out of range.
+ *   n_total   the sum of the segments' n: sizes the grid (the kernel itself reads the lengths from the records).
+ *   groups    HOST, n_groups <= DBW_ADAM_MAX_GROUPS, copied by value into the launch.  Doubles, as torch holds them: the
+ *             per-step scalars are formed in double and then rounded ((float)(1 - 0.999), not 1 - (float)0.999).
+ *   lr        DEVICE (n_groups) fp32.
+ *   step      DEVICE (n_segments) int64, 8-byte aligned, values in [0, 2^40): steps taken so far per segment, advanced by the
+ *             kernel.  While the kernel runs, bits 40.. of step[0] count the CTAs that are done; they are zero again when it
+ *             ends.
+ */
+#define DBW_ADAM_MAX_SEGMENTS 64
+#define DBW_ADAM_MAX_GROUPS 8
+typedef struct DbwAdamSegment {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  int64_t n;
+  int32_t group;
+  int32_t active;
+} DbwAdamSegment;
+typedef struct DbwAdamGroup { double beta1, beta2, eps, weight_decay; } DbwAdamGroup;
+
+int dbw_adam_step(const DbwAdamSegment* segments, int32_t n_segments, int64_t n_total, const DbwAdamGroup* groups,
+                  int32_t n_groups, const float* lr, int64_t* step, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

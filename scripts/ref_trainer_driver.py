@@ -1,12 +1,14 @@
 """Drives the reference's UNMODIFIED `src/trainer.py` (+ optimizer.py, scheduler.py, utils/*, configs/dtu/*.yml) on this repo's
 model, from a checkout of monniert/differentiable-blocksworld.
 
-    python scripts/ref_trainer_driver.py --reference /path/to/differentiable-blocksworld <run_dir> [--iters N]
+    python scripts/ref_trainer_driver.py --reference /path/to/differentiable-blocksworld <run_dir> [--iters N] [--graphed]
 
 What is swapped (INTEGRATION.md A, nothing in the reference tree is edited or copied):
   * `model.create_model`                 -> dbw_b200.dbw.create_model   (the drop-in)
   * `dataset.create_train_val_test_loader` -> a synthetic multi-view loader (no DTU images on disk here)
   * missing third-party modules          -> dbw_b200.compat stand-ins
+  * with --graphed (needs a GPU), also `optimizer.create_optimizer` -> dbw_b200.optim.create_optimizer, and the trainer's model
+    becomes a dbw_b200.graph.GraphedModel: every `run_single_batch_train` is one replay of a captured step, update included
 
 With a GPU the model renders for real.  WITHOUT one the product renderer refuses to run -- there is
 no CPU fallback, by design -- so this driver replaces the model's three render entry points by parameter-touching dummies and
@@ -77,7 +79,10 @@ def main():
     ap.add_argument('run_dir')
     ap.add_argument('--reference', required=True, help='checkout of monniert/differentiable-blocksworld')
     ap.add_argument('--iters', type=int, default=3)
+    ap.add_argument('--graphed', action='store_true', help='train through a captured step with the update inside (needs a GPU)')
     args = ap.parse_args()
+    if args.graphed and not torch.cuda.is_available():
+        sys.exit('--graphed needs a GPU: a captured step has no stand-in')
     ref = os.path.abspath(args.reference)
     shimmed = compat.install()
     sys.path.insert(0, os.path.join(ref, 'src'))
@@ -85,6 +90,10 @@ def main():
     import model as ref_model
     ref_model.create_model = b200.create_model
     ref_dataset.create_train_val_test_loader = synthetic_loaders
+    if args.graphed:
+        import optimizer as ref_optimizer
+        from dbw_b200.optim import create_optimizer
+        ref_optimizer.create_optimizer = create_optimizer
     import trainer as ref_trainer                          # the reference's file, unmodified
     from utils import load_yaml                            # the reference's config loader (scan24.yml + default.yml merge)
     assert os.path.realpath(ref_trainer.__file__).startswith(ref)
@@ -102,6 +111,12 @@ def main():
         T = ref_trainer.Trainer(cfg, run_dir, seed=cfg['training']['seed'])
     if T.model.loss_weights.get('perceptual') and getattr(T.model, 'perceptual_loss', None) is None:
         T.model.set_perceptual_loss(lambda imgs, rec: (imgs - rec).abs().mean())        # stand-in callable (no LPIPS weights here)
+    if args.graphed:
+        from dbw_b200.graph import GraphedModel, GraphedStep
+        from dbw_b200.parallel import ViewParallel
+        example = {k: v.to(T.device) for k, v in next(iter(T.train_loader))[0].items()}
+        T.model.train()
+        T.model = GraphedModel(GraphedStep(ViewParallel(T.model), example, len(example['imgs']), optimizer=T.optimizer))
     groups = [len(g['params']) for g in T.optimizer.param_groups]
     lrs = [g['lr'] for g in T.optimizer.param_groups]
     before = {n: p.detach().clone() for n, p in T.model.named_parameters()}
@@ -118,7 +133,7 @@ def main():
     T.save(epoch=1, batch=it)
     moved = sorted(n for n, p in T.model.named_parameters() if not torch.equal(p.detach(), before[n]))
     ckpt = torch.load(run_dir / 'model.pkl', map_location='cpu', weights_only=False)
-    out = {'shimmed': shimmed, 'stubbed_render': stubbed, 'device': str(T.device), 'loss_names': T.model.loss_names,
+    out = {'shimmed': shimmed, 'stubbed_render': stubbed, 'graphed': args.graphed, 'optimizer': type(T.optimizer).__name__, 'device': str(T.device), 'loss_names': T.model.loss_names,
            'param_groups': groups, 'lrs': lrs, 'moved': moved, 'cur_epoch': T.model.cur_epoch,
            'checkpoint_keys': sorted(ckpt['model_state'].keys()), 'model_name': ckpt['model_name'],
            'train_metrics_rows': len(open(run_dir / 'train_metrics.tsv').read().strip().splitlines()),
