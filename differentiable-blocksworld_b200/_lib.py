@@ -85,6 +85,7 @@ class DbwMapDesc(ctypes.Structure):
 
 EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
            'dbw_render_forward_loss', 'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
+           'dbw_camera_project', 'dbw_camera_project_backward',
            'dbw_composite_mse', 'dbw_composite_mse_backward', 'dbw_render_forward_host', 'dbw_host_arena_release', 'dbw_launch_count',
            'dbw_timing_enable', 'dbw_timing_read', 'dbw_timing_reset', 'dbw_scene_geometry_forward', 'dbw_scene_geometry_backward',
            'dbw_opacity_forward', 'dbw_opacity_backward', 'dbw_texture_prep_forward_multi', 'dbw_texture_prep_backward_multi',
@@ -125,6 +126,8 @@ def lib():
         L.dbw_render_forward_loss_grad.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz, ctypes.POINTER(DbwLossEpilogue),
                                                                                                ctypes.c_int32, vp, sz, vp]
         L.dbw_render_backward_deferred.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 7 + [sz, vp]
+        L.dbw_camera_project.argtypes = [ctypes.c_int32, ctypes.c_int32] + [vp] * 4 + [ctypes.c_float, vp, vp]
+        L.dbw_camera_project_backward.argtypes = [ctypes.c_int32, ctypes.c_int32] + [vp] * 4 + [ctypes.c_float] + [vp] * 6
         L.dbw_composite_mse.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
         L.dbw_composite_mse_backward.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
         L.dbw_render_forward_host.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 6

@@ -305,6 +305,137 @@ __global__ void __launch_bounds__(DBW_CAM_NT) camera_grad_kernel(const float* __
   }
 }
 
+// ------------------------------------------------------------------------------------------------ per-view projection
+// dbw_camera_project: project_verts_kernel's arithmetic with each view's own (fx, fy, px, py) read from intr (B,4)
+__global__ void camera_project_kernel(const float* __restrict__ vw, const float* __restrict__ R, const float* __restrict__ T,
+                                      const float* __restrict__ intr, float eps, int B, int V, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * V) return;
+  const int b = i / V, v = i - b * V;
+  const float fx = intr[b * 4], fy = intr[b * 4 + 1], px = intr[b * 4 + 2], py = intr[b * 4 + 3];
+  const float X = vw[v * 3], Y = vw[v * 3 + 1], Z = vw[v * 3 + 2];
+  const float* r = R + b * 9; const float* t = T + b * 3;
+  const float xv = X * r[0] + Y * r[3] + Z * r[6] + t[0];
+  const float yv = X * r[1] + Y * r[4] + Z * r[7] + t[1];
+  const float zv = X * r[2] + Y * r[5] + Z * r[8] + t[2];
+  const float sgn = (zv > 0.f) ? 1.f : ((zv < 0.f) ? -1.f : 1.f);
+  const float den = sgn * fmaxf(fabsf(zv), eps);
+  out[i * 3] = (fx * xv + px * zv) / den;
+  out[i * 3 + 1] = (fy * yv + py * zv) / den;
+  out[i * 3 + 2] = zv;
+}
+
+// world-vertex gradient of dbw_camera_project: project_verts_backward_kernel with per-view intrinsics (one warp per vertex,
+// lanes over the views, no atomics: g_vw receives one add per element)
+__global__ void camera_project_verts_backward_kernel(const float* __restrict__ vw, const float* __restrict__ R,
+                                                     const float* __restrict__ T, const float* __restrict__ intr, float eps,
+                                                     int B, int V, const float* __restrict__ g_ndc, float* __restrict__ g_vw) {
+  const int v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (v >= V) return;
+  const float X = vw[v * 3], Y = vw[v * 3 + 1], Z = vw[v * 3 + 2];
+  float ax = 0.f, ay = 0.f, az = 0.f;
+  for (int b = lane; b < B; b += 32) {
+    const float* r = R + b * 9; const float* t = T + b * 3; const float* k = intr + b * 4;
+    const float* g = g_ndc + ((size_t)b * V + v) * 3;
+    float gxv, gyv, gzv;
+    dbw_project_backward(X, Y, Z, r, t, k[0], k[1], k[2], k[3], eps, g[0], g[1], g[2], gxv, gyv, gzv);
+    ax += r[0] * gxv + r[1] * gyv + r[2] * gzv;
+    ay += r[3] * gxv + r[4] * gyv + r[5] * gzv;
+    az += r[6] * gxv + r[7] * gyv + r[8] * gzv;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ax += __shfl_xor_sync(0xffffffffu, ax, o); ay += __shfl_xor_sync(0xffffffffu, ay, o); az += __shfl_xor_sync(0xffffffffu, az, o);
+  }
+  if (lane == 0) { g_vw[v * 3] += ax; g_vw[v * 3 + 1] += ay; g_vw[v * 3 + 2] += az; }
+}
+
+// camera gradient of dbw_camera_project: camera_grad_kernel's fixed-order per-view sums, with the view's 4 intrinsics
+// sums after its 9 + 3 pose sums; each element of g_R / g_T / g_intr receives one atomic add per call
+#define DBW_CAMK_N 16
+__global__ void __launch_bounds__(DBW_CAM_NT) camera_project_camera_backward_kernel(
+    const float* __restrict__ vw, const float* __restrict__ R, const float* __restrict__ T, const float* __restrict__ intr,
+    float eps, int V, const float* __restrict__ g_ndc, float* __restrict__ g_R, float* __restrict__ g_T, float* __restrict__ g_intr) {
+  __shared__ float s_part[DBW_CAM_NT / 32][DBW_CAMK_N];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* r = R + b * 9; const float* t = T + b * 3;
+  const float fx = intr[b * 4], fy = intr[b * 4 + 1], px = intr[b * 4 + 2], py = intr[b * 4 + 3];
+  float acc[DBW_CAMK_N];                                         // g_R (9), g_T (3), g_intr (4)
+#pragma unroll
+  for (int k = 0; k < DBW_CAMK_N; ++k) acc[k] = 0.f;
+  for (int v = tid; v < V; v += DBW_CAM_NT) {
+    const float* g = g_ndc + ((size_t)b * V + v) * 3;
+    const float gx = g[0], gy = g[1], gz = g[2];
+    if (gx == 0.f && gy == 0.f && gz == 0.f) continue;          // a vertex no face of this view differentiated
+    const float X = vw[v * 3], Y = vw[v * 3 + 1], Z = vw[v * 3 + 2];
+    float gxv, gyv, gzv;
+    dbw_project_backward(X, Y, Z, r, t, fx, fy, px, py, eps, gx, gy, gz, gxv, gyv, gzv);
+    dbw_camera_accumulate(X, Y, Z, gxv, gyv, gzv, acc, acc + 9);
+    dbw_intrinsics_accumulate(X, Y, Z, r, t, eps, gx, gy, acc + 12);
+  }
+#pragma unroll
+  for (int k = 0; k < DBW_CAMK_N; ++k) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < DBW_CAMK_N; ++k) s_part[warp][k] = acc[k];
+  }
+  __syncthreads();
+  if (tid < DBW_CAMK_N) {
+    float s = 0.f;
+    for (int w = 0; w < DBW_CAM_NT / 32; ++w) s += s_part[w][tid];
+    float* dst = tid < 9 ? (g_R ? g_R + b * 9 + tid : nullptr)
+               : tid < 12 ? (g_T ? g_T + b * 3 + (tid - 9) : nullptr)
+                          : (g_intr ? g_intr + b * 4 + (tid - 12) : nullptr);
+    if (dst && s != 0.f) atomicAdd(dst, s);
+  }
+}
+
+static int check_camera_project(const char* who, int32_t n_views, int32_t n_verts, const float* verts, const float* R,
+                                const float* T, const float* intrinsics, float eps) {
+  char msg[200];
+  const char* why = (n_views <= 0 || n_verts <= 0) ? "n_views and n_verts must be positive"
+                  : ((long long)n_views * n_verts * 3 > 0x7fffffffLL || (long long)n_verts * 32 > 0x7fffffffLL)
+                      ? "too many views or vertices for one call (32-bit indexing)"
+                  : (!verts || !R || !T || !intrinsics) ? "verts, R, T and intrinsics are required"
+                  : !(eps > 0.f) ? "eps must be positive"
+                  : nullptr;
+  if (!why) return 0;
+  snprintf(msg, sizeof(msg), "%s: %s", who, why);
+  return fail(msg);
+}
+
+extern "C" int dbw_camera_project(int32_t n_views, int32_t n_verts, const float* verts, const float* R, const float* T,
+                                  const float* intrinsics, float eps, float* verts_ndc, void* stream) {
+  if (check_camera_project("dbw_camera_project", n_views, n_verts, verts, R, T, intrinsics, eps)) return -1;
+  if (!verts_ndc) return fail("dbw_camera_project: verts_ndc is required");
+  const int n = n_views * n_verts;
+  camera_project_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(verts, R, T, intrinsics, eps, n_views, n_verts, verts_ndc);
+  LAUNCH_CK("camera_project_kernel");
+  return 0;
+}
+
+extern "C" int dbw_camera_project_backward(int32_t n_views, int32_t n_verts, const float* verts, const float* R, const float* T,
+                                           const float* intrinsics, float eps, const float* g_ndc, float* g_verts, float* g_R,
+                                           float* g_T, float* g_intrinsics, void* stream) {
+  if (check_camera_project("dbw_camera_project_backward", n_views, n_verts, verts, R, T, intrinsics, eps)) return -1;
+  if (!g_ndc) return fail("dbw_camera_project_backward: g_ndc is required");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g_verts) {
+    camera_project_verts_backward_kernel<<<(n_verts * 32 + 127) / 128, 128, 0, st>>>(verts, R, T, intrinsics, eps, n_views, n_verts,
+                                                                                      g_ndc, g_verts);
+    LAUNCH_CK("camera_project_verts_backward_kernel");
+  }
+  if (g_R || g_T || g_intrinsics) {
+    camera_project_camera_backward_kernel<<<n_views, DBW_CAM_NT, 0, st>>>(verts, R, T, intrinsics, eps, n_verts, g_ndc, g_R, g_T,
+                                                                          g_intrinsics);
+    LAUNCH_CK("camera_project_camera_backward_kernel");
+  }
+  return 0;
+}
+
 // order-preserving float <-> int map, so that atomicMin/atomicMax on ints order floats of either sign
 __device__ __forceinline__ int f2ord(float f) { const int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }

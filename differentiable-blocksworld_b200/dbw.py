@@ -117,6 +117,7 @@ class DifferentiableBlocksWorld(nn.Module):
         self.alpha_group_faces = None     # None: one opacity entry per block (alpha_group = BNF); 1: one per face, as dbw.py:219 packs them
         self.n_total_views = None         # data-parallel context (parallel.py): views of the whole step
         self.grad_sum_point = None        # likewise: parallel.GradSumPoint, sums the scene tensors' gradients over ranks inside the backward
+        self.per_view_intrinsics = False  # False: the reference's cameras (K[0] of the first batch for every view, read once)
         self.noise_generator = None       # RNG shared by all ranks for opacity noise / overlap samples
         self.opacity_noise_buffer = None  # pre-drawn randn (N,) used instead of drawing inside forward (graph.py)
         self.overlap_samples_buffer = None  # pre-drawn U(0,1) (N,1000,3) for the overlap term, likewise
@@ -257,9 +258,22 @@ class DifferentiableBlocksWorld(nn.Module):
         rec = self._composite(env_rgba, fg_rgba)
         return self.compute_losses(imgs, rec, rgb_loss=self.criterion(imgs, rec) * (len(imgs) / float(n_total)))
 
+    def set_per_view_intrinsics(self, on=True):
+        """on: every render reads inp['K'] (B,4,4) on the device and draws each view with its own intrinsics (fx, fy, px, py),
+        with no host read; off (the default): the reference's behaviour, the first batch's K[0] for every view.  A call whose
+        inp['K'] requires grad renders per view either way, and K then receives its gradient."""
+        self.per_view_intrinsics = bool(on)
+        return self
+
+    def _view_K(self, inp):
+        """inp['K'] when this call renders each view with its own intrinsics, else None (the renderers' one camera)"""
+        K = inp.get('K')
+        return K if torch.is_tensor(K) and (self.per_view_intrinsics or K.requires_grad) else None
+
     def _install_cameras(self, inp):
-        """dbw.py:204-208: the first batch's intrinsics become the cameras of all four renderers"""
-        if 'K' in inp and self.renderer.cameras.K is None:
+        """dbw.py:204-208: the first batch's intrinsics become the cameras of all four renderers (not needed, and no host
+        read, when the call renders with per-view intrinsics)"""
+        if 'K' in inp and self.renderer.cameras.K is None and self._view_K(inp) is None:
             for r in self._renderers():
                 r.update_cameras(device=inp['imgs'].device, K=inp['K'][0:1])
                 r.cameras.intrinsics()          # the one host read of K happens here, never inside a step
@@ -270,7 +284,7 @@ class DifferentiableBlocksWorld(nn.Module):
 
     def _render_layers(self, inp, filter_transparent=False):
         """(environment RGBA, blocks RGBA) in decoupled mode (every shipped config), (whole-scene RGBA, None) otherwise"""
-        B, R, T = len(inp['imgs']), inp['R'], inp['T']
+        B, R, T, K = len(inp['imgs']), inp['R'], inp['T'], self._view_K(inp)
         self._install_cameras(inp)
         fine, hard_filter, renderer = self._phase(filter_transparent)
         if not self.decouple_rendering:
@@ -278,20 +292,20 @@ class DifferentiableBlocksWorld(nn.Module):
             alpha = None
             if not hard_filter:
                 alpha = torch.cat([torch.ones(self.env_n_faces, device=R.device), self._alpha.repeat_interleave(self.BNF)])
-            return renderer(scene.extend(B), R=R, T=T, faces_alpha=alpha), None
+            return renderer(scene.extend(B), R=R, T=T, faces_alpha=alpha, K=K), None
         if self._fused_scene_ok(R):
-            return self._render_decoupled_fused(R, T, hard_filter, renderer)
+            return self._render_decoupled_fused(R, T, hard_filter, renderer, K)
         env = join_meshes_as_scene([self.build_bkg(world_coord=True), self.build_ground(world_coord=True)])
-        env_rgba = self.renderer_env(env.extend(B), R=R, T=T)
+        env_rgba = self.renderer_env(env.extend(B), R=R, T=T, K=K)
         if self.static_topology:
             verts, faces, fvu, fmap, maps, table = self._blocks_static(hard_filter)
             alpha = None if hard_filter else self._alpha.repeat_interleave(self.BNF)
-            return env_rgba, self._raster(renderer, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4=False)
+            return env_rgba, self._raster(renderer, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4=False, K=K)
         blocks = self.build_blocks(filter_transparent=hard_filter, as_scene=True)
         if len(blocks) == 0:
             return env_rgba, torch.zeros_like(env_rgba)
         alpha = None if hard_filter else self._alpha.repeat_interleave(self.BNF)
-        return env_rgba, renderer(blocks.extend(B), R=R, T=T, faces_alpha=alpha)
+        return env_rgba, renderer(blocks.extend(B), R=R, T=T, faces_alpha=alpha, K=K)
 
     def _fused_scene_ok(self, ref):
         """the fused scene kernels apply: static topology on the GPU, and a box decimation the texture-prep kernel has
@@ -300,8 +314,9 @@ class DifferentiableBlocksWorld(nn.Module):
         return (self.static_topology and self.fused_scene and ref.is_cuda and (not decim_live or self.decim_factor in (1, 8)))
 
     @staticmethod
-    def _raster(r, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4, alpha_group=1, n_static_faces=0):
-        return render_scene(verts, faces, fvu, fmap, maps, table, R, T, r.cameras.intrinsics(), r.img_size, r.sigma,
+    def _raster(r, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4, alpha_group=1, n_static_faces=0, K=None):
+        intr = K if K is not None else r.cameras.intrinsics()          # K (B,4,4): per-view intrinsics (render_scene)
+        return render_scene(verts, faces, fvu, fmap, maps, table, R, T, intr, r.img_size, r.sigma,
                             r.faces_per_pixel, r.z_clip, r.detach_bary, r.clip_inside, r.background_color, alpha,
                             r.perspective_correct, blur_radius=r.blur_radius, maps_are_texels4=texels4,
                             alpha_group=alpha_group, n_static_faces=n_static_faces)
@@ -419,14 +434,14 @@ class DifferentiableBlocksWorld(nn.Module):
             alpha = alpha[:, None].expand(-1, self.BNF).reshape(-1)
         return alpha
 
-    def _render_decoupled_fused(self, R, T, hard_filter, renderer):
+    def _render_decoupled_fused(self, R, T, hard_filter, renderer, K=None):
         """environment pass + blocks pass over the fused scene tensors -> (env RGBA, blocks RGBA)"""
         st = self._static_arrays()
         (env_verts, env_atlas, env_table), (blk_verts, atlas, table, fmap, alpha) = self._scene_tensors(hard_filter)
         env_rgba = self._raster(self.renderer_env, env_verts, st['faces_e'], st['fvu_e'], st['fmap_e'], env_atlas, env_table,
-                                R, T, None, texels4=True, n_static_faces=self.bkg_n_faces)
+                                R, T, None, texels4=True, n_static_faces=self.bkg_n_faces, K=K)
         fg_rgba = self._raster(renderer, blk_verts, st['faces_b'], st['fvu_b'], fmap, atlas, table, R, T, alpha, texels4=True,
-                               alpha_group=self.alpha_group_faces or self.BNF)
+                               alpha_group=self.alpha_group_faces or self.BNF, K=K)
         return env_rgba, fg_rgba
 
     def _fused_loss_ok(self, imgs):
@@ -448,8 +463,11 @@ class DifferentiableBlocksWorld(nn.Module):
                             ScenePass(st['faces_b'], st['fvu_b'], st['fmap_b'], table, renderer, alpha_group=self.alpha_group_faces or self.BNF))
         # data parallel with pose gradients: the poses are this rank's slices of pose leaves that went through the sum point
         R, T = self.grad_sum_point.cameras(inp) if self.grad_sum_point is not None else (inp['R'], inp['T'])
+        K = self._view_K(inp)
+        if self.grad_sum_point is not None:            # intrinsics leaves riding through the point replace inp's K
+            K = self.grad_sum_point.intrinsics(K)
         return scene_mse(env_verts, env_atlas, blk_verts, atlas, alpha, R, T, inp['imgs'], self._passes[1],
-                         self._passes[2], fmap, n_total_views=self.n_total_views or len(inp['imgs']), view_rows=inp.get('rows'))
+                         self._passes[2], fmap, n_total_views=self.n_total_views or len(inp['imgs']), view_rows=inp.get('rows'), K=K)
 
     def can_sum_gradients_at_scene_tensors(self, imgs):
         """the step's gradients may be summed over data-parallel ranks at the scene tensors (vertices, opacities, texture CELLS)
@@ -576,7 +594,7 @@ class DifferentiableBlocksWorld(nn.Module):
             if len(blocks) > 0:
                 parts.append(blocks)
             colors = self.get_scene_face_colors(filter_transparent=hard_filter).repeat(B, 1)
-            rec = renderer.draw_edges(rec, join_meshes_as_scene(parts).extend(B), inp['R'], inp['T'], colors=colors)
+            rec = renderer.draw_edges(rec, join_meshes_as_scene(parts).extend(B), inp['R'], inp['T'], colors=colors, K=self._view_K(inp))
         return rec
 
     def predict_synthetic(self, inp, labels=None):
@@ -585,7 +603,7 @@ class DifferentiableBlocksWorld(nn.Module):
         blocks = self.build_blocks(filter_transparent=True, synthetic_colors=True, as_scene=True)
         if len(blocks) == 0:
             return torch.ones_like(inp['imgs'])
-        return self.renderer_light(blocks.extend(len(inp['imgs'])), R=inp['R'], T=inp['T'], viz_purpose=True)[:, :3]
+        return self.renderer_light(blocks.extend(len(inp['imgs'])), R=inp['R'], T=inp['T'], viz_purpose=True, K=self._view_K(inp))[:, :3]
 
     @torch.no_grad()
     def get_scene_face_colors(self, filter_transparent=False, w_env=True):
@@ -681,7 +699,7 @@ class DifferentiableBlocksWorld(nn.Module):
             inp = {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in inp.items()}
             self._install_cameras(inp)
             imgs, n = inp['imgs'], len(inp['imgs'])
-            rec = (self.renderer(scene.extend(n), inp['R'], inp['T'], viz_purpose=True)[:, :3] if hard_inference
+            rec = (self.renderer(scene.extend(n), inp['R'], inp['T'], viz_purpose=True, K=self._view_K(inp))[:, :3] if hard_inference
                    else self.predict(inp, labels, filter_transparent=True))
             losses = self.compute_losses(imgs, rec)
             sums['L_tot'] += float(losses['total']) * n
@@ -721,17 +739,19 @@ class DifferentiableBlocksWorld(nn.Module):
                 break
             inp = {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in inp.items()}
             self._install_cameras(inp)
+            K_all = self._view_K(inp)
             for k in range(min(len(inp['imgs']), n_inputs - count)):
                 tag = str(count).zfill(n_zeros)
                 img, R, T = inp['imgs'][k:k + 1], inp['R'][k:k + 1], inp['T'][k:k + 1]
+                K = K_all[k:k + 1] if K_all is not None else None
                 _save_png(img[0], path / f'{tag}_inp.png')
-                rec = self.renderer(meshes, R, T, viz_purpose=True)[:, :3]
+                rec = self.renderer(meshes, R, T, viz_purpose=True, K=K)[:, :3]
                 _save_png(rec[0], path / f'{tag}_rec.png')
-                _save_png(self.renderer.draw_edges(rec, syn_blocks, R, T, colors)[0], path / f'{tag}_rec_col.png')
-                _save_png(self.renderer.draw_edges(img, syn_blocks, R, T, colors)[0], path / f'{tag}_rec_col_inp.png')
-                syn = self.renderer_light(syn_blocks, R, T, viz_purpose=True)[:, :3]
+                _save_png(self.renderer.draw_edges(rec, syn_blocks, R, T, colors, K=K)[0], path / f'{tag}_rec_col.png')
+                _save_png(self.renderer.draw_edges(img, syn_blocks, R, T, colors, K=K)[0], path / f'{tag}_rec_col_inp.png')
+                syn = self.renderer_light(syn_blocks, R, T, viz_purpose=True, K=K)[:, :3]
                 _save_png(syn[0], path / f'{tag}_rec_syn_nobkg.png')
-                _save_png(self.renderer_light.draw_edges(syn, syn_blocks, R, T, linewidth=0.7, colors=(0.3, 0.3, 0.3))[0],
+                _save_png(self.renderer_light.draw_edges(syn, syn_blocks, R, T, linewidth=0.7, colors=(0.3, 0.3, 0.3), K=K)[0],
                           path / f'{tag}_rec_syn_nobkg_edged.png')
                 count += 1
         return count

@@ -20,7 +20,7 @@ import torch
 
 from . import _lib
 from ._lib import DbwLossEpilogue
-from .renderer import _c, _stream, scene_settings
+from .renderer import _c, _stream, scene_settings, project_verts, view_intrinsics, cameras_need_grad
 
 N_PARTIALS = 1024
 GRAD_VERTS, GRAD_MAPS, GRAD_ALPHA = 1, 2, 4          # grad_mask bits of dbw_render_forward_loss_grad (DBW_GRAD_*)
@@ -43,11 +43,15 @@ class ScenePass:
         self.map_table_host, self.r = map_table_host, renderer
         self.alpha_group, self.n_static_faces = alpha_group, n_static_faces
 
-    def settings(self, verts, maps, B, faces_alpha, view_rows=None):
+    def settings(self, verts, maps, B, faces_alpha, view_rows=None, ndc=False, static_faces=True):
+        """ndc: `verts` are per-view projected (B,V,3) NDC vertices (per-view intrinsics); static_faces=False: differentiate the
+        static faces too (a render whose cameras take a gradient)"""
         r = self.r
-        return scene_settings(verts, self.faces, maps, self.map_table_host, B, r.cameras.intrinsics(), r.img_size, r.sigma,
+        intr = (1., 1., 0., 0.) if ndc else r.cameras.intrinsics()
+        return scene_settings(verts, self.faces, maps, self.map_table_host, B, intr, r.img_size, r.sigma,
                               r.faces_per_pixel, r.z_clip, r.detach_bary, r.clip_inside, r.background_color, faces_alpha,
-                              r.perspective_correct, False, r.blur_radius, True, self.alpha_group, self.n_static_faces, view_rows)
+                              r.perspective_correct, ndc, r.blur_radius, True, self.alpha_group,
+                              self.n_static_faces if static_faces else 0, view_rows)
 
 
 def _workspace(cfg, dev):
@@ -63,7 +67,7 @@ class _SceneMSEFn(torch.autograd.Function):
         L = _lib.lib()
         dev = blk_verts.device
         B, _, H, W = imgs.shape
-        f32 = lambda t: t.detach().contiguous().float()
+        f32 = lambda t: t.detach().contiguous().float() if t is not None else None      # R, T: None when verts are NDC
         env_verts, env_maps, blk_verts, blk_maps = f32(env_verts), f32(env_maps), f32(blk_verts), f32(blk_maps)
         R, T, imgs = f32(R), f32(T), f32(imgs)
         fa = f32(blk_alpha) if blk_alpha is not None else None
@@ -176,12 +180,22 @@ class _SceneMSEFn(torch.autograd.Function):
 
 
 def scene_mse(env_verts, env_atlas, blk_verts, blk_atlas, blk_alpha, R, T, imgs, env_pass, blk_pass, blk_face_map,
-              n_total_views=None, return_rec=False, view_rows=None):
+              n_total_views=None, return_rec=False, view_rows=None, K=None):
     """MSE between `imgs` (B,3,H,W) and the blocks composited over the environment, both rendered from raw scene tensors
     (float4 texel atlases from scene_ops.scene_atlases).  `n_total_views`: size of the GLOBAL batch the mean runs over
-    (view-sharded data parallelism); `view_rows` (B,2) int32: the [row_begin, row_end) of each view this rank owns.  Returns the loss, or (loss, rec) with a non-differentiable `rec`."""
+    (view-sharded data parallelism); `view_rows` (B,2) int32: the [row_begin, row_end) of each view this rank owns.
+    K (B,4,4): per-view intrinsics -- both passes' vertices are projected per view (renderer.project_verts) and rendered as NDC
+    input, and R, T and K receive gradients through the projection.  Returns the loss, or (loss, rec) with a non-differentiable `rec`."""
     B, _, H, W = imgs.shape
     inv = 1.0 / (float(n_total_views or B) * 3 * H * W)
+    if K is not None:
+        static = not cameras_need_grad(R, T, K)
+        intr = view_intrinsics(K, B)                          # read out of K once for both passes
+        env_verts, blk_verts = project_verts(env_verts, R, T, intr=intr), project_verts(blk_verts, R, T, intr=intr)
+        cfgs = (env_pass.settings(env_verts, env_atlas, B, None, view_rows, ndc=True, static_faces=static),
+                blk_pass.settings(blk_verts, blk_atlas, B, blk_alpha, view_rows, ndc=True, static_faces=static))
+        return _SceneMSEFn.apply(env_verts, env_atlas, blk_verts, blk_atlas, blk_alpha, None, None, imgs, env_pass, blk_pass,
+                                 blk_face_map, cfgs, inv, bool(return_rec))
     # settings are made out here: inside Function.forward grad mode is off and the passes would not save fragment state
     cfgs = (env_pass.settings(env_verts, env_atlas, B, None, view_rows), blk_pass.settings(blk_verts, blk_atlas, B, blk_alpha, view_rows))
     return _SceneMSEFn.apply(env_verts, env_atlas, blk_verts, blk_atlas, blk_alpha, R, T, imgs, env_pass, blk_pass,

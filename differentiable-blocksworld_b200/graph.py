@@ -13,11 +13,17 @@ gradient into the caller's graph behind run()'s inp['R'] / inp['T'] -- a small e
 The parameter update (GraphedStep(optimizer=BucketAdam)): the optimiser's one launch (optim.py) is captured after the point
 where the gradients are final -- the captured all-reduce, or the backward when the sum happens inside it or there is one rank
 -- so one replay is one training iteration.  Every rank applies the same elementwise update to the same summed gradients.  The
-learning rates are read on the device: a scheduler changes them between replays without a new capture."""
+learning rates are read on the device: a scheduler changes them between replays without a new capture.
+
+Per-view intrinsics (model.set_per_view_intrinsics(True)): inp['K'] is one of the static inputs, copied in before each replay, so
+a batch with other intrinsics is rendered with them without a new capture.  Intrinsics gradients (a ViewParallel built with
+intrinsics=True, and a K that requires grad in example_inp): (fx, fy, px, py) of the full batch become one more static leaf
+beside the poses, and its summed gradient is back-propagated into the caller's K after the replay."""
 import torch
 
 from .optim import BucketAdam
-from .parallel import pose_backward, refuse_camera_gradients, wants_pose_gradients
+from .parallel import (camera_leaves, pose_backward, refuse_camera_gradients, wants_intrinsics_gradients, wants_pose_gradients)
+from .renderer import intrinsics_of
 
 
 class GraphedStep:
@@ -32,7 +38,7 @@ class GraphedStep:
             if n_total_views != len(example_inp['imgs']):
                 raise ValueError('GraphedStep: with camera-pose gradients example_inp is the full batch of n_total_views views')
             self.pose = view_parallel.pose_leaves(example_inp)
-            example_inp = {k: v for k, v in view_parallel.shard(example_inp)[0].items() if k not in ('R', 'T')}
+            example_inp = {k: v for k, v in view_parallel.shard(example_inp)[0].items() if k not in self._leaf_keys}
         # The gradient all-reduce is captured INTO the graph when it is the peer-memory kernel (a plain launch).  An
         # ncclAllReduce is issued right after the replay instead: captured, it hung on 2 GPUs with this image's NCCL (round 1).
         if capture_all_reduce is None:
@@ -64,7 +70,8 @@ class GraphedStep:
         """what the captured control flow depends on: the training-schedule switches of dbw.py:210-212,276,331-334"""
         m = self.model
         frozen = self.optimizer.captured_constants() if self.optimizer is not None else ()      # a capture holds them by value
-        return (m.training, m.is_live('coarse_learning'), m.is_live('decimate_txt'), m.is_live('kill_blocks'), *frozen)
+        return (m.training, m.is_live('coarse_learning'), m.is_live('decimate_txt'), m.is_live('kill_blocks'), m.per_view_intrinsics,
+                *frozen)
 
     def _bind_buffers(self):
         self.model.opacity_noise_buffer, self.model.overlap_samples_buffer = self.noise_buf, self.overlap_buf
@@ -103,7 +110,7 @@ class GraphedStep:
         losses, reduced = self.vp.local_step(self.static_inp, None, self.n_total, collective=self.capture_all_reduce, poses=self.pose)
         self.inside = self.vp.reduces_inside_backward(self.static_inp)      # the collective sits INSIDE the backward (parallel.GradSumPoint)
         if self.capture_all_reduce and not reduced:
-            self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views)
+            self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views, intrinsics=self._intrinsics_leaf)
         if self.optimizer is not None and torch.cuda.is_current_stream_capturing():      # the warm-up runs must not train
             self.optimizer.launch(self.segment_table)
         return losses
@@ -112,31 +119,47 @@ class GraphedStep:
     def _pose_views(self):
         return self.n_total if self.pose is not None else 0
 
+    @property
+    def _intrinsics_leaf(self):
+        return self.pose is not None and self.pose[3] is not None
+
+    @property
+    def _leaf_keys(self):
+        """the inputs held as static leaves rather than copied into static inputs"""
+        return ('R', 'T', 'K') if self._intrinsics_leaf else ('R', 'T')
+
     def check_poses(self, inp):
-        """poses in `inp` must require grad exactly when this step was captured with pose gradients"""
-        if inp is None or not any(k in inp for k in ('R', 'T')):
+        """poses (and K) in `inp` must require grad exactly when this step was captured with their gradients"""
+        if inp is None or not any(k in inp for k in ('R', 'T', 'K')):
             return
         if self.pose is None and wants_pose_gradients(inp):
             if self.vp.max_pose_views == 0:
                 refuse_camera_gradients(inp, 'GraphedStep')
-            raise RuntimeError('GraphedStep: these poses require grad, but the step was captured with poses that do not; '
-                               'build the step from an example whose poses require grad')
+            raise RuntimeError('GraphedStep: these cameras require grad, but the step was captured with cameras that do not; '
+                               'build the step from an example whose cameras require grad')
+        if 'K' in inp and wants_intrinsics_gradients(inp) != self._intrinsics_leaf:
+            if not self.vp.intrinsics:
+                refuse_camera_gradients(inp, 'GraphedStep', intrinsics_only=True)
+            raise RuntimeError(f"GraphedStep: inp['K'].requires_grad is {wants_intrinsics_gradients(inp)}, but the step was captured "
+                               f"with {self._intrinsics_leaf}; build the step from an example whose K matches")
         if self.pose is not None and not wants_pose_gradients(inp):
-            raise RuntimeError('GraphedStep: the step was captured with poses that require grad, but these do not')
+            raise RuntimeError('GraphedStep: the step was captured with cameras that require grad, but these do not')
 
     def staged(self, inp):
         """[(static buffer, value)] for the tensors of `inp` that a run copies into the static inputs: with pose gradients,
         this rank's slice of the full-batch per-view tensors; the poses themselves are not among them (load_poses)"""
         if self.pose is not None:
-            inp = self.vp.take({k: v for k, v in inp.items() if k not in ('R', 'T')}, self.pose[2], self.n_total)
+            inp = self.vp.take({k: v for k, v in inp.items() if k not in self._leaf_keys}, self.pose[2], self.n_total)
         return [(self.static_inp[k], v) for k, v in inp.items() if k in self.static_inp]
 
     def load_poses(self, inp, non_blocking=True):
-        """copy inp's full-batch poses into the static pose leaves (on the current stream)"""
+        """copy inp's full-batch poses (and intrinsics) into the static camera leaves (on the current stream)"""
         with torch.no_grad():
             for k, leaf in zip(('R', 'T'), self.pose[:2]):
                 if k in inp:
                     leaf.copy_(inp[k].detach(), non_blocking=non_blocking)
+            if self._intrinsics_leaf and 'K' in inp:
+                self.pose[3].copy_(intrinsics_of(inp['K'].detach()), non_blocking=non_blocking)
 
     def run(self, inp=None, non_blocking=True, all_reduce=True):
         """inp: optional dict of (host or device) tensors for this step, copied into the static buffers.
@@ -164,13 +187,13 @@ class GraphedStep:
         for p, g in zip(self.vp.bucket.params, self.grads):
             p.grad = g
         if self.pose is not None:
-            for q, g in zip(self.pose, self.pose_grads):
+            for q, g in zip(camera_leaves(self.pose), self.pose_grads):
                 q.grad = g
         if not self.capture_all_reduce and all_reduce and self.vp.world_size > 1:
             if self.inside:
                 raise RuntimeError('this step sums its gradients inside the backward (parallel.GradSumPoint) but was captured '
                                    'with capture_all_reduce=False: its gradients are local and cannot be reduced afterwards')
-            self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views)
+            self.vp.bucket.all_reduce(self.vp.group, pose_views=self._pose_views, intrinsics=self._intrinsics_leaf)
         if self.pose is not None and inp is not None:
             pose_backward(inp, self.pose_grads)
         return self.losses
@@ -223,7 +246,7 @@ class PipelinedGraphedStep:
         cur.wait_event(self.ready[b])
         poses = None
         if self.steps[b].pose is not None:          # the poses as they are now, not as they were at the prefetch
-            poses = {k: host_inp[k] for k in ('R', 'T') if k in host_inp}
+            poses = {k: host_inp[k] for k in self.steps[b]._leaf_keys if k in host_inp}
         losses = self.steps[b].run(poses, all_reduce=all_reduce)
         self.free[b].record(cur)
         self.i += 1

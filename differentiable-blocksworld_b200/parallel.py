@@ -16,7 +16,8 @@ Correctness conditions handled here:
 Camera poses that require grad (ViewParallel(max_pose_views=N)): the step renders its shard from slices of full-batch pose
 leaves, so each rank's pose gradient is a (B, 12) block with zeros on the views it did not render; that block rides in the same
 one collective as the scene's gradients (the tail of the leaf bucket, or through the GradSumPoint), and the sum is handed on
-to the caller's R / T with one small eager backward."""
+to the caller's R / T with one small eager backward.  Intrinsics that require grad (ViewParallel(max_pose_views=N,
+intrinsics=True)) ride the same way: a (B, 4) leaf of (fx, fy, px, py) per view after the poses, handed on to the caller's K."""
 import ctypes
 
 import torch
@@ -32,26 +33,47 @@ def shard_views(n_views, world_size, rank):
     return slice(start, start + base + (1 if rank < extra else 0))
 
 
-def refuse_camera_gradients(inp, who):
-    """Camera poses that require grad are refused rather than silently left without a gradient: under view or row-band
-    sharding a rank holds only partial per-view sums of them, and a captured graph's static input buffers do not carry a
-    gradient back to the caller's tensors."""
-    for k in ('R', 'T'):
+def refuse_camera_gradients(inp, who, intrinsics_only=False):
+    """Camera poses or intrinsics that require grad are refused rather than silently left without a gradient: under view or
+    row-band sharding a rank holds only partial per-view sums of them, and a captured graph's static input buffers do not carry
+    a gradient back to the caller's tensors.  intrinsics_only: the step carries pose gradients, but not intrinsics gradients."""
+    for k in (('K',) if intrinsics_only else ('R', 'T', 'K')):
         v = inp.get(k) if inp is not None else None
         if torch.is_tensor(v) and v.requires_grad:
-            raise RuntimeError(f"{who}: inp['{k}'] requires grad, but this step was not built for camera-pose gradients: "
-                               f"construct its ViewParallel with max_pose_views >= the views of a step, detach the poses, or "
-                               f"call the model directly")
+            how = ('construct its ViewParallel with max_pose_views >= the views of a step and intrinsics=True' if k == 'K' else
+                   'construct its ViewParallel with max_pose_views >= the views of a step')
+            raise RuntimeError(f"{who}: inp['{k}'] requires grad, but this step was not built for its gradient: {how}, detach "
+                               f"it, or call the model directly")
 
 
 def wants_pose_gradients(inp):
-    """inp's camera poses require grad"""
-    return inp is not None and any(torch.is_tensor(inp.get(k)) and inp[k].requires_grad for k in ('R', 'T'))
+    """inp's camera poses or intrinsics require grad"""
+    return inp is not None and any(torch.is_tensor(inp.get(k)) and inp[k].requires_grad for k in ('R', 'T', 'K'))
+
+
+def wants_intrinsics_gradients(inp):
+    return inp is not None and torch.is_tensor(inp.get('K')) and inp['K'].requires_grad
+
+
+def camera_leaves(poses):
+    """the leaves of pose_leaves()'s (R, T, views, intrinsics or None) that take a gradient, in bucket order"""
+    return [q for q in (poses[0], poses[1], poses[3]) if q is not None]
+
+
+def intrinsics_matrix(intr):
+    """(B,4) (fx, fy, px, py) -> a (B,4,4) K holding them where renderer.intrinsics_of reads them (other entries 0: unread)"""
+    fx, fy, px, py = intr.unbind(1)
+    z = torch.zeros_like(fx)              # built on the device: no host copy inside a captured step
+    return torch.stack([fx, z, px, z, z, fy, py, z, z, z, z, z, z, z, z, z], -1).view(-1, 4, 4)
 
 
 def pose_backward(inp, grads):
-    """continue the step's summed pose gradients (g_R (B,3,3), g_T (B,3)) into the caller's graph behind inp['R'] / inp['T']"""
+    """continue the step's summed camera gradients (g_R (B,3,3), g_T (B,3)[, g_intrinsics (B,4)]) into the caller's graph behind
+    inp['R'] / inp['T'] (/ inp['K'], through its fx, fy, px, py entries)"""
+    from .renderer import intrinsics_of
     pairs = [(inp[k], g) for k, g in zip(('R', 'T'), grads) if torch.is_tensor(inp.get(k)) and inp[k].requires_grad]
+    if len(grads) > 2 and wants_intrinsics_gradients(inp):
+        pairs.append((intrinsics_of(inp['K']), grads[2]))
     if pairs:
         torch.autograd.backward([t for t, _ in pairs], [g.to(t.dtype) for t, g in pairs])
 
@@ -142,21 +164,33 @@ class GradSumPoint:
 
     def __init__(self, peer):
         self.peer = peer
-        self.pose_leaves = None          # (R (B,3,3), T (B,3), views): full-batch pose leaves that ride through the point
-        self._cameras = None
+        self.pose_leaves = None          # (R (B,3,3), T (B,3), views, intrinsics (B,4) or None): full-batch camera leaves that ride through the point
+        self._cameras = self._K = None
 
     def __call__(self, *tensors):
         if self.pose_leaves is None:
             return _GradSumFn.apply(self, *tensors)
-        R, T, views = self.pose_leaves
-        *out, R, T = _GradSumFn.apply(self, *tensors, R, T)
-        self._cameras = (R[views], T[views])
+        views = self.pose_leaves[2]
+        leaves = camera_leaves(self.pose_leaves)
+        out = _GradSumFn.apply(self, *tensors, *leaves)
+        out, cams = out[:len(tensors)], out[len(tensors):]
+        self._cameras = (cams[0][views], cams[1][views])
+        self._K = intrinsics_matrix(cams[2][views]) if len(cams) > 2 else None
         return tuple(out)
 
     def ride(self, poses):
-        """poses = (R, T, views) or None: from the next call on, the pose leaves pass through the point with the scene tensors,
-        so their gradients join the same one exchange; the model then renders from cameras()"""
-        self.pose_leaves, self._cameras = poses, None
+        """poses = (R, T, views, intrinsics or None) or None: from the next call on, the camera leaves pass through the point with
+        the scene tensors, so their gradients join the same one exchange; the model then renders from cameras() / intrinsics()"""
+        self.pose_leaves, self._cameras, self._K = poses, None, None
+
+    def intrinsics(self, K):
+        """the per-view K a model renders its shard from: this rank's slice of the point's intrinsics output when intrinsics
+        leaves ride along, `K` (the model's own choice) otherwise"""
+        if self.pose_leaves is None or self.pose_leaves[3] is None:
+            return K
+        if self._K is None:
+            raise RuntimeError('GradSumPoint.intrinsics() before the point was called on the scene tensors')
+        return self._K
 
     def cameras(self, inp):
         """the (R, T) a model renders its shard from, read after it has called the point: this rank's slices of the point's pose
@@ -186,18 +220,19 @@ class GradSumPoint:
 class GradBucket:
     """All parameter gradients as views into one flat buffer -> a single all-reduce per step."""
 
-    def __init__(self, params, peer_factory=None, min_floats=0, max_pose_views=0):
+    def __init__(self, params, peer_factory=None, min_floats=0, max_pose_views=0, intrinsics=False):
         """peer_factory(n_floats, device) -> PeerAllReduce or None: when given and successful, the flat buffer IS the peer-memory
         arena's bucket (csrc/dbw_comm.cu) and all_reduce() is its kernel; else a plain tensor and torch.distributed.
         min_floats: capacity the arena needs for its other user (GradSumPoint).
         max_pose_views: room for the pose gradients of that many views (12 floats each: the B x 9 entries of g_R, then the
-        B x 3 of g_T) after the parameter gradients, gathered and all-reduced with them"""
+        B x 3 of g_T) after the parameter gradients, gathered and all-reduced with them.
+        intrinsics: 4 more floats per pose view, for the B x 4 intrinsics gradients after g_T"""
         self.params = [p for p in params if p.requires_grad]
         n = sum(p.numel() for p in self.params)
         ref = self.params[0]
         self.n = n
         n_pad = (n + 3) // 4 * 4                     # padded: 128-bit all-reduce lanes
-        n_all = n_pad + 12 * int(max_pose_views)
+        n_all = n_pad + (16 if intrinsics else 12) * int(max_pose_views)
         self.peer = peer_factory(max(n_all, (int(min_floats) + 3) // 4 * 4), ref.device) if peer_factory is not None else None
         if self.peer is not None:
             self.peer.flat.zero_()
@@ -226,7 +261,8 @@ class GradBucket:
         of the bucket, no accumulate-add per parameter); a single cat then writes them into the flat buffer and the
         .grad attributes become the bucket views again.  CUDA-graph capturable.  gather=False stops after the backward:
         the .grad attributes are autograd's own tensors and the flat buffer is not written (no collective reads it).
-        poses: the step's pose leaves (R (B,3,3), T (B,3)); the same cat writes their gradients into the pose region"""
+        poses: the step's camera leaves (R (B,3,3), T (B,3)[, intrinsics (B,4)]); the same cat writes their gradients into the
+        pose region"""
         for p in (*self.params, *poses):
             p.grad = None
         total.backward()
@@ -258,10 +294,11 @@ class GradBucket:
         """the gradients as one flat vector in bucket order, whichever way the last backward left them"""
         return torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).reshape(-1) for p in self.params])
 
-    def all_reduce(self, group=None, pose_views=0):
-        """sum the bucket over the ranks; pose_views: the pose gradients of that many views ride in the same collective"""
+    def all_reduce(self, group=None, pose_views=0, intrinsics=False):
+        """sum the bucket over the ranks; pose_views: the pose gradients of that many views ride in the same collective
+        (intrinsics: and their intrinsics gradients)"""
         if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
-            buf = self._all[:self.flat.numel() + 12 * pose_views]
+            buf = self._all[:self.flat.numel() + (16 if intrinsics else 12) * pose_views]
             if self.peer is not None:
                 self.peer.all_reduce(buf)
             else:
@@ -279,7 +316,7 @@ class ViewParallel:
     VIEW_KEYS = ('imgs', 'R', 'T', 'K')
 
     def __init__(self, model, group=None, seed=227391, row_bands=False, collective='nccl', reduce_at='auto', gather_grads=None,
-                 peer_factory=None, max_pose_views=0):
+                 peer_factory=None, max_pose_views=0, intrinsics=False):
         """collective: 'nccl' (torch.distributed all_reduce; also what gloo groups use), 'p2p' (the NVLink peer-memory kernel
         of csrc/dbw_comm.cu, CUDA-graph capturable) or 'auto' (p2p if it initialises on this node, else nccl).
         reduce_at: 'leaf' (all-reduce the parameter gradients after the backward), 'scene' (sum the gradients of the scene
@@ -294,9 +331,15 @@ class ViewParallel:
         max_pose_views: 0 refuses camera poses that require grad; N > 0 reserves 12 N floats of the bucket / arena and accepts
         them on steps of at most N views.  Such a step takes FULL-BATCH inputs (all views' imgs, K, R, T, identical on every
         rank) and leaves the gradient of the global loss with respect to all B views' poses in the caller's graph, the same
-        on every rank (pose_step)"""
+        on every rank (pose_step).
+        intrinsics: with max_pose_views = N > 0, reserve 4 N more floats and accept a K (B,4,4) that requires grad likewise: its
+        (fx, fy, px, py) entries receive the gradient of the global loss (the model renders such a step per view)"""
         self.model, self.group, self.seed = model, group, seed
         self.max_pose_views = int(max_pose_views)
+        self.intrinsics = bool(intrinsics) and self.max_pose_views > 0
+        if intrinsics and not self.intrinsics:
+            raise ValueError('ViewParallel: intrinsics=True needs max_pose_views > 0 (the views whose gradients it reserves room for)')
+        cam_floats = (16 if self.intrinsics else 12) * self.max_pose_views
         self.reduce_at, self.gather_grads = reduce_at, gather_grads
         self.row_bands = row_bands          # shard at (view, row band) granularity (needs the model's fused-loss path)
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -314,7 +357,7 @@ class ViewParallel:
 
         want_point = reduce_at in ('scene', 'auto') and hasattr(model, 'grad_sum_floats')
         self.bucket = GradBucket(model.parameters(), peer_factory or arena_factory,
-                                 model.grad_sum_floats() + 12 * self.max_pose_views if want_point else 0, self.max_pose_views)
+                                 model.grad_sum_floats() + cam_floats if want_point else 0, self.max_pose_views, self.intrinsics)
         self.sum_point = GradSumPoint(self.bucket.peer) if (want_point and self.bucket.peer is not None) else None
         if reduce_at == 'scene' and self.sum_point is None and self.world_size > 1:
             raise RuntimeError("reduce_at='scene' needs the peer-memory collective (collective='p2p' or 'auto') and a model with grad_sum_floats()")
@@ -334,7 +377,7 @@ class ViewParallel:
         sl, rows = self.views(B, inp['imgs'].shape[-2])
         out = self.take(inp, sl, B)
         if rows is not None:
-            out['rows'] = rows
+            out['rows'] = rows.to(inp['imgs'].device)          # where the kernels read them: beside the images
         return out, B
 
     def views(self, n_views, height):
@@ -358,23 +401,30 @@ class ViewParallel:
         """a step whose poses require grad: refused unless this wrapper reserved room for at least its B views"""
         if self.max_pose_views == 0:
             refuse_camera_gradients(inp, who)
+        if not self.intrinsics:
+            refuse_camera_gradients(inp, who, intrinsics_only=True)
         B = len(inp['imgs'])
         if B > self.max_pose_views:
             raise ValueError(f'{who}: a step of {B} views with camera-pose gradients, but the ViewParallel reserved room for '
                              f'max_pose_views={self.max_pose_views}')
-        for k, shape in (('R', (B, 3, 3)), ('T', (B, 3))):
+        for k, shape in (('R', (B, 3, 3)), ('T', (B, 3)), ('K', (B, 4, 4))):
+            if k == 'K' and not wants_intrinsics_gradients(inp):
+                continue
             if tuple(inp[k].shape) != shape:
                 raise ValueError(f"{who}: with camera-pose gradients inp['{k}'] is the full batch {shape}, got {tuple(inp[k].shape)}")
 
     def pose_leaves(self, inp):
-        """(R, T, views): leaves holding the values of inp's full-batch poses, which the step renders its shard from"""
+        """(R, T, views, intrinsics): leaves holding the values of inp's full-batch poses -- and, when inp['K'] requires grad, of
+        its (B,4) (fx, fy, px, py), else None -- which the step renders its shard from"""
+        from .renderer import intrinsics_of
         B = len(inp['imgs'])
-        return (inp['R'].detach().to(torch.float32, copy=True).requires_grad_(True),
-                inp['T'].detach().to(torch.float32, copy=True).requires_grad_(True), self.views(B, inp['imgs'].shape[-2])[0])
+        leaf = lambda t: t.detach().to(torch.float32, copy=True).requires_grad_(True)
+        intr = leaf(intrinsics_of(inp['K'])) if wants_intrinsics_gradients(inp) else None
+        return leaf(inp['R']), leaf(inp['T']), self.views(B, inp['imgs'].shape[-2])[0], intr
 
     @staticmethod
     def pose_grads(poses):
-        return [q.grad if q.grad is not None else torch.zeros_like(q) for q in poses[:2]]
+        return [q.grad if q.grad is not None else torch.zeros_like(q) for q in camera_leaves(poses)]
 
     def _sync_rng(self, device):
         g = getattr(self.model, 'noise_generator', None)
@@ -399,17 +449,21 @@ class ViewParallel:
         self.model.n_total_views = n_total_views
         self.model.grad_sum_point = self.sum_point if (inside and collective) else None
         if poses is not None:
-            R, T, views = poses
-            if self.model.grad_sum_point is not None:          # the model renders from sum_point.cameras()
+            R, T, views, intr = poses
+            if self.model.grad_sum_point is not None:          # the model renders from sum_point.cameras() / intrinsics()
                 self.sum_point.ride(poses)
                 inp = dict(inp, R=R.detach()[views], T=T.detach()[views])
+                if intr is not None and 'K' in inp:
+                    inp['K'] = inp['K'].detach()
             else:
                 inp = dict(inp, R=R[views], T=T[views])
+                if intr is not None:                             # a K that requires grad: the model renders per view
+                    inp['K'] = intrinsics_matrix(intr[views])
         try:
             losses = self.model(inp, labels)
             gather = self.gather_grads if self.gather_grads is not None else (self.world_size > 1 and not inside)
             self.bucket.backward(self.weighted_total(losses, len(inp['imgs']), n_total_views, replicated_everywhere=inside),
-                                 gather=gather, poses=poses[:2] if poses is not None else ())
+                                 gather=gather, poses=camera_leaves(poses) if poses is not None else ())
         finally:
             self.model.grad_sum_point = None
             if self.sum_point is not None:
@@ -432,7 +486,8 @@ class ViewParallel:
         self._step += 1
         losses, reduced = self.local_step(inp, labels, n_total_views, collective=all_reduce, poses=poses)
         if all_reduce and not reduced:
-            self.bucket.all_reduce(self.group, pose_views=n_total_views if poses is not None else 0)
+            self.bucket.all_reduce(self.group, pose_views=n_total_views if poses is not None else 0,
+                                   intrinsics=poses is not None and poses[3] is not None)
         if poses is not None:
             pose_backward(full, self.pose_grads(poses))
         return losses

@@ -128,6 +128,72 @@ class _RenderFn(torch.autograd.Function):
         return g_verts, g_maps, g_fa, g_R, g_T, None, None, None, None, None, None, None, None
 
 
+class _ProjectFn(torch.autograd.Function):
+    """autograd seam over dbw_camera_project / dbw_camera_project_backward (include/dbw_render.h)."""
+
+    @staticmethod
+    def forward(ctx, verts, R, T, intr, eps):
+        if not verts.is_cuda:
+            raise DbwError('the CUDA renderer needs CUDA tensors (there is no CPU fallback)')
+        verts, R, T, intr = (t.detach().contiguous().float() for t in (verts, R, T, intr))
+        B, V = R.shape[0], verts.shape[0]
+        out = torch.empty(B, V, 3, dtype=torch.float32, device=verts.device)
+        _lib.check(_lib.lib().dbw_camera_project(B, V, _c(verts), _c(R), _c(T), _c(intr), ctypes.c_float(eps), _c(out), _stream()),
+                   'dbw_camera_project')
+        ctx.save_for_backward(verts, R, T, intr)
+        ctx.eps = eps
+        return out
+
+    @staticmethod
+    def backward(ctx, g_ndc):
+        verts, R, T, intr = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        B, V = R.shape[0], verts.shape[0]
+        # one zero-fill for every gradient wanted: vertices, then the 9 + 3 + 4 camera floats of each view
+        sizes = [verts.numel() if need[0] else 0, R.numel() if need[1] else 0, T.numel() if need[2] else 0, intr.numel() if need[3] else 0]
+        flat = torch.zeros(sum(sizes), dtype=torch.float32, device=verts.device)
+        grads, o = [], 0
+        for t, n in zip((verts, R, T, intr), sizes):
+            grads.append(flat[o:o + n].view_as(t) if n else None)
+            o += n
+        _lib.check(_lib.lib().dbw_camera_project_backward(B, V, _c(verts), _c(R), _c(T), _c(intr), ctypes.c_float(ctx.eps),
+                                                          _c(g_ndc.contiguous().float()), *[_c(g) for g in grads], _stream()),
+                   'dbw_camera_project_backward')
+        return (*grads, None)
+
+
+def intrinsics_of(K):
+    """(B,4) = (fx, fy, px, py) of per-view intrinsics K (B,4,4), read as K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2] by device
+    indexing (no host read; autograd scatters a gradient back into exactly those four entries).  The other entries of K --
+    skew among them -- are ignored, as by the single-camera path."""
+    K = K.reshape(-1, 4, 4)
+    return torch.stack([K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2]], dim=-1)
+
+
+def view_intrinsics(K, B):
+    """(B,4) (fx, fy, px, py) of B views from K (B,4,4), or from one (1,4,4) / (4,4) K shared by all of them"""
+    intr = intrinsics_of(K)
+    if intr.shape[0] != B:
+        if intr.shape[0] != 1:
+            raise DbwError(f'K must hold 1 or {B} cameras (one per view), got {intr.shape[0]}')
+        intr = intr.expand(B, -1)
+    return intr
+
+
+def project_verts(verts, R, T, K=None, eps=EPS, intr=None):
+    """world vertices (V,3) -> (B,V,3) = (x_ndc, y_ndc, z_view), each view b through its own R[b], T[b] and intrinsics K[b]
+    (B,4,4) (a single (1,4,4) / (4,4) K serves every view), or through intr (B,4) from view_intrinsics() when several passes
+    share the cameras.  Differentiable with respect to all inputs."""
+    if intr is None:
+        intr = view_intrinsics(K, R.shape[0])
+    return _ProjectFn.apply(verts, R, T, intr, float(eps))
+
+
+def cameras_need_grad(R, T, K):
+    """a render from these cameras differentiates them: its static faces then get gradients too (they move in the image)"""
+    return torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in (R, T, K))
+
+
 _TABLE_CACHE = {}
 
 
@@ -219,7 +285,15 @@ def render_scene(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, 
     """Functional form over raw tensors (used by Renderer.forward and by the parity tests).
     verts (V,3) [or (B,V,3) NDC], faces (F,3) int32, faces_uvs (F,3,2), face_map (F) int32, maps flat float buffer,
     map_table_host [(offset,H,W)], R (B,3,3), T (B,3), faces_alpha None | (F,) | (B*F,).
+    intr: (fx, fy, px, py) floats shared by every view, or a tensor K (B,4,4) of per-view intrinsics: the world vertices are
+    then projected per view on the device (project_verts) and rendered as NDC input; R, T and K receive gradients.
     maps_are_texels4: `maps` is a float4 (RGB+pad) texel atlas from scene_ops.scene_atlases (offsets stay 3*texel)."""
+    if torch.is_tensor(intr):
+        if verts_are_ndc or R is None:
+            raise DbwError('per-view intrinsics project world vertices: they need R and T, and verts_are_ndc=False')
+        if cameras_need_grad(R, T, intr):
+            n_static_faces = 0
+        verts, R, T, intr, verts_are_ndc = project_verts(verts, R, T, intr), None, None, (1., 1., 0., 0.), True
     dev = verts.device
     B = R.shape[0] if R is not None else verts.shape[0]
     cfg, map_table = scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigma, faces_per_pixel, z_clip,
@@ -304,10 +378,10 @@ class Renderer(nn.Module):
         if self.shading_type not in ('raw', 'flat') or (lit != (self.shading_type == 'flat')):
             raise NotImplementedError(f'shading_type={self.shading_type} with lights={self.light_kwargs.get("name", "ambient")}: '
                                       'only raw+ambient (training) and flat+directional (renderer_light) are implemented')
-        faces_alpha = kwargs.get('faces_alpha')
+        faces_alpha, K = kwargs.get('faces_alpha'), kwargs.get('K')
         verts, faces, fvu, fmap, maps, table = self._scene(meshes)
         H, W = self.img_size
-        intr = self.cameras.intrinsics()
+        intr = K if K is not None else self.cameras.intrinsics()      # K (B,4,4): each view with its own intrinsics
         shade = self._flat_shade(verts, faces, R) if lit else None
         if viz_purpose:
             # VizMeshRenderer (renderer.py:56-60,178-183): hard 4x supersampled render, box-filtered, no gradient
@@ -322,12 +396,13 @@ class Renderer(nn.Module):
 
     # ------------------------------------------------------------------ edge overlays (renderer.py:134-175)
     @torch.no_grad()
-    def render_edges(self, meshes, R, T, image_size=None, linewidth=1, return_pix2face=False, faces_per_pixel=1):
+    def render_edges(self, meshes, R, T, image_size=None, linewidth=1, return_pix2face=False, faces_per_pixel=1, K=None):
         """mask of the pixels closer than `linewidth` pixels to an edge of the face(s) they see: a hard rasterization whose
-        signed squared NDC distances are thresholded at (linewidth * 2 / min(image_size))^2."""
+        signed squared NDC distances are thresholded at (linewidth * 2 / min(image_size))^2.  K (B,4,4): per-view intrinsics."""
         image_size = tuple(image_size or self.img_size)
         verts, faces, fvu, fmap, maps, table = self._scene(meshes)
-        _, ids, dists = render_scene(verts, faces, fvu, fmap, maps, table, R, T, self.cameras.intrinsics(), image_size, 0.0,
+        intr = K if K is not None else self.cameras.intrinsics()
+        _, ids, dists = render_scene(verts, faces, fvu, fmap, maps, table, R, T, intr, image_size, 0.0,
                                      faces_per_pixel, self.z_clip, perspective_correct=self.perspective_correct,
                                      return_dists=True)
         mask = (-dists < (linewidth * 2 / min(image_size)) ** 2).float().max(1, keepdim=True)[0]       # (B,1,H,W)
@@ -339,7 +414,7 @@ class Renderer(nn.Module):
             return mask, pix2face                                           # batch-packed ids like fragments.pix_to_face
         return mask
 
-    def draw_edges(self, img, meshes, R=None, T=None, colors=None, linewidth=1, antialias=True):
+    def draw_edges(self, img, meshes, R=None, T=None, colors=None, linewidth=1, antialias=True, K=None):
         dev = meshes.device
         B = img.shape[0] if isinstance(img, torch.Tensor) and img.dim() == 4 else 1
         if R is None:
@@ -354,7 +429,7 @@ class Renderer(nn.Module):
             img_size, linewidth = (img_size[0] * 4, img_size[1] * 4), linewidth * 4
         if isinstance(colors, (list, tuple)):
             colors = torch.Tensor(colors)
-        mask, pix2face = self.render_edges(meshes, R, T, image_size=img_size, linewidth=linewidth, return_pix2face=True)
+        mask, pix2face = self.render_edges(meshes, R, T, image_size=img_size, linewidth=linewidth, return_pix2face=True, K=K)
         if colors.dim() == 2:
             face_img = colors.to(mask.device)[pix2face].permute(0, 3, 1, 2)               # one colour per (packed) face
         else:

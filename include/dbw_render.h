@@ -239,6 +239,31 @@ int dbw_render_backward_deferred(const DbwRenderSettings* settings, const float*
                                  void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
 
 /*
+ * The camera projection on its own, with each view's own intrinsics (the datasets give every view its own K, src/dataset/dtu.py
+ * and bmvs.py decompose one projection matrix per view): world -> NDC for B views,
+ *   X_view = X_world @ R[b] + T[b];  x_ndc = (fx[b] x + px[b] z) / d,  y_ndc = (fy[b] y + py[b] z) / d,  z_ndc = z,
+ *   d = sign(z) max(|z|, eps)  (sign(0) = +1) -- the arithmetic of the forward's own projection with one (fx, fy, px, py),
+ * bit for bit when every view has the same intrinsics.  Its output is the `verts` of a verts_are_ndc = 1 render, so every
+ * render entry point above draws each view with its own camera; that render's g_verts (B,V,3) is this backward's g_ndc.
+ *   verts (V,3), R (B,3,3), T (B,3), intrinsics (B,4) = (fx, fy, px, py) per view, eps > 0 (proj_eps);  verts_ndc (B,V,3).
+ * One launch.
+ */
+int dbw_camera_project(int32_t n_views, int32_t n_verts, const float* verts, const float* R, const float* T,
+                       const float* intrinsics, float eps, float* verts_ndc, void* stream);
+/*
+ * Backward of dbw_camera_project: from g_ndc (B,V,3), ACCUMULATE g_verts (V,3), g_R (B,3,3), g_T (B,3) and
+ * g_intrinsics (B,4): g_fx = sum_v gx x_view / d, g_fy = sum_v gy y_view / d, g_px = sum_v gx z_view / d,
+ * g_py = sum_v gy z_view / d (|z| < eps: d is the constant +-eps, no z term, as in dbw_render_backward).  Any output may be
+ * NULL.  g_verts: one warp per vertex sums the views, no atomics.  g_R / g_T / g_intrinsics: per-view sums in a fixed order (one
+ * CTA per view, as dbw_render_backward's camera gradient), one atomic add per element per call.  At most two launches.
+ * A render whose camera or intrinsics gradient is wanted runs with n_static_faces = 0: the static faces move in the image when
+ * the camera does.
+ */
+int dbw_camera_project_backward(int32_t n_views, int32_t n_verts, const float* verts, const float* R, const float* T,
+                                const float* intrinsics, float eps, const float* g_ndc, float* g_verts, float* g_R,
+                                float* g_T, float* g_intrinsics, void* stream);
+
+/*
  * Fused scene construction (src/model/dbw.py:267-352), so that a training step needs no eager tensor ops between the
  * leaf parameters and the rasterizer.  All pointers are device pointers.
  */
