@@ -97,7 +97,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_u
            'dbw_lpips_conv3x3', 'dbw_lpips_conv_first', 'dbw_lpips_dgrad_last', 'dbw_lpips_maxpool', 'dbw_lpips_maxpool_backward',
            'dbw_lpips_head_forward', 'dbw_lpips_head_backward',
            'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached',
-           'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward',
+           'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward', 'dbw_vgg_head_forward',
+           'dbw_vgg_head_backward',
            'dbw_adam_step']
 
 _lib = None
@@ -185,6 +186,8 @@ def lib():
         L.dbw_vgg_loss_workspace_bytes.argtypes = [i64, i32, i32, op, i32, ctypes.POINTER(sz)]
         L.dbw_vgg_loss_forward.argtypes = [np_, op, vp, vp, i64, i32, i32, i32, vp, vp, sz, vp]
         L.dbw_vgg_loss_backward.argtypes = [np_, op, vp, i64, i32, i32, vp, vp, sz, vp]
+        L.dbw_vgg_head_forward.argtypes = [vp, vp, ctypes.c_float, i64, i32, i32, i32, vp, vp]
+        L.dbw_vgg_head_backward.argtypes = [vp, vp, ctypes.c_float, i64, i32, i32, i32, vp, i32, vp, vp]
         L.dbw_adam_step.argtypes = [vp, i32, i64, ctypes.POINTER(DbwAdamGroup), i32, vp, vp, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')

@@ -1051,12 +1051,11 @@ void vgg_chain_outputs(float* const* keep, int last, float* S0, float* S1, float
   }
 }
 
-int vgg_head_forward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
-                     float* part, cudaStream_t st) {
-  if (normalized) return head_forward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, part, st);
+// the plain head of C channels (64, 128, 256 or 512): partials (B, head_chunks(H, W)) as head_forward writes them
+int head_plain_forward(const float* f0, const float* f1, float w, int64_t B, int H, int W, int C, float* part, cudaStream_t st) {
   const int n = (int)head_chunks(H, W), HW = H * W;
   const dim3 grid((unsigned)n, (unsigned)B);
-  switch (LP_TAP_C[k]) {
+  switch (C) {
     case 64: vgg_head_plain_forward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
     case 128: vgg_head_plain_forward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
     case 256: vgg_head_plain_forward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, w, HW, part, n); break;
@@ -1066,12 +1065,11 @@ int vgg_head_forward(const float* f0, const float* f1, const float* lin, float w
   return 0;
 }
 
-int vgg_head_backward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
-                      const float* grad_value, int accumulate, float* g, cudaStream_t st) {
-  if (normalized) return head_backward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, grad_value, accumulate, g, st);
+int head_plain_backward(const float* f0, const float* f1, float w, int64_t B, int H, int W, int C, const float* grad_value,
+                        int accumulate, float* g, cudaStream_t st) {
   const dim3 grid((unsigned)head_chunks(H, W), (unsigned)B);
   const int HW = H * W;
-  switch (LP_TAP_C[k]) {
+  switch (C) {
     case 64: vgg_head_plain_backward_kernel<64><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
     case 128: vgg_head_plain_backward_kernel<128><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
     case 256: vgg_head_plain_backward_kernel<256><<<grid, 256, 0, st>>>(f0, f1, w, HW, grad_value, accumulate, g); break;
@@ -1079,6 +1077,18 @@ int vgg_head_backward(const float* f0, const float* f1, const float* lin, float 
   }
   LP_LAUNCH_CK("vgg_head_plain_backward_kernel");
   return 0;
+}
+
+int vgg_head_forward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
+                     float* part, cudaStream_t st) {
+  if (normalized) return head_forward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, part, st);
+  return head_plain_forward(f0, f1, w, B, H, W, LP_TAP_C[k], part, st);
+}
+
+int vgg_head_backward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
+                      const float* grad_value, int accumulate, float* g, cudaStream_t st) {
+  if (normalized) return head_backward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, grad_value, accumulate, g, st);
+  return head_plain_backward(f0, f1, w, B, H, W, LP_TAP_C[k], grad_value, accumulate, g, st);
 }
 
 float vgg_head_weight(const DbwVggLossOptions* opt, int k) { return opt->sum_channels ? 1.f : 1.f / (float)LP_TAP_C[k]; }
@@ -1372,4 +1382,23 @@ extern "C" int dbw_vgg_loss_backward(const DbwLpipsNet* net, const DbwVggLossOpt
   if (!vgg_net_ok(net, opt) || !grad_value || !grad_in1 || !workspace)
     return dbw_fail_("dbw_vgg_loss_backward: null pointer argument", cudaSuccess);
   return vgg_backward_impl(net, opt, grad_value, B, H, W, grad_in1, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// the plain head alone, for tests: the launchers of the whole term
+extern "C" int dbw_vgg_head_forward(const float* f0, const float* f1, float w, int64_t B, int32_t H, int32_t W, int32_t C,
+                                    float* partials, void* stream) {
+  if (const int rc = check_head_args("dbw_vgg_head_forward: bad sizes (1 <= B <= 65535, 1 <= H, W <= 32767, C = 64, 128, 256 or 512)",
+                                     B, H, W, C, 0))
+    return rc;
+  if (!f0 || !f1 || !partials) return dbw_fail_("dbw_vgg_head_forward: null pointer argument", cudaSuccess);
+  return head_plain_forward(f0, f1, w, B, H, W, C, partials, (cudaStream_t)stream);
+}
+
+extern "C" int dbw_vgg_head_backward(const float* f0, const float* f1, float w, int64_t B, int32_t H, int32_t W, int32_t C,
+                                     const float* grad_value, int32_t accumulate, float* g, void* stream) {
+  if (const int rc = check_head_args("dbw_vgg_head_backward: bad sizes (1 <= B <= 65535, 1 <= H, W <= 32767, C = 64, 128, 256 or 512)",
+                                     B, H, W, C, 0))
+    return rc;
+  if (!f0 || !f1 || !grad_value || !g) return dbw_fail_("dbw_vgg_head_backward: null pointer argument", cudaSuccess);
+  return head_plain_backward(f0, f1, w, B, H, W, C, grad_value, accumulate, g, (cudaStream_t)stream);
 }

@@ -605,6 +605,13 @@ int dbw_lpips_backward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache*
  *  - the head partials: per requested level in order (not padded between levels), B x ceil(H_k W_k / 64) floats;
  *  - 2568 constants the forward writes: per level k, 512 floats whose first C_k hold w; then shift 0 and scale 1 (4 floats
  *    each), the identity transform used without normalize_input.
+ *
+ * dbw_vgg_head_forward and dbw_vgg_head_backward run one head without normalize_features, as the whole term does, on NHWC
+ * features f0 (imgs) and f1 (rec) of shape (B, H, W, C), C = 64, 128, 256 or 512, with weight w.  The forward writes
+ * partials (B, ceil(H*W / 64)), partial[b][c] the sum of w * (f0 - f1)^2 over channels and pixels 64c .. 64c + 63.  The
+ * backward writes g (B, H, W, C) = (d sum_b grad_value[b] head_b / d f1 + (accumulate ? g : 0)) * [f1 > 0], head_b being the
+ * spatial mean of image b's head.  The head with normalize_features is dbw_lpips_head_forward / _backward with train = 0 and
+ * lin = the level's w in the constants above.
  */
 typedef struct DbwVggLossOptions {
   int32_t levels;
@@ -620,6 +627,10 @@ int dbw_vgg_loss_forward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, c
                          void* stream);
 int dbw_vgg_loss_backward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B, int32_t H,
                           int32_t W, float* grad_in1, void* workspace, size_t workspace_bytes, void* stream);
+int dbw_vgg_head_forward(const float* f0, const float* f1, float w, int64_t B, int32_t H, int32_t W, int32_t C, float* partials,
+                         void* stream);
+int dbw_vgg_head_backward(const float* f0, const float* f1, float w, int64_t B, int32_t H, int32_t W, int32_t C,
+                          const float* grad_value, int32_t accumulate, float* g, void* stream);
 
 /*
  * Optimiser: one Adam step over every parameter tensor of a model in ONE launch -- torch.optim.Adam's single-tensor path
