@@ -99,7 +99,7 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_u
            'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached',
            'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward', 'dbw_vgg_head_forward',
            'dbw_vgg_head_backward',
-           'dbw_adam_step']
+           'dbw_adam_step', 'dbw_viz_workspace_bytes', 'dbw_render_forward_viz']
 
 _lib = None
 
@@ -131,6 +131,8 @@ def lib():
         L.dbw_camera_project_backward.argtypes = [ctypes.c_int32, ctypes.c_int32] + [vp] * 4 + [ctypes.c_float] + [vp] * 6
         L.dbw_composite_mse.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
         L.dbw_composite_mse_backward.argtypes = [ctypes.c_int32] * 3 + [vp] * 3 + [ctypes.c_float] + [vp] * 5
+        L.dbw_viz_workspace_bytes.argtypes = [ctypes.POINTER(DbwRenderSettings), ctypes.c_int32, ctypes.POINTER(sz)]
+        L.dbw_render_forward_viz.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [ctypes.c_int32, vp, ctypes.c_int32, vp, vp, vp, sz, vp]
         L.dbw_render_forward_host.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 5 + [sz] + [vp] * 6
         L.dbw_host_arena_release.restype = None
         L.dbw_scene_geometry_forward.argtypes = [ctypes.POINTER(DbwSceneGeometry), vp, ctypes.c_int32, vp, vp]

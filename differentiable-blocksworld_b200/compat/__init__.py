@@ -11,8 +11,9 @@ iopath (SURVEY.md 8b "Caveat", 8f rank 3).
 What is real: `toolz`'s five dict helpers, the PyTorch3D containers / constructors the model surface hands to the trainer
 (`Meshes`, `TexturesUV`, `join_meshes_as_*`, `ico_sphere`, `SubdivideMeshes`, the 6D-rotation transforms -- all this repo's
 own implementations), the point-cloud ops of the reference's 3-D evaluation (`knn_points` / `knn_gather` on the sm_90a
-k-NN kernels, the chamfer helpers and `chamfer_distance`, `sample_points_from_meshes`: dbw_b200/pointcloud.py), the two
-`seaborn` / `matplotlib.colors` calls behind the block colour map (`utils/plot.py:77-87`).
+k-NN kernels, the chamfer helpers and `chamfer_distance`, `sample_points_from_meshes`: dbw_b200/pointcloud.py), the
+look-at cameras `look_at_view_transform` / `look_at_rotation` (dbw_b200/views.py), the two `seaborn` / `matplotlib.colors`
+calls behind the block colour map (`utils/plot.py:77-87`).
 Everything else the reference imports at module load but only calls on its export / evaluation paths (PLY / OBJ I/O, the
 SVD ICP, `Pointclouds`, Open3D, video writing, plotting, LPIPS weights) is a named placeholder that raises
 `NotImplementedError` when CALLED: the control plane stays out of scope (SURVEY 8), the import graph is satisfied."""
@@ -28,6 +29,7 @@ from torch import nn
 
 from .. import geometry as G
 from .. import pointcloud as PC
+from .. import views as V
 from ..structures import Meshes, TexturesUV, join_meshes_as_batch, join_meshes_as_scene
 
 
@@ -119,9 +121,10 @@ def _pytorch3d():
             _validate_chamfer_reduction_inputs=PC._validate_chamfer_reduction_inputs,
             _handle_pointcloud_input=PC._handle_pointcloud_input)
     names = ['FoVPerspectiveCameras', 'PerspectiveCameras', 'RasterizationSettings', 'MeshRenderer', 'MeshRasterizer', 'BlendParams',
-             'DirectionalLights', 'PointLights', 'AmbientLights', 'TexturesVertex', 'look_at_view_transform', 'look_at_rotation',
+             'DirectionalLights', 'PointLights', 'AmbientLights', 'TexturesVertex',
              'SoftPhongShader', 'HardPhongShader', 'SoftSilhouetteShader', 'Materials']
-    _module('pytorch3d.renderer', TexturesUV=TexturesUV, **{n: P(f'renderer.{n}') for n in names})
+    _module('pytorch3d.renderer', TexturesUV=TexturesUV, look_at_view_transform=V.look_at_view_transform,
+            look_at_rotation=V.look_at_rotation, **{n: P(f'renderer.{n}') for n in names})
     _module('pytorch3d.renderer.mesh')
     _module('pytorch3d.renderer.mesh.shader', SoftPhongShader=P('renderer.mesh.shader.SoftPhongShader'))
     _module('pytorch3d.renderer.mesh.shading', phong_shading=P('phong_shading'), flat_shading=P('flat_shading'),

@@ -30,6 +30,7 @@
 #include "dbw_math.cuh"
 #include "dbw_fraglist.cuh"
 #include "dbw_camera.cuh"
+#include "dbw_viz_math.cuh"
 
 // ------------------------------------------------------------------------------------------------ error plumbing
 static thread_local char g_err[512] = "";
@@ -117,7 +118,8 @@ static bool keeps_colours(const DbwRenderSettings& s) {
   if (!s.save_fragment_state) return false;
   return g_keep_unread || !(s.save_fragment_state == 2 && s.faces_per_pixel == 1 && s.sigma == 0.f);
 }
-static Workspace carve(const DbwRenderSettings& s, void* base) {
+// bins = false: no coarse bins (a hard single-layer render never reads them; the resolving render leaves them out)
+static Workspace carve(const DbwRenderSettings& s, void* base, bool bins = true) {
   Workspace w; char* p = (char*)base; size_t off = 0;
   const size_t B = s.n_views, V = s.n_verts, S = 2 * (size_t)s.n_faces;
   w.verts_ndc = (float*)(p + off); off += align_up(B * V * 3 * sizeof(float));
@@ -132,7 +134,7 @@ static Workspace carve(const DbwRenderSettings& s, void* base) {
   // coarse bins: every list can hold all 2F slots (worst case), so they are only used while that stays below 1 GB
   w.cbin_nx = (s.width + DBW_CBIN - 1) / DBW_CBIN; w.cbin_ny = (s.height + DBW_CBIN - 1) / DBW_CBIN;
   const size_t nb = (size_t)w.cbin_nx * w.cbin_ny;
-  const bool use_bins = B * nb * S * sizeof(int) <= ((size_t)1 << 30) && nb > 1;
+  const bool use_bins = bins && B * nb * S * sizeof(int) <= ((size_t)1 << 30) && nb > 1;
   w.cbin_count = use_bins ? (int*)(p + off) : nullptr;  off += use_bins ? align_up(B * nb * sizeof(int)) : 0;
   w.cbin_list = use_bins ? (int*)(p + off) : nullptr;   off += use_bins ? align_up(B * nb * S * sizeof(int)) : 0;
   w.maps4 = (float4*)(p + off);    off += s.maps_are_texels4 ? 0 : align_up((size_t)(s.n_map_floats / 3) * sizeof(float4));
@@ -1078,7 +1080,47 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
 // identical to the generic kernel's: same edge functions, same (depth, slot) order.
 #define HARD_NT 256
 #define HARD_CAP 64
-__global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const RasterParams P) {
+// Outputs of the resolving variant (VIZ): the settings describe the 4H x 4W sample grid, these the H x W frames.
+struct VizOut {
+  const float* bkg; int bkg_stride;    // (1 or B, 3, H, W) background composited under the frame, or NULL; stride 0 or 3HW
+  float* rgba;                         // (B, 4, H, W) resolved RGBA (RGB composited when bkg), or NULL
+  unsigned char* rgb8;                 // (B, H, W, 3) uint8 frames, or NULL
+};
+__device__ __forceinline__ void hard_viz_resolve(const RasterParams& P, const VizOut& Z, bool live, int view, int xi, int yi,
+                                                 int lane, const float (&c)[4]);
+// texture coordinates (its record is read back from global memory: the tile list may have been recycled), colour and opacity
+// of the winning fragment of a hard single-layer pass.  The same operations as the tail of the plain kernel below, which keeps
+// its own copy: routing it through this function changes its instruction schedule (same registers, same results).
+struct HardShade { f3 color; float u, v, a; int map_id; };
+__device__ __forceinline__ HardShade hard_shade(const RasterParams& P, const int4* s_desc, int view, int best_slot, f3 best_bc) {
+  const size_t gs = (size_t)view * 2 * P.F + best_slot;
+  f3 bu = best_bc;
+  if (__float_as_int(__ldg(&P.rec[gs * 4 + 2]).w) & 1) {
+    const float* cv = P.conv + gs * 9;
+    bu.x = best_bc.x * cv[0] + best_bc.y * cv[3] + best_bc.z * cv[6];
+    bu.y = best_bc.x * cv[1] + best_bc.y * cv[4] + best_bc.z * cv[7];
+    bu.z = best_bc.x * cv[2] + best_bc.y * cv[5] + best_bc.z * cv[8];
+  }
+  const float4 q0 = __ldg(&P.rec2[gs * 2]), q1 = __ldg(&P.rec2[gs * 2 + 1]);
+  HardShade w;
+  w.u = bu.x * q0.x + bu.y * q0.z + bu.z * q1.x;
+  w.v = bu.x * q0.y + bu.y * q0.w + bu.z * q1.y;
+  w.map_id = __float_as_int(q1.z);
+  Texel4 tx;
+  fetch_color(P, w.u, w.v, s_desc[w.map_id], tx);
+  const int face = best_slot >= P.F ? best_slot - P.F : best_slot;
+  w.a = 1.f;                                         // inside a face of a hard pass: opacity 1 (x the face's entry)
+  if (P.faces_alpha) w.a *= __ldg(&P.faces_alpha[alpha_index(P, view, face)]);
+  if (P.face_shade) {
+    const float* m = P.face_shade + ((size_t)view * P.F + face) * 3;
+    tx.color.x *= __ldg(m); tx.color.y *= __ldg(m + 1); tx.color.z *= __ldg(m + 2);
+  }
+  w.color = tx.color;
+  return w;
+}
+
+template <bool VIZ>
+__device__ __forceinline__ void hard_forward_body(const RasterParams& P, const VizOut& Z) {
   __shared__ float4 s_bbox[HARD_CAP];
   __shared__ float4 s_rec[HARD_CAP * 4];
   __shared__ int s_slot[HARD_CAP];
@@ -1159,6 +1201,17 @@ __global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const R
       // (the next round's atomics come after the barrier at the top of the loop)
     }
   }
+  if (VIZ) {
+    // every lane takes part in the resolve's shuffles: a sample outside the image belongs to a frame pixel outside it
+    float c[4] = {P.bg0, P.bg1, P.bg2, 0.f};
+    if (live && best_j >= 0) {
+      const HardShade w = hard_shade(P, s_desc, view, best_slot, best_bc);
+      const float occ = 1.f - w.a;
+      c[0] = w.a * w.color.x + occ * P.bg0; c[1] = w.a * w.color.y + occ * P.bg1; c[2] = w.a * w.color.z + occ * P.bg2; c[3] = w.a;
+    }
+    hard_viz_resolve(P, Z, live, view, xi, yi, lane, c);
+    return;
+  }
   if (!live) return;
   const size_t plane = (size_t)P.H * P.W;
   const size_t pix = (size_t)yi * P.W + xi;
@@ -1201,6 +1254,46 @@ __global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const R
   const float occ = 1.f - a;
   o[0] = a * tx.color.x + occ * P.bg0; o[plane] = a * tx.color.y + occ * P.bg1; o[2 * plane] = a * tx.color.z + occ * P.bg2;
   o[3 * plane] = a;
+}
+
+__global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const RasterParams P) { hard_forward_body<false>(P, VizOut{}); }
+
+// The resolving variant renders the VizMeshRenderer frame (hard render on the 4H x 4W sample grid, avg_pool2d(., 4)) without
+// the sample image: a warp's 8 x 4 samples are the 4 x 4 samples of two frame pixels, which its lanes sum in registers.
+__global__ void __launch_bounds__(HARD_NT, 5) resolve_hard_viz_kernel(const RasterParams P, const VizOut Z) { hard_forward_body<true>(P, Z); }
+
+// The 16 samples of a frame pixel are lanes (g + c) + 8 r, r, c in [0, 4), g = 0 or 4.  Each sum runs in avg_pool2d's order
+// (dbw_viz_math.cuh), so the frame equals avg_pool2d(render at 4H x 4W, 4) bit for bit.
+__device__ __forceinline__ void hard_viz_resolve(const RasterParams& P, const VizOut& Z, bool live, int view, int xi, int yi,
+                                                 int lane, const float (&c)[4]) {
+  const int g = lane & 4;
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int ch = 0; ch < 4; ++ch) acc[ch] = dbw_viz_box_add(acc[ch], __shfl_sync(0xffffffffu, c[ch], r * 8 + g + k));
+  if (!live || (lane & ~4)) return;
+  const int H = P.H >> 2, W = P.W >> 2;
+  const size_t plane = (size_t)H * W, pix = (size_t)(yi >> 2) * W + (xi >> 2);
+  float f[4];
+#pragma unroll
+  for (int ch = 0; ch < 4; ++ch) f[ch] = dbw_viz_box_mean(acc[ch]);
+  if (Z.bkg) {
+    const float* b = Z.bkg + (size_t)view * Z.bkg_stride + pix;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) f[ch] = dbw_viz_composite(f[ch], f[3], __ldg(b + ch * plane));
+  }
+  if (Z.rgba) {
+    float* o = Z.rgba + (size_t)view * 4 * plane + pix;
+    o[0] = f[0]; o[plane] = f[1]; o[2 * plane] = f[2]; o[3 * plane] = f[3];
+  }
+  if (Z.rgb8) {
+    unsigned char* o = Z.rgb8 + ((size_t)view * plane + pix) * 3;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) o[ch] = dbw_viz_u8(f[ch]);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ backward
@@ -1992,11 +2085,12 @@ static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st) {
 
 // the backward scratch and the gradients a loss-epilogue forward computes itself (dbw_render_forward_loss_grad)
 struct EpilogueGrad { void* scratch; size_t scratch_bytes; int32_t mask; };
+// viz: the resolving hard render of dbw_render_forward_viz (its frames replace out_rgba)
 static int render_forward_impl(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream, const EpilogueGrad* eg = nullptr);
+                               void* stream, const EpilogueGrad* eg = nullptr, const VizOut* viz = nullptr);
 
 extern "C" int dbw_render_forward(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                   const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
@@ -2048,13 +2142,13 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream, const EpilogueGrad* eg) {
+                               void* stream, const EpilogueGrad* eg, const VizOut* viz) {
   if (validate(s)) return -1;
-  if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || (!out_rgba && !eg) || !workspace)
+  if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || (!out_rgba && !eg && !viz) || !workspace)
     return fail("dbw_render_forward: null pointer argument");
   if (!s->verts_are_ndc && (!R || !T)) return fail("dbw_render_forward: R and T are required unless verts_are_ndc");
   if (s->save_fragment_state == 2 && faces_alpha) return fail("dbw_render_forward: save_fragment_state = 2 declares a pass without faces_alpha");
-  Workspace w = carve(*s, workspace);
+  Workspace w = carve(*s, workspace, !viz);
   if (workspace_bytes < w.total) return fail("dbw_render_forward: workspace too small (see dbw_workspace_bytes)");
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s->n_views, V = s->n_verts, F = s->n_faces;
@@ -2106,7 +2200,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   {
     ScopedTimer timer(0, K, st);
     // a hard single-layer render without distances has its own kernel (dbw_debug_generic_kernel_only(1): the generic one)
-    const bool hard = K == 1 && s->sigma == 0.f && s->blur_radius == 0.f && !out_dists && !ep && !g_no_hard_kernel;
+    const bool hard = viz || (K == 1 && s->sigma == 0.f && s->blur_radius == 0.f && !out_dists && !ep && !g_no_hard_kernel);
     if (!hard && w.cbin_list) {
       coarse_bin_kernel<<<dim3(B, w.cbin_nx * w.cbin_ny), 256, 0, st>>>(w.bbox, w.view_flags, F, s->height, s->width, w.cbin_nx,
                                                                         w.cbin_ny, w.cbin_count, w.cbin_list);
@@ -2116,7 +2210,8 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
     }
     if (hard) {
       const dim3 grid(P.B, (P.W + 15) / 16, (P.H + 15) / 16);
-      raster_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P);
+      if (viz) resolve_hard_viz_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *viz);
+      else raster_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P);
     } else {
       const cudaError_t e = K <= 4 ? launch_forward<DBW_FWD_NT_SMALLK>(P, st) : launch_forward<DBW_FWD_NT>(P, st);
       if (e != cudaSuccess) return fail("raster_forward_kernel attribute", e);
@@ -2124,6 +2219,42 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   }
   LAUNCH_CK("raster_forward_kernel");
   return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ resolving hard render
+// settings that dbw_render_forward_viz cannot serve (NULL: none); the settings describe the factor x factor sample grid
+static const char* viz_unsupported(const DbwRenderSettings& s, int32_t factor) {
+  if (factor != 4) return "factor must be 4 (the supersampling of the reference's VizMeshRenderer)";
+  if (s.faces_per_pixel != 1 || s.sigma != 0.f || s.blur_radius != 0.f) return "a hard render needs faces_per_pixel = 1, sigma = 0, blur_radius = 0";
+  if (s.height % factor || s.width % factor) return "height and width (of the sample grid) must be multiples of factor";
+  if (s.view_rows) return "view_rows is not supported";
+  if (s.save_fragment_state) return "no fragment records are written (save_fragment_state must be 0)";
+  return nullptr;
+}
+
+extern "C" int dbw_viz_workspace_bytes(const DbwRenderSettings* s, int32_t factor, size_t* bytes) {
+  if (validate(s)) return -1;
+  if (const char* why = viz_unsupported(*s, factor)) { char msg[192]; snprintf(msg, sizeof(msg), "dbw_viz_workspace_bytes: %s", why); return fail(msg); }
+  if (!bytes) return fail("dbw_viz_workspace_bytes: null output");
+  *bytes = carve(*s, nullptr, false).total;
+  return 0;
+}
+
+extern "C" int dbw_render_forward_viz(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
+                                      const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
+                                      const float* T, const float* faces_alpha, const float* face_shade, int32_t factor,
+                                      const float* bkg, int32_t bkg_views, float* out_rgba, uint8_t* out_rgb8, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  if (validate(s)) return -1;
+  const char* why = viz_unsupported(*s, factor);
+  if (!why && !out_rgba && !out_rgb8) why = "out_rgba and out_rgb8 are both NULL";
+  if (!why && bkg && bkg_views != 1 && bkg_views != s->n_views) why = "bkg_views must be 1 or n_views";
+  if (why) { char msg[192]; snprintf(msg, sizeof(msg), "dbw_render_forward_viz: %s", why); return fail(msg); }
+  const size_t plane = (size_t)(s->height / factor) * (s->width / factor);
+  if (3 * plane > (size_t)INT32_MAX) return fail("dbw_render_forward_viz: frame too large");
+  const VizOut viz = {bkg, bkg && bkg_views > 1 ? (int)(3 * plane) : 0, out_rgba, out_rgb8};
+  return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, nullptr, nullptr,
+                             workspace, workspace_bytes, face_shade, nullptr, nullptr, stream, nullptr, &viz);
 }
 
 // adds the cell-gradient copies of the backward scratch into g_maps, times *scale (NULL = 1)

@@ -713,11 +713,15 @@ class DifferentiableBlocksWorld(nn.Module):
 
     @torch.no_grad()
     def qualitative_eval(self, loader, device, path=None, NV=240, n_inputs=10):
-        """the still images and meshes of dbw.py:495-554: texture maps, the scene as OBJ (with and without background), and
-        per input view the hard reconstruction, its block-coloured edge overlays and the lit synthetic-colour render.
-        The reference's mp4 trajectories (NV frames through imageio / ffmpeg) and the ground-truth point-cloud PLY are
-        export paths outside the render hot path and are not written."""
+        """the outputs of dbw.py:495-554: texture maps, the scene as OBJ (with and without background), `gt.ply` (3000 points
+        of loader.dataset.pc_gt, seed 123) when the dataset has a ground-truth cloud, `rotated_mesh.mp4` (NV frames around
+        the scene), and per input view the hard reconstruction, its block-coloured edge overlays, the lit synthetic-colour
+        render and the videos `{tag}_rec_traj.mp4` / `{tag}_rec_traj_syn.mp4` (NV frames along get_circle_traj about the
+        view; with per-view intrinsics, drawn with the view's own K).  Videos are rendered by the resolving kernel
+        (views.py) and written with OpenCV; without OpenCV they are skipped with a warning.  Returns the number of views."""
         from pathlib import Path
+        from . import views
+        from .dtu_eval import write_ply
         path = Path(path) if path is not None else Path('.')
         path.mkdir(parents=True, exist_ok=True)
         self.eval()
@@ -732,6 +736,13 @@ class DifferentiableBlocksWorld(nn.Module):
         syn_blocks = self.build_blocks(filter_transparent=True, synthetic_colors=True, as_scene=True)
         if len(syn_blocks) == 0:
             return None
+        gt = getattr(getattr(loader, 'dataset', None), 'pc_gt', None)
+        if gt is not None:
+            gt = torch.as_tensor(gt)
+            write_ply(path / 'gt.ply', gt[torch.randperm(len(gt), generator=torch.Generator().manual_seed(123))[:3000]].cpu().numpy())
+        videos = _video_writer_available()
+        R_traj, _ = views.get_circle_traj(N_views=NV)
+        R_traj = R_traj.to(device)
         colors = self.get_scene_face_colors(filter_transparent=True, w_env=False)
         count, n_zeros = 0, int(np.log10(max(n_inputs - 1, 1))) + 1
         for inp, labels in loader:
@@ -753,8 +764,32 @@ class DifferentiableBlocksWorld(nn.Module):
                 _save_png(syn[0], path / f'{tag}_rec_syn_nobkg.png')
                 _save_png(self.renderer_light.draw_edges(syn, syn_blocks, R, T, linewidth=0.7, colors=(0.3, 0.3, 0.3), K=K)[0],
                           path / f'{tag}_rec_syn_nobkg_edged.png')
+                if videos:
+                    R_k, T_k = R @ R_traj, T.expand(NV, -1)
+                    views.save_trajectory_as_video(meshes, path / f'{tag}_rec_traj.mp4', R_k, T_k, renderer=self.renderer, K=K)
+                    views.save_trajectory_as_video(syn_blocks, path / f'{tag}_rec_traj_syn.mp4', R_k, T_k, renderer=self.renderer_light,
+                                                   K=K)
                 count += 1
+        if videos:        # after the first batch has installed the renderers' camera (the reference's is set during training)
+            views.save_mesh_as_video(meshes, path / 'rotated_mesh.mp4', n_views=NV, renderer=self.renderer)
         return count
+
+
+_WARNED_NO_CV2 = False
+
+
+def _video_writer_available():
+    """OpenCV writes the videos; without it qualitative_eval warns once and writes the stills only"""
+    global _WARNED_NO_CV2
+    try:
+        import cv2  # noqa: F401
+        return True
+    except ImportError as exc:
+        if not _WARNED_NO_CV2:
+            import warnings
+            warnings.warn(f'[dbw_b200] OpenCV is unavailable ({exc}): qualitative_eval writes no videos', RuntimeWarning)
+            _WARNED_NO_CV2 = True
+        return False
 
 
 def _save_png(chw, path):

@@ -308,6 +308,70 @@ def render_scene(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, 
     return res                           # rgba | (rgba, slot ids) | (rgba, slot ids, signed squared distances)
 
 
+VIZ_FACTOR = 4      # VizMeshRenderer's supersampling (renderer.py:56-60)
+
+
+def _viz_settings(verts, faces, maps, map_table_host, B, intr, image_size, z_clip, detach_bary, clip_inside, background,
+                  perspective_correct, verts_are_ndc):
+    """settings of a resolving render: the hard pass (K = 1, sigma = 0) on the 4H x 4W sample grid of (H, W) frames"""
+    H, W = image_size
+    with torch.no_grad():            # no fragment records
+        return scene_settings(verts, faces, maps, map_table_host, B, intr, (H * VIZ_FACTOR, W * VIZ_FACTOR), 0.0, 1, z_clip,
+                              detach_bary, clip_inside, background, perspective_correct=perspective_correct,
+                              verts_are_ndc=verts_are_ndc, blur_radius=0.0)
+
+
+def viz_bytes(n_verts, n_faces, map_table_host, maps_numel, B, image_size):
+    """device bytes of a resolving render of B (H, W) frames: workspace, float RGBA frames and uint8 frames"""
+    s = make_settings(B, image_size[0] * VIZ_FACTOR, image_size[1] * VIZ_FACTOR, 1, n_verts, n_faces, len(map_table_host), 0,
+                      (1., 1., 0., 0.), 0.0, 0.0, None, (0., 0., 0.), n_map_floats=maps_numel)
+    ws = ctypes.c_size_t(0)
+    _lib.check(_lib.lib().dbw_viz_workspace_bytes(ctypes.byref(s), VIZ_FACTOR, ctypes.byref(ws)), 'dbw_viz_workspace_bytes')
+    return ws.value + B * image_size[0] * image_size[1] * (4 * 4 + 3)
+
+
+@torch.no_grad()
+def render_scene_viz(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, intr, image_size, z_clip=None,
+                     detach_bary=False, clip_inside=True, background=(0., 0., 0.), perspective_correct=True, face_shade=None,
+                     bkg=None, frames_u8=False):
+    """VizMeshRenderer's frame (renderer.py:56-60,178-183) in one kernel: the hard render at 4H x 4W resolved 4x4 on chip
+    (dbw_render_forward_viz), equal bit for bit to avg_pool2d(render_scene(..., (4H, 4W), 0.0, 1, ...), 4).
+    Arguments as render_scene; image_size is the (H, W) of the frames.  bkg (3,H,W) or (1 | B,3,H,W): composited under the
+    RGB as rec * alpha + (1 - alpha) * bkg.  Returns rgba (B,4,H,W), and with frames_u8 also (B,H,W,3) uint8 frames,
+    uint8(trunc(clamp(rgb * 255, 0, 255))) of the same RGB."""
+    if torch.is_tensor(intr):
+        verts, R, T, intr, verts_are_ndc = project_verts(verts, R, T, intr), None, None, (1., 1., 0., 0.), True
+    else:
+        verts_are_ndc = False
+    dev = verts.device
+    if not verts.is_cuda:
+        raise DbwError('the CUDA renderer needs CUDA tensors (there is no CPU fallback)')
+    B = R.shape[0] if R is not None else verts.shape[0]
+    H, W = image_size
+    cfg, map_table = _viz_settings(verts, faces, maps, map_table_host, B, intr, image_size, z_clip, detach_bary, clip_inside,
+                                   background, perspective_correct, verts_are_ndc)
+    if R is None:
+        R = torch.eye(3, device=dev)[None].expand(B, -1, -1)
+        T = torch.zeros(B, 3, device=dev)
+    L = _lib.lib()
+    ws_bytes = ctypes.c_size_t(0)
+    _lib.check(L.dbw_viz_workspace_bytes(ctypes.byref(cfg), VIZ_FACTOR, ctypes.byref(ws_bytes)), 'dbw_viz_workspace_bytes')
+    ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
+    n_bkg = 0
+    if bkg is not None:
+        bkg = bkg.to(device=dev, dtype=torch.float32).reshape(-1, 3, H, W).contiguous()
+        n_bkg = bkg.shape[0]
+    rgba = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)
+    rgb8 = torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev) if frames_u8 else None
+    # converted copies are held until the launch is enqueued: a temporary freed earlier could be handed to the next one
+    args = [verts.contiguous().float(), faces.to(torch.int32).contiguous(), faces_uvs.contiguous().float(),
+            face_map.to(torch.int32).contiguous(), maps.contiguous().float(), map_table, R.contiguous().float(),
+            T.contiguous().float(), None, face_shade.contiguous().float() if face_shade is not None else None]
+    _lib.check(L.dbw_render_forward_viz(ctypes.byref(cfg), *[_c(a) for a in args], VIZ_FACTOR, _c(bkg), n_bkg, _c(rgba), _c(rgb8),
+                                        _c(ws), ws.numel(), _stream()), 'dbw_render_forward_viz')
+    return (rgba, rgb8) if frames_u8 else rgba
+
+
 class Renderer(nn.Module):
     def __init__(self, img_size, **kwargs):
         super().__init__()
@@ -373,16 +437,20 @@ class Renderer(nn.Module):
         maps, table = meshes.textures.packed_maps()
         return verts, faces, fvu, fmap, maps, table
 
-    def forward(self, meshes, R, T, viz_purpose=False, **kwargs):
+    def _shade(self, verts, faces, R):
+        """the per-(view, face) flat-shading multiplier of a lit renderer, None for the raw one"""
         lit = self.light_kwargs.get('name', 'ambient') == 'directional'
         if self.shading_type not in ('raw', 'flat') or (lit != (self.shading_type == 'flat')):
             raise NotImplementedError(f'shading_type={self.shading_type} with lights={self.light_kwargs.get("name", "ambient")}: '
                                       'only raw+ambient (training) and flat+directional (renderer_light) are implemented')
+        return self._flat_shade(verts, faces, R) if lit else None
+
+    def forward(self, meshes, R, T, viz_purpose=False, **kwargs):
         faces_alpha, K = kwargs.get('faces_alpha'), kwargs.get('K')
         verts, faces, fvu, fmap, maps, table = self._scene(meshes)
         H, W = self.img_size
         intr = K if K is not None else self.cameras.intrinsics()      # K (B,4,4): each view with its own intrinsics
-        shade = self._flat_shade(verts, faces, R) if lit else None
+        shade = self._shade(verts, faces, R)
         if viz_purpose:
             # VizMeshRenderer (renderer.py:56-60,178-183): hard 4x supersampled render, box-filtered, no gradient
             with torch.no_grad():
@@ -393,6 +461,23 @@ class Renderer(nn.Module):
         return render_scene(verts, faces, fvu, fmap, maps, table, R, T, intr, (H, W), self.sigma, self.faces_per_pixel,
                             self.z_clip, self.detach_bary, self.clip_inside, self.background_color, faces_alpha,
                             self.perspective_correct, blur_radius=self.blur_radius, face_shade=shade)
+
+    @torch.no_grad()
+    def render_viz(self, meshes, R, T, K=None, bkg=None, frames_u8=False):
+        """forward(meshes, R, T, viz_purpose=True, K=K) -- the same bits -- in one resolving kernel that never writes the 4x
+        supersampled image (render_scene_viz): rgba (B,4,H,W), RGB composited over bkg ((3,H,W) or (1 | B,3,H,W)) when given;
+        with frames_u8 also the (B,H,W,3) uint8 frames a video encoder takes.  No gradient."""
+        verts, faces, fvu, fmap, maps, table = self._scene(meshes)
+        intr = K if K is not None else self.cameras.intrinsics()
+        return render_scene_viz(verts, faces, fvu, fmap, maps, table, R, T, intr, self.img_size, self.z_clip, self.detach_bary,
+                                self.clip_inside, self.background_color, self.perspective_correct,
+                                face_shade=self._shade(verts, faces, R), bkg=bkg, frames_u8=frames_u8)
+
+    def viz_bytes(self, meshes, n_views):
+        """device bytes render_viz needs for n_views frames of this renderer"""
+        verts, faces = meshes.get_mesh_verts_faces(0)
+        maps, table = meshes.textures.packed_maps()
+        return viz_bytes(verts.shape[-2], faces.shape[0], table, maps.numel(), n_views, self.img_size)
 
     # ------------------------------------------------------------------ edge overlays (renderer.py:134-175)
     @torch.no_grad()

@@ -136,6 +136,27 @@ int dbw_render_forward(const DbwRenderSettings* settings, const float* verts, co
                        const float* face_shade, float* out_dists, void* stream);
 
 /*
+ * Resolving hard render of VizMeshRenderer (src/model/renderer.py:56-60,178-183): the hard render (faces_per_pixel = 1,
+ * sigma = 0, blur_radius = 0) on the factor x factor sample grid that `settings` describes (height and width are the SAMPLE
+ * grid's, multiples of factor), box-filtered to H = height / factor, W = width / factor inside the raster kernel.  The sample
+ * image never reaches memory.  Arguments up to face_shade are dbw_render_forward's.
+ *   factor     4 (the only supersampling of the reference); anything else is refused
+ *   bkg        (bkg_views, 3, H, W) background composited under each frame, rec * alpha + (1 - alpha) * bkg, or NULL;
+ *              bkg_views is 1 (shared) or n_views
+ *   out_rgba   (B,4,H,W) frames, or NULL: equal bit for bit to avg_pool2d(dbw_render_forward at height x width, factor),
+ *              then (with bkg) the composite of the RGB planes in torch's order; the alpha plane is never composited
+ *   out_rgb8   (B,H,W,3) uint8(trunc(clamp(rgb * 255, 0, 255))) of the same RGB, or NULL (not both NULL)
+ *   workspace  dbw_viz_workspace_bytes() bytes (no coarse bins, no fragment records: save_fragment_state must be 0)
+ * view_rows is refused.  dbw_debug_generic_kernel_only does not apply.
+ */
+int dbw_viz_workspace_bytes(const DbwRenderSettings* settings, int32_t factor, size_t* bytes);
+int dbw_render_forward_viz(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
+                           const float* faces_uvs, const int32_t* face_map, const float* maps,
+                           const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                           const float* face_shade, int32_t factor, const float* bkg, int32_t bkg_views,
+                           float* out_rgba, uint8_t* out_rgb8, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Backward of the same (replaces autograd through layered_rgb_blend, grid_sample, interpolate_face_attributes
  * and _C.rasterize_meshes_backward).  grad_rgba (B,4,H,W), multiplied by the device scalar *grad_scale (NULL = 1) as it is
  * read.  Outputs accumulate:
