@@ -83,7 +83,7 @@ class DbwMapDesc(ctypes.Structure):
                 ('reserved', ctypes.c_int32)]
 
 
-EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
+EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generic_blocks_loss', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
            'dbw_render_forward_loss', 'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_camera_project', 'dbw_camera_project_backward',
            'dbw_composite_mse', 'dbw_composite_mse_backward', 'dbw_render_forward_host', 'dbw_host_arena_release', 'dbw_launch_count',
@@ -148,6 +148,8 @@ def lib():
         L.dbw_comm_destroy.argtypes = [vp]
         L.dbw_debug_generic_kernel_only.restype = None
         L.dbw_debug_generic_kernel_only.argtypes = [ctypes.c_int]
+        L.dbw_debug_generic_blocks_loss.restype = None
+        L.dbw_debug_generic_blocks_loss.argtypes = [ctypes.c_int]
         L.dbw_debug_keep_unread_outputs.restype = None
         L.dbw_debug_keep_unread_outputs.argtypes = [ctypes.c_int]
         L.dbw_texture_prep_forward_multi.argtypes = [ctypes.POINTER(DbwTexJob), ctypes.c_int32, vp]
@@ -209,7 +211,7 @@ def launch_count():
 
 
 def kernel_time_ms(kind, K=0):
-    """(total ms, launches) of the raster kernel `kind` (0 forward, 1 backward) recorded since the last reset."""
+    """(total ms, launches) of the raster kernel `kind` (0 forward, 1 backward, 2 the blocks loss kernel) recorded since the last reset."""
     tot, n = ctypes.c_double(0), ctypes.c_int(0)
     check(lib().dbw_timing_read(kind, K, ctypes.byref(tot), ctypes.byref(n)), 'dbw_timing_read')
     return tot.value, n.value

@@ -95,6 +95,9 @@ typedef struct DbwMapDesc { int32_t offset, height, width, reserved; } DbwMapDes
 int dbw_abi_version(void);
 /* Test hook: 1 = hard single-layer renders (K = 1, sigma = 0) go through the generic raster kernel instead of their dedicated one. */
 void dbw_debug_generic_kernel_only(int on);
+/* Test / benchmark hook: 1 = the coarse phase's blocks loss pass (dbw_render_forward_loss_grad with faces_per_pixel > 4) runs
+ * the generic raster kernel instead of its dedicated one.  The loss is the same bit for bit. */
+void dbw_debug_generic_blocks_loss(int on);
 /* Test hook: 1 = keep writing what no backward reads (the colours of a save_fragment_state = 2 hard single-layer pass, the
  * alpha plane of an env_alpha_unread epilogue's g_env), for tests that compare against the computation that writes them.  Set it before
  * dbw_workspace_bytes: it changes the forward workspace's size. */
@@ -371,7 +374,8 @@ void dbw_host_arena_release(void);
 uint64_t dbw_launch_count(void);
 
 /* Optional live timing of the two rasterization kernels with CUDA events on the launch stream (bench.py's roofline):
- * kind 0 = raster forward, 1 = raster backward; K filters by faces_per_pixel (0 = any).  dbw_timing_read synchronises
+ * kind 0 = raster forward, 1 = raster backward, 2 = the dedicated blocks loss kernel alone (inside kind 0); K filters by
+ * faces_per_pixel (0 = any).  dbw_timing_read synchronises
  * on the recorded events and returns their summed duration and count; dbw_timing_reset frees them. */
 void dbw_timing_enable(int on);
 int dbw_timing_read(int kind, int K, double* total_ms, int* count);
