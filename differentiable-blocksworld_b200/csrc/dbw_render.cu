@@ -689,10 +689,12 @@ __device__ __forceinline__ TexTap map_tap(float u, float v, int4 d) {
   return t;
 }
 __device__ __forceinline__ void tap_only(float u, float v, int4 d, Texel4& s) { s.tap = map_tap(u, v, d); }
+// CELLS: the caller knows that d is a cell map (d.w != 0)
+template <bool CELLS = false>
 __device__ __forceinline__ void fetch_color(const RasterParams& P, float u, float v, int4 d, Texel4& s) {
   s.tap = map_tap(u, v, d);
   s.c00 = ld_texel(P.maps4, s.tap.i00);
-  if (d.w) {          // cell map: the four taps usually share one cell (49 of 64 footprints at f = 8); each distinct cell is loaded once
+  if (CELLS || d.w) { // cell map: the four taps usually share one cell (49 of 64 footprints at f = 8); each distinct cell is loaded once
     s.c01 = s.tap.i01 == s.tap.i00 ? s.c00 : ld_texel(P.maps4, s.tap.i01);
     s.c10 = s.tap.i10 == s.tap.i00 ? s.c00 : ld_texel(P.maps4, s.tap.i10);
     s.c11 = s.tap.i11 == s.tap.i01 ? s.c01 : (s.tap.i11 == s.tap.i10 ? s.c10 : ld_texel(P.maps4, s.tap.i11));
@@ -758,16 +760,24 @@ __device__ __forceinline__ int centre_out(int rank, int n) {
   return (rank & 1) ? c - ((rank + 1) >> 1) : c + (rank >> 1);
 }
 
+template <bool BLOCKS>
 __device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4* lA, float* lV, int stride, const int4* s_desc,
                                                   float* s_galpha, bool live, int n, f2 p, const float (&g)[4], int view,
                                                   int lane, int warp);
 
-// One kernel for every K: the per-pixel list of the K nearest fragments lives in (dynamic) shared memory (dbw_fraglist.cuh).
+// One body for every K: the per-pixel list of the K nearest fragments lives in (dynamic) shared memory (dbw_fraglist.cuh).
 // EP: with the compositing + MSE loss epilogue (DbwLossEpilogue); a template flag so that plain renders carry none of it.
 // With P.ep_grad the epilogue then also runs the pass's detach_bary backward on the list still in shared memory
 // (epilogue_backward): no fragment record and no gradient image goes through HBM.
-template <int NT, bool EP>
-__global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_MINB) raster_forward_kernel(const RasterParams P) {
+// BLOCKS (with EP, NT = 128: blocks_loss_kernel): the coarse phase's blocks loss pass, which the dispatch sends here only with
+// ep_grad, cell maps, no optional output (fragment records, ids, distances, flat shading, image) and at most
+// DBW_ALPHA_SMEM_MAX opacity entries per view.  The branches it never takes are compiled out, and the view's opacity table
+// is staged in shared memory beside the opacity sums, so that the shading loop and the backward's pass 1 read no global
+// memory but the texels.  Every decision and every loss term is the generic instantiation's; the gradients differ only by
+// the order of their atomics.
+template <int NT, bool EP, bool BLOCKS>
+__device__ __forceinline__ void raster_forward_body(const RasterParams& P) {
+  static_assert(!BLOCKS || (EP && NT == 128), "the blocks loss pass is a loss-epilogue pass of 128 threads");
   // faces a tile lists at once (more: chunked path)
 #ifndef DBW_LIST_CAP
 #define DBW_LIST_CAP 64      // tile lists average 17 faces (max 64) at cfg 2: 5 KB instead of 10.5 KB buys a 7th resident CTA
@@ -780,7 +790,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   __shared__ int s_count;
   __shared__ __align__(8) uint64_t s_bar;      // mbarrier of the TMA record gather
   extern __shared__ float4 s_dyn[];            // fragment lists: K*NT float4 (pz, bits, sd, u), K*NT float (v); then the map table
-                                               // (and with ep_grad the opacity sums)
+                                               // (and with ep_grad the opacity sums, then with BLOCKS the opacity table)
   uint32_t bar_phase = 0;
 
   constexpr int TILE_H = NT / 16;
@@ -805,10 +815,13 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   // the bin scan, so that nobody waits for it
   int4* const s_desc = reinterpret_cast<int4*>(reinterpret_cast<float*>(s_dyn + (size_t)P.K * NT) + (size_t)P.K * NT);
   float* const s_galpha = reinterpret_cast<float*>(s_desc + P.M);
-  if (EP && P.ep_grad && P.faces_alpha && P.g_faces_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX)
-    for (int i = tid; i < P.n_alpha; i += NT) s_galpha[i] = 0.f;
+  float* const s_alpha = s_galpha + P.n_alpha;
+  const bool alpha_sums = EP && (BLOCKS || (P.ep_grad && P.n_alpha <= DBW_ALPHA_SMEM_MAX)) && P.faces_alpha && P.g_faces_alpha;
+  if (alpha_sums) for (int i = tid; i < P.n_alpha; i += NT) s_galpha[i] = 0.f;
   DbwMapDesc my_desc = {0, 0, 0, 0};
   if (tid < P.M) my_desc = P.map_table[tid];
+  float my_alpha = 0.f;          // BLOCKS: this thread's opacity entry, stored with its map-table entry
+  if (BLOCKS && P.faces_alpha && tid < P.n_alpha) my_alpha = __ldg(&P.faces_alpha[(size_t)view * P.alpha_stride + tid]);
   const int4 vbox = __ldg(reinterpret_cast<const int4*>(P.view_bbox) + view);      // in flight across the barrier
   const int vflags = __ldg(P.view_flags + view);
   __syncthreads();
@@ -834,7 +847,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   const size_t slot_base = (size_t)view * 2 * P.F;
   const float4* bbox = P.bbox + slot_base;
   const float4* rec = P.rec + slot_base * 4;
-  const bool dist_inside = (!P.clip_inside && P.sigma > 0.f) || P.out_dists != nullptr;
+  const bool dist_inside = (!P.clip_inside && P.sigma > 0.f) || (!BLOCKS && P.out_dists != nullptr);
 
   // stage the records of the `cnt` listed faces in shared memory, then test every pixel against every listed face
   auto raster_list = [&](int cnt) {
@@ -928,6 +941,10 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   }
   if (tid < P.M) s_desc[tid] = make_int4(my_desc.offset / 3, my_desc.height, my_desc.width, my_desc.reserved);
   for (int m = tid + NT; m < P.M; m += NT) { const DbwMapDesc d = P.map_table[m]; s_desc[m] = make_int4(d.offset / 3, d.height, d.width, d.reserved); }
+  if (BLOCKS && P.faces_alpha) {
+    if (tid < P.n_alpha) s_alpha[tid] = my_alpha;
+    for (int i = tid + NT; i < P.n_alpha; i += NT) s_alpha[i] = __ldg(&P.faces_alpha[(size_t)view * P.alpha_stride + i]);
+  }
   __syncthreads();
   const int total = s_count;
   if (total <= CAP) {
@@ -997,24 +1014,25 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   }
 #pragma unroll 1
   for (int k = 0; k < n; ++k) {
+    if (BLOCKS && occ == 0.f) break;      // no per-layer output: every later layer contributes exactly 0
     const float4 e = lA[k * NT];
     const int bits = __float_as_int(e.y), slot = bits & DBW_FRAG_SLOT_MASK;
     const float d0 = e.z;
-    if (P.topk) P.topk[((size_t)view * K + k) * plane + pix] = slot;
-    if (P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = d0;
+    if (!BLOCKS && P.topk) P.topk[((size_t)view * K + k) * plane + pix] = slot;
+    if (!BLOCKS && P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = d0;
     if (occ == 0.f) continue;     // behind a fully opaque fragment (fine phase: alpha = 1 inside a face): contributes exactly 0
     n_saved = k + 1;
     const float v = lV[k * NT];
     const int face = slot >= P.F ? slot - P.F : slot;
     Texel4 tx;
-    fetch_color(P, e.w, v, s_desc[(unsigned)bits >> DBW_FRAG_MAP_SHIFT], tx);
+    fetch_color<BLOCKS>(P, e.w, v, s_desc[(unsigned)bits >> DBW_FRAG_MAP_SHIFT], tx);
     float a = frag_alpha(d0, P.sigma, P.clip_inside);
-    if (P.faces_alpha) a *= __ldg(&P.faces_alpha[alpha_index(P, view, face)]);
-    if (P.face_shade) {          // flat shading: colour = texel * (ambient + diffuse * relu(n . l)) per (view, face)
+    if (P.faces_alpha) a *= BLOCKS ? s_alpha[alpha_index(P, 0, face)] : __ldg(&P.faces_alpha[alpha_index(P, view, face)]);
+    if (!BLOCKS && P.face_shade) {          // flat shading: colour = texel * (ambient + diffuse * relu(n . l)) per (view, face)
       const float* m = P.face_shade + ((size_t)view * P.F + face) * 3;
       tx.color.x *= __ldg(m); tx.color.y *= __ldg(m + 1); tx.color.z *= __ldg(m + 2);
     }
-    if (P.frag) {                 // what the backward streams instead of re-deriving geometry and texels: two 16 B records
+    if (!BLOCKS && P.frag) {      // what the backward streams instead of re-deriving geometry and texels: two 16 B records
       const size_t fi = ((size_t)view * K + k) * plane + pix;
       P.frag[fi] = make_float4(e.y, e.w, v, d0);
       if (P.frag_rgb) P.frag_rgb[fi] = make_float4(tx.color.x, tx.color.y, tx.color.z, 0.f);
@@ -1023,10 +1041,10 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     r += w * tx.color.x; g += w * tx.color.y; bl += w * tx.color.z;
     occ *= (1.f - a);
   }
-  if (P.nfrag) P.nfrag[(size_t)view * plane + pix] = (unsigned char)n_saved;
+  if (!BLOCKS && P.nfrag) P.nfrag[(size_t)view * plane + pix] = (unsigned char)n_saved;
   for (int k = n; k < K; ++k) {
-    if (P.topk) P.topk[((size_t)view * K + k) * plane + pix] = -1;
-    if (P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = -1.f;
+    if (!BLOCKS && P.topk) P.topk[((size_t)view * K + k) * plane + pix] = -1;
+    if (!BLOCKS && P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = -1.f;
   }
   float* o = P.out_rgba + (size_t)view * 4 * plane + pix;
   const float fc[3] = {r + occ * P.bg0, g + occ * P.bg1, bl + occ * P.bg2};
@@ -1052,11 +1070,11 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
       gm += gr * (fc[c] - ec);
     }
     ep_g[3] = gm;
-    if (P.out_rgba) { o[0] = ep_g[0]; o[plane] = ep_g[1]; o[2 * plane] = ep_g[2]; o[3 * plane] = gm; }
+    if (!BLOCKS && P.out_rgba) { o[0] = ep_g[0]; o[plane] = ep_g[1]; o[2 * plane] = ep_g[2]; o[3 * plane] = gm; }
     if (!P.ep_skip_env_alpha) ge[3 * plane] = 0.f;
   }
   }   // live
-  if (EP && P.ep_grad) epilogue_backward(P, lA, lV, NT, s_desc, s_galpha, live, n_saved, p, ep_g, view, lane, warp);
+  if (BLOCKS || (EP && P.ep_grad)) epilogue_backward<BLOCKS>(P, lA, lV, NT, s_desc, s_galpha, live, n_saved, p, ep_g, view, lane, warp);
   if (EP) {
     // one atomic per warp into a strip of partial sums (the caller adds them up): no single hot address
 #pragma unroll
@@ -1066,7 +1084,7 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
       atomicAdd(&P.ep_partials[(cta * (NT / 32) + warp) & P.ep_part_mask], ep_sq * P.ep_inv_count);
     }
   }
-  if (EP && P.ep_grad && P.faces_alpha && P.g_faces_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX) {
+  if (alpha_sums) {
     __syncthreads();                 // one global atomic per (CTA, opacity entry), as in raster_backward_kernel
     for (int i = tid; i < P.n_alpha; i += NT) {
       const float v = s_galpha[i];
@@ -1074,6 +1092,12 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
     }
   }
 }
+
+template <int NT, bool EP>
+__global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_MINB) raster_forward_kernel(const RasterParams P) {
+  raster_forward_body<NT, EP, false>(P);
+}
+__global__ void __launch_bounds__(128, DBW_FWD_MINB) blocks_loss_kernel(const RasterParams P) { raster_forward_body<128, true, true>(P); }
 
 // ------------------------------------------------------------------------------------------------ hard single-layer forward
 // K = 1, sigma = 0 (the environment pass, src/model/dbw.py:135-138,219; VizMeshRenderer's 4x supersampled renders,
@@ -1610,7 +1634,9 @@ __device__ __forceinline__ void suffix_backward(const RasterParams& P, const flo
 // dist, u) and lV (v), `stride` apart -- so pass 1 re-fetches each layer's texels (L1/L2-resident), scatters the texture
 // gradient into the CTA's cell-gradient copy and overwrites the entry, whose depth and UV are dead by then, with what pass 2
 // needs: (alpha, cdot, e, occ) in lA and the bits in lV.  Pass 2 is suffix_backward.  n: the layers the shading loop
-// blended.  Called by every lane of the warp (lanes that are not `live` take part with empty keys).
+// blended.  Called by every lane of the warp (lanes that are not `live` take part with empty keys).  BLOCKS (blocks_loss_kernel):
+// cell maps, the opacities from the table staged after the sums, and the sums always in shared memory.
+template <bool BLOCKS>
 __device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4* lA, float* lV, int stride, const int4* s_desc,
                                                   float* s_galpha, bool live, int n, f2 p, const float (&g)[4], int view,
                                                   int lane, int warp) {
@@ -1631,9 +1657,10 @@ __device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4*
       const int face = slot >= P.F ? slot - P.F : slot;
       const int4 desc = s_desc[(unsigned)bits >> DBW_FRAG_MAP_SHIFT];
       Texel4 tx;
-      fetch_color(P, e.w, lV[k * stride], desc, tx);
+      fetch_color<BLOCKS>(P, e.w, lV[k * stride], desc, tx);
       const float ea = frag_alpha(e.z, P.sigma, P.clip_inside);
-      const float a = P.faces_alpha ? ea * __ldg(&P.faces_alpha[alpha_index(P, view, face)]) : ea;
+      const float a = !P.faces_alpha ? ea : ea * (BLOCKS ? s_galpha[P.n_alpha + alpha_index(P, 0, face)]
+                                                         : __ldg(&P.faces_alpha[alpha_index(P, view, face)]));
       const float cdot = tx.color.x * gr + tx.color.y * gg + tx.color.z * gb;
       lA[k * stride] = make_float4(a, cdot, ea, occ);
       lV[k * stride] = __int_as_float(bits);
@@ -1649,445 +1676,7 @@ __device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4*
   }
   const bool want_alpha = P.faces_alpha != nullptr && P.g_faces_alpha != nullptr;
   suffix_backward(P, lA, reinterpret_cast<const int*>(lV), stride, n_px, n_warp, p, gr, gg, gb, ga, view, (size_t)view * 2 * P.F,
-                  want_alpha, want_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX, s_galpha, P.sigma > 0.f && P.g_tri != nullptr, lane);
-}
-
-// ------------------------------------------------------------------------------------------------ coarse-phase blocks loss pass
-// blocks_loss_kernel: raster_forward_kernel<128, true> with ep_grad, specialised to what dbw_render_forward_loss_grad serves
-// at K > 4 (detach_bary, cell maps, no fragment records, no ids / distances / flat shading / image output, at most
-// DBW_ALPHA_SMEM_MAX opacity entries per view): the branches it can never take are gone, and the view's opacity table is
-// staged in shared memory once per CTA beside the opacity sums, so that the shading loop and the backward's pass 1 read no
-// global memory but the texels.  Every decision and every loss term is the generic kernel's: the same dbw_math.cuh /
-// dbw_fraglist.cuh functions in the same order (the same offer order, the same sort of split views' lists); the gradients
-// differ only by the order of their atomics.  Three further removals of global loads can be compiled in; they are left out
-// by default because on an H100 each made the kernel slower (DESIGN §6):
-#ifndef DBW_BL_STAGE_UV
-#define DBW_BL_STAGE_UV 0           // 1: the listed faces' UV records (32 B) staged by TMA with their face records
-#endif
-#ifndef DBW_BL_EDGE_SMEM
-#define DBW_BL_EDGE_SMEM 0          // 1: on the fast path a fragment carries its list index in the map field, and the suffix
-#endif                              //    pass reads the edge from the staged face record (needs DBW_BL_STAGE_UV for the map id)
-#ifndef DBW_BL_BOX_SMEM
-#define DBW_BL_BOX_SMEM 1           // 0: the pixel-level box reject recomputed from the staged vertices (no s_bbox)
-#endif
-#define BL_NT 128
-static_assert(!DBW_BL_EDGE_SMEM || DBW_BL_STAGE_UV, "the list index replaces the map id only when the UV records are staged");
-
-// bilinear colour of a fragment on a cell map (the cell-map branch of fetch_color)
-__device__ __forceinline__ void fetch_cell_color(const RasterParams& P, float u, float v, int4 d, Texel4& s) {
-  s.tap = map_tap(u, v, d);
-  s.c00 = ld_texel(P.maps4, s.tap.i00);
-  s.c01 = s.tap.i01 == s.tap.i00 ? s.c00 : ld_texel(P.maps4, s.tap.i01);
-  s.c10 = s.tap.i10 == s.tap.i00 ? s.c00 : ld_texel(P.maps4, s.tap.i10);
-  s.c11 = s.tap.i11 == s.tap.i01 ? s.c01 : (s.tap.i11 == s.tap.i10 ? s.c10 : ld_texel(P.maps4, s.tap.i11));
-  s.color.x = s.c00.x * s.tap.w00 + s.c01.x * s.tap.w01 + s.c10.x * s.tap.w10 + s.c11.x * s.tap.w11;
-  s.color.y = s.c00.y * s.tap.w00 + s.c01.y * s.tap.w01 + s.c10.y * s.tap.w10 + s.c11.y * s.tap.w11;
-  s.color.z = s.c00.z * s.tap.w00 + s.c01.z * s.tap.w01 + s.c10.z * s.tap.w10 + s.c11.z * s.tap.w11;
-}
-
-// What the blocks loss kernel's per-pixel loops read from shared memory.  `listed` (DBW_BL_EDGE_SMEM, fast path): a
-// fragment's map field holds its index in the tile list (rec, uv) instead of its map id.
-struct BlocksSmem {
-  const float4* rec; const float4* uv; const float* alpha; float* galpha; const int4* desc;
-  size_t slot_base; bool listed;
-};
-__device__ __forceinline__ int4 bl_desc(const BlocksSmem& S, int bits) {
-  const int m = (int)((unsigned)bits >> DBW_FRAG_MAP_SHIFT);
-  if (DBW_BL_EDGE_SMEM && S.listed) return S.desc[__float_as_int(S.uv[m * 2 + 1].z)];
-  return S.desc[m];
-}
-
-// suffix_backward for the blocks loss kernel: the opacity sums always in shared memory (keyed by the entry within the view)
-__device__ __forceinline__ void blocks_suffix_backward(const RasterParams& P, const BlocksSmem& S, const float4* s_q,
-                                                       const int* s_bits, int n, int n_warp, f2 p, float gr, float gg,
-                                                       float gb, float ga, bool want_alpha, bool want_dist, int lane) {
-  if (!want_alpha && !want_dist) return;
-  float Tacc = P.bg0 * gr + P.bg1 * gg + P.bg2 * gb - ga;
-  struct EdgeGeom { float4 r0; float2 r1; float4 r3; };
-  auto load_edge = [&](int kk, EdgeGeom& g) {
-    g.r0 = make_float4(0.f, 0.f, 0.f, 0.f); g.r1 = make_float2(0.f, 0.f); g.r3 = g.r0;
-    if (!want_dist || kk < 0 || kk >= n) return;
-    const int bits = s_bits[kk * BL_NT];
-    if (P.clip_inside && !(bits & DBW_FRAG_OUTSIDE_BIT)) return;          // clamp(d, 0): no distance gradient inside the face
-    if (DBW_BL_EDGE_SMEM && S.listed) {
-      const int j = (int)((unsigned)bits >> DBW_FRAG_MAP_SHIFT);
-      g.r0 = S.rec[j * 4]; g.r3 = S.rec[j * 4 + 3];
-      g.r1 = *reinterpret_cast<const float2*>(&S.rec[j * 4 + 1]);
-      return;
-    }
-    const size_t gsl = S.slot_base + (bits & DBW_FRAG_SLOT_MASK);
-    g.r0 = __ldg(&P.rec[gsl * 4]); g.r3 = __ldg(&P.rec[gsl * 4 + 3]);
-    g.r1 = __ldg(reinterpret_cast<const float2*>(&P.rec[gsl * 4 + 1]));
-  };
-  EdgeGeom eg_next;
-  load_edge(n_warp - 1, eg_next);
-  for (int k = n_warp - 1; k >= 0; --k) {
-    const EdgeGeom eg = eg_next;
-    load_edge(k - 1, eg_next);
-    int akey = -1, vkey = -1;
-    float aval = 0.f;
-    float gv4[4] = {0.f, 0.f, 0.f, 0.f};
-    if (k < n) {
-      const float4 q = s_q[k * BL_NT];        // (alpha, cdot, e, occ)
-      const float g_alpha = q.w * (q.y - Tacc);
-      Tacc = q.x * q.y + (1.f - q.x) * Tacc;
-      if (g_alpha != 0.f) {
-        const int bits = s_bits[k * BL_NT], slot = bits & DBW_FRAG_SLOT_MASK;
-        const int face = slot >= P.F ? slot - P.F : slot;
-        if (want_alpha) { akey = alpha_index(P, 0, face); aval = g_alpha * q.z; }
-        if (want_dist) {
-          const bool inside = !(bits & DBW_FRAG_OUTSIDE_BIT);
-          float g_sd = 0.f;
-          if (P.clip_inside) { if (!inside) g_sd = g_alpha * (-q.x / P.sigma); }
-          else g_sd = g_alpha * (-q.x * (1.f - q.z) / P.sigma);
-          const float g_dist = inside ? -g_sd : g_sd;
-          if (g_dist != 0.f) {
-            const int edge = (bits >> DBW_FRAG_EDGE_SHIFT) & 3;
-            const f2 v0 = {eg.r0.x, eg.r0.y}, v1 = {eg.r0.z, eg.r0.w}, v2 = {eg.r1.x, eg.r1.y};
-            const f2 ea = edge == 2 ? v1 : v0, eb = edge == 0 ? v1 : v2;
-            const float il = edge == 0 ? eg.r3.y : (edge == 1 ? eg.r3.z : eg.r3.w);
-            f2 g_a = {0.f, 0.f}, g_b = {0.f, 0.f};
-            seg_backward(p, ea, eb, il, g_dist, g_a, g_b);
-            vkey = slot * 4 + edge;
-            gv4[0] = g_a.x; gv4[1] = g_a.y; gv4[2] = g_b.x; gv4[3] = g_b.y;
-          }
-        }
-      }
-    }
-    if (want_alpha && __ballot_sync(0xffffffffu, akey >= 0)) warp_agg_add1(S.galpha, akey, aval, lane);
-    if (want_dist && __ballot_sync(0xffffffffu, vkey >= 0)) warp_agg_add_edge(P.g_tri + S.slot_base * 9, vkey, gv4, lane);
-  }
-}
-
-// epilogue_backward for the blocks loss kernel (cell taps, opacities from the staged table)
-__device__ __forceinline__ void blocks_epilogue_backward(const RasterParams& P, const BlocksSmem& S, float4* lA, float* lV,
-                                                         bool live, int n, f2 p, const float (&g)[4], int lane, int warp) {
-  const float gr = g[0], gg = g[1], gb = g[2], ga = g[3];
-  const bool any_grad = live && ((gr != 0.f) || (gg != 0.f) || (gb != 0.f) || (ga != 0.f));
-  const int n_px = any_grad ? n : 0;
-  int n_warp = n_px;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) n_warp = max(n_warp, __shfl_xor_sync(0xffffffffu, n_warp, o));
-  float occ = 1.f;
-  for (int k = 0; k < n_warp; ++k) {
-    int tkey = -1, t01 = -1, t10 = -1, t11 = -1;
-    bool tcells = false;
-    float tg[3] = {0.f, 0.f, 0.f}, tw[4] = {0.f, 0.f, 0.f, 0.f};
-    if (k < n_px) {
-      const float4 e = lA[k * BL_NT];
-      const int bits = __float_as_int(e.y), slot = bits & DBW_FRAG_SLOT_MASK;
-      const int face = slot >= P.F ? slot - P.F : slot;
-      const int4 desc = bl_desc(S, bits);
-      Texel4 tx;
-      fetch_cell_color(P, e.w, lV[k * BL_NT], desc, tx);
-      const float ea = frag_alpha(e.z, P.sigma, P.clip_inside);
-      const float a = P.faces_alpha ? ea * S.alpha[alpha_index(P, 0, face)] : ea;
-      const float cdot = tx.color.x * gr + tx.color.y * gg + tx.color.z * gb;
-      lA[k * BL_NT] = make_float4(a, cdot, ea, occ);
-      lV[k * BL_NT] = __int_as_float(bits);
-      const float w = occ * a;
-      if (w != 0.f && P.g_maps4) {
-        tkey = tx.tap.i00; t01 = tx.tap.i01; t10 = tx.tap.i10; t11 = tx.tap.i11; tcells = desc.w != 0;
-        tg[0] = w * gr; tg[1] = w * gg; tg[2] = w * gb;
-        tw[0] = tx.tap.w00; tw[1] = tx.tap.w01; tw[2] = tx.tap.w10; tw[3] = tx.tap.w11;
-      }
-      occ *= (1.f - a);
-    }
-    if (P.g_maps4) warp_tex_scatter<false>(P, tkey, t01, t10, t11, tcells, tg, tw, lane, warp);
-  }
-  const bool want_alpha = P.faces_alpha != nullptr && P.g_faces_alpha != nullptr;
-  blocks_suffix_backward(P, S, lA, reinterpret_cast<const int*>(lV), n_px, n_warp, p, gr, gg, gb, ga, want_alpha,
-                         P.sigma > 0.f && P.g_tri != nullptr, lane);
-}
-
-// Dynamic shared memory: the fragment lists (K x BL_NT float4, K x BL_NT float), the map table (M int4), then with
-// faces_alpha the opacity sums and the opacity table (n_alpha floats each).
-__global__ void __launch_bounds__(BL_NT, DBW_FWD_MINB) blocks_loss_kernel(const RasterParams P) {
-  constexpr int NT = BL_NT, CAP = DBW_LIST_CAP, TILE_H = NT / 16;
-  __shared__ float4 s_rec[CAP * 4];
-  __shared__ float4 s_uv[DBW_BL_STAGE_UV ? CAP * 2 : 1];     // rec2 of the listed faces: (u0 v0 u1 v1) (u2 v2 map -)
-  __shared__ float4 s_bbox[DBW_BL_BOX_SMEM ? CAP : 1];
-  __shared__ int s_slot[CAP];
-  __shared__ int s_count;
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ float s_ndc[DBW_BL_BOX_SMEM ? TILE_W + TILE_H : 4];   // the tile's pixel NDC coordinates, or only its bounds
-  extern __shared__ float4 s_dyn[];
-  uint32_t bar_phase = 0;
-
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int view = blockIdx.x;
-  const int tile_y = centre_out(blockIdx.z, gridDim.z);
-  const int tx0 = blockIdx.y * TILE_W, ty0 = tile_y * TILE_H;
-  const int xi = tx0 + (warp & 1) * 8 + (lane & 7);
-  const int yi = ty0 + (warp >> 1) * 4 + (lane >> 3);
-  int row_lo = 0, row_hi = P.H;
-  if (P.view_rows) { row_lo = P.view_rows[view * 2]; row_hi = P.view_rows[view * 2 + 1]; }
-  if (ty0 >= row_hi || ty0 + TILE_H <= row_lo) return;
-  const bool live = xi < P.W && yi < P.H && yi >= row_lo && yi < row_hi;
-  const int tx1 = min(tx0 + TILE_W, P.W) - 1, ty1 = min(ty0 + TILE_H, P.H) - 1;
-#if DBW_BL_BOX_SMEM
-  if (tid < TILE_W) s_ndc[tid] = pix_to_ndc(P.W - 1 - min(tx0 + tid, P.W - 1), P.W, P.H);
-  else if (tid < TILE_W + TILE_H) s_ndc[tid] = pix_to_ndc(P.H - 1 - min(ty0 + tid - TILE_W, P.H - 1), P.H, P.W);
-#else
-  if (tid == 0) s_ndc[0] = pix_to_ndc(P.W - 1 - tx1, P.W, P.H);
-  else if (tid == 1) s_ndc[1] = pix_to_ndc(P.W - 1 - min(tx0, P.W - 1), P.W, P.H);
-  else if (tid == 2) s_ndc[2] = pix_to_ndc(P.H - 1 - ty1, P.H, P.W);
-  else if (tid == 3) s_ndc[3] = pix_to_ndc(P.H - 1 - min(ty0, P.H - 1), P.H, P.W);
-#endif
-  if (tid == 0) { s_count = 0; mbar_init(&s_bar, 1); }
-  const int K = P.K;
-  int4* const s_desc = reinterpret_cast<int4*>(reinterpret_cast<float*>(s_dyn + (size_t)K * NT) + (size_t)K * NT);
-  float* const s_galpha = reinterpret_cast<float*>(s_desc + P.M);
-  float* const s_alpha = s_galpha + P.n_alpha;
-  const bool has_alpha = P.faces_alpha != nullptr;
-  if (has_alpha && P.g_faces_alpha) for (int i = tid; i < P.n_alpha; i += NT) s_galpha[i] = 0.f;
-  DbwMapDesc my_desc = {0, 0, 0, 0};
-  if (tid < P.M) my_desc = P.map_table[tid];
-  float my_alpha = 0.f;          // this thread's opacity entry, stored with its map-table entry after the bin scan
-  if (has_alpha && tid < P.n_alpha) my_alpha = __ldg(&P.faces_alpha[(size_t)view * P.alpha_stride + tid]);
-  const int4 vbox = __ldg(reinterpret_cast<const int4*>(P.view_bbox) + view);
-  const int vflags = __ldg(P.view_flags + view);
-#if !DBW_BL_BOX_SMEM
-  // this pixel's NDC coordinates: the same exact evaluation the generic kernel shares through shared memory
-  const f2 p = {pix_to_ndc(P.W - 1 - min(xi, P.W - 1), P.W, P.H), pix_to_ndc(P.H - 1 - min(yi, P.H - 1), P.H, P.W)};
-#endif
-  __syncthreads();
-#if DBW_BL_BOX_SMEM
-  const f2 p = {s_ndc[xi - tx0], s_ndc[TILE_W + yi - ty0]};
-  const float t_xmin = s_ndc[tx1 - tx0], t_xmax = s_ndc[0], t_ymin = s_ndc[TILE_W + ty1 - ty0], t_ymax = s_ndc[TILE_W];
-#else
-  const float t_xmin = s_ndc[0], t_xmax = s_ndc[1], t_ymin = s_ndc[2], t_ymax = s_ndc[3];
-#endif
-  const bool tile_empty = ord2f(vbox.x) > t_xmax || ord2f(vbox.y) < t_xmin || ord2f(vbox.z) > t_ymax || ord2f(vbox.w) < t_ymin;
-
-  float4* const lA = s_dyn + tid;
-  float* const lV = reinterpret_cast<float*>(s_dyn + (size_t)K * NT) + tid;
-  int n = 0;
-
-  const int* clist = nullptr;
-  int nslots = tile_empty ? 0 : ((vflags & 1) ? 2 * P.F : P.F);
-  if (P.cbin_list && !tile_empty) {
-    const size_t b = (size_t)view * P.cbin_nx * P.cbin_ny + (size_t)(ty0 / DBW_CBIN) * P.cbin_nx + tx0 / DBW_CBIN;
-    clist = P.cbin_list + b * 2 * P.F;
-    nslots = __ldg(P.cbin_count + b);
-  }
-  const size_t slot_base = (size_t)view * 2 * P.F;
-  const float4* bbox = P.bbox + slot_base;
-  const float4* rec = P.rec + slot_base * 4;
-  const float4* rec2 = P.rec2 + slot_base * 2;
-  const bool dist_inside = !P.clip_inside && P.sigma > 0.f;
-  const float sqrt_blur = P.sqrt_blur;
-  bool listed = false;           // fast path with DBW_BL_EDGE_SMEM: fragments carry their list index
-
-  auto raster_list = [&](int cnt) {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (tid == 0) mbar_arrive_expect_tx(&s_bar, (uint32_t)cnt * (DBW_BL_STAGE_UV ? 96u : 64u));
-    for (int j = tid; j < cnt; j += NT) {
-      const size_t s = (size_t)s_slot[j];
-      bulk_copy_g2s(&s_rec[j * 4], &rec[s * 4], 64u, &s_bar);
-      if (DBW_BL_STAGE_UV) bulk_copy_g2s(&s_uv[j * 2], &rec2[s * 2], 32u, &s_bar);
-    }
-    mbar_wait(&s_bar, bar_phase);
-    bar_phase ^= 1u;
-    if (live) {
-      for (int j = 0; j < cnt; ++j) {
-#if DBW_BL_BOX_SMEM
-        const float4 b4 = s_bbox[j];
-        if (p.x > b4.y || p.x < b4.x || p.y > b4.w || p.y < b4.z) continue;
-        const float4 r0 = s_rec[j * 4], r1 = s_rec[j * 4 + 1];
-#else
-        const float4 r0 = s_rec[j * 4], r1 = s_rec[j * 4 + 1];
-        // the slot's box (face_setup_kernel: listed slots are valid), from its vertices
-        if (p.x > fmaxf(fmaxf(r0.x, r0.z), r1.x) + sqrt_blur || p.x < fminf(fminf(r0.x, r0.z), r1.x) - sqrt_blur ||
-            p.y > fmaxf(fmaxf(r0.y, r0.w), r1.y) + sqrt_blur || p.y < fminf(fminf(r0.y, r0.w), r1.y) - sqrt_blur) continue;
-#endif
-        const TriGeom t = unpack_tri(r0, r1, s_rec[j * 4 + 2], s_rec[j * 4 + 3]);
-        const Edges ed = eval_edges(p, t);
-        if (!ed.inside && P.blur == 0.f) continue;
-        float dist = 1.f; int edge = 0;
-        const bool need_dist = !ed.inside || dist_inside || t.neighbor >= 0;
-        if (need_dist) dist = tri_dist2_edge(p, t, edge);
-        if (!ed.inside && dist >= P.blur) continue;
-        const Bary b = bary_from_edges(ed, t, P.persp, P.clipb);
-        if (b.pz < 0.f) continue;
-        const int slot = s_slot[j];
-        if (n == K && t.neighbor < 0 && !frag_key_less(__float_as_uint(b.pz + 0.f), slot, lA[(K - 1) * NT])) continue;
-        f3 bu = b.bc;
-        if (t.flags & 1) {
-          const float* cv = P.conv + (slot_base + slot) * 9;
-          bu.x = b.bc.x * cv[0] + b.bc.y * cv[3] + b.bc.z * cv[6];
-          bu.y = b.bc.x * cv[1] + b.bc.y * cv[4] + b.bc.z * cv[7];
-          bu.z = b.bc.x * cv[2] + b.bc.y * cv[5] + b.bc.z * cv[8];
-        }
-#if DBW_BL_STAGE_UV
-        const float4 q0 = s_uv[j * 2], q1 = s_uv[j * 2 + 1];
-#else
-        const float4 q0 = __ldg(&rec2[(size_t)slot * 2]), q1 = __ldg(&rec2[(size_t)slot * 2 + 1]);
-#endif
-        const float u = bu.x * q0.x + bu.y * q0.z + bu.z * q1.x;
-        const float v = bu.x * q0.y + bu.y * q0.w + bu.z * q1.y;
-        n = fraglist_offer(lA, lV, NT, n, K, b.pz, slot, edge, b.inside ? -dist : dist, dist, t.neighbor, u, v,
-                           listed ? j : __float_as_int(q1.z));
-      }
-    }
-  };
-
-  const float rx0 = t_xmin - sqrt_blur, rx1 = t_xmax + sqrt_blur, ry0 = t_ymin - sqrt_blur, ry1 = t_ymax + sqrt_blur;
-  const bool split = vflags & 1;
-  auto scan_hit = [&](int& s, float4& bb) -> bool {
-    if (s >= nslots) return false;
-    if (clist) s = __ldg(clist + s);
-    else if (split) s = frag_order_slot(s, P.F);
-    bb = __ldg(&bbox[s]);
-    if (bb.x > t_xmax || bb.y < t_xmin || bb.z > t_ymax || bb.w < t_ymin) return false;
-    const float4 r0 = __ldg(&rec[(size_t)s * 4]);
-    const float2 r1 = __ldg(reinterpret_cast<const float2*>(&rec[(size_t)s * 4 + 1]));
-    return tri_overlaps_rect({r0.x, r0.y}, {r0.z, r0.w}, {r1.x, r1.y}, rx0, rx1, ry0, ry1);
-  };
-  for (int base = 0; base < nslots; base += 4 * NT) {
-    float4 bb[4]; int sid[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int i = base + q * NT + tid;
-      sid[q] = i < nslots ? (clist ? __ldg(clist + i) : i) : -1;
-    }
-#pragma unroll
-    for (int q = 0; q < 4; ++q) bb[q] = sid[q] >= 0 ? __ldg(&bbox[sid[q]]) : make_float4(INFINITY, -INFINITY, INFINITY, -INFINITY);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int sl = sid[q];
-      bool hit = !(bb[q].x > t_xmax || bb[q].y < t_xmin || bb[q].z > t_ymax || bb[q].w < t_ymin);
-      if (hit) {
-        const float4 r0 = __ldg(&rec[(size_t)sl * 4]);
-        const float2 r1 = __ldg(reinterpret_cast<const float2*>(&rec[(size_t)sl * 4 + 1]));
-        hit = tri_overlaps_rect({r0.x, r0.y}, {r0.z, r0.w}, {r1.x, r1.y}, rx0, rx1, ry0, ry1);
-      }
-      const unsigned m = __ballot_sync(0xffffffffu, hit);
-      if (m == 0u) continue;
-      int wbase = 0;
-      if (lane == 0) wbase = atomicAdd(&s_count, __popc(m));
-      wbase = __shfl_sync(0xffffffffu, wbase, 0);
-      const int pos = wbase + __popc(m & ((1u << lane) - 1u));
-      if (hit && pos < CAP) { s_slot[pos] = sl; if (DBW_BL_BOX_SMEM) s_bbox[pos] = bb[q]; }
-    }
-  }
-  if (tid < P.M) s_desc[tid] = make_int4(my_desc.offset / 3, my_desc.height, my_desc.width, my_desc.reserved);
-  for (int m = tid + NT; m < P.M; m += NT) { const DbwMapDesc d = P.map_table[m]; s_desc[m] = make_int4(d.offset / 3, d.height, d.width, d.reserved); }
-  if (has_alpha) {
-    if (tid < P.n_alpha) s_alpha[tid] = my_alpha;
-    for (int i = tid + NT; i < P.n_alpha; i += NT) s_alpha[i] = __ldg(&P.faces_alpha[(size_t)view * P.alpha_stride + i]);
-  }
-  __syncthreads();
-  const int total = s_count;
-  if (total <= CAP) {
-    listed = DBW_BL_EDGE_SMEM != 0;
-    if (split && total > 1) {           // the generic kernel's sort of the tile list into frag_order_key order
-      constexpr int PER = (CAP + NT - 1) / NT;
-      int sl[PER], rk[PER]; float4 bx[PER];
-#pragma unroll
-      for (int r = 0; r < PER; ++r) {
-        const int j = tid + r * NT;
-        if (j < total) { sl[r] = s_slot[j]; if (DBW_BL_BOX_SMEM) bx[r] = s_bbox[j]; rk[r] = frag_order_rank(s_slot, total, j, P.F); }
-      }
-      __syncthreads();
-#pragma unroll
-      for (int r = 0; r < PER; ++r)
-        if (tid + r * NT < total) { s_slot[rk[r]] = sl[r]; if (DBW_BL_BOX_SMEM) s_bbox[rk[r]] = bx[r]; }
-      __syncthreads();
-    }
-    if (total > 0) raster_list(total);
-  } else {
-    __shared__ int s_wcount[NT / 32];
-    constexpr int BS = NT < CAP ? NT : CAP;
-    int cnt = 0;
-    for (int base = 0; base < nslots; base += BS) {
-      float4 bb = make_float4(0, 0, 0, 0);
-      int sl = base + tid;
-      const bool hit = tid < BS && scan_hit(sl, bb);
-      const unsigned m = __ballot_sync(0xffffffffu, hit);
-      if (lane == 0) s_wcount[warp] = __popc(m);
-      __syncthreads();
-      int pos = cnt;
-#pragma unroll
-      for (int w = 0; w < NT / 32; ++w) { const int c = s_wcount[w]; pos += w < warp ? c : 0; cnt += c; }
-      if (hit) {
-        pos += __popc(m & ((1u << lane) - 1u));
-        s_slot[pos] = sl;
-        if (DBW_BL_BOX_SMEM) s_bbox[pos] = bb;
-      }
-      __syncthreads();
-      const bool last = base + BS >= nslots;
-      if (cnt > CAP - BS || last) {
-        raster_list(cnt);
-        __syncthreads();
-        cnt = 0;
-      }
-    }
-  }
-
-  const BlocksSmem S = {s_rec, s_uv, s_alpha, s_galpha, s_desc, slot_base, listed};
-  float ep_sq = 0.f;
-  float ep_g[4] = {0.f, 0.f, 0.f, 0.f};
-  int n_saved = 0;
-  if (live) {
-    float occ = 1.f, r = 0.f, g = 0.f, bl = 0.f;
-    const size_t plane = (size_t)P.H * P.W;
-    const size_t pix = (size_t)yi * P.W + xi;
-    float ep_e[3], ep_t[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      ep_e[c] = __ldg(P.ep_env + (size_t)view * 4 * plane + (size_t)c * plane + pix);
-      ep_t[c] = __ldg(P.ep_target + (size_t)view * 3 * plane + (size_t)c * plane + pix);
-    }
-#pragma unroll 1
-    for (int k = 0; k < n; ++k) {
-      if (occ == 0.f) break;      // behind a fully opaque fragment: every later layer contributes exactly 0
-      const float4 e = lA[k * NT];
-      const int bits = __float_as_int(e.y), slot = bits & DBW_FRAG_SLOT_MASK;
-      n_saved = k + 1;
-      const float v = lV[k * NT];
-      const int face = slot >= P.F ? slot - P.F : slot;
-      Texel4 tx;
-      fetch_cell_color(P, e.w, v, bl_desc(S, bits), tx);
-      float a = frag_alpha(e.z, P.sigma, P.clip_inside);
-      if (has_alpha) a *= s_alpha[alpha_index(P, 0, face)];
-      const float w = occ * a;
-      r += w * tx.color.x; g += w * tx.color.y; bl += w * tx.color.z;
-      occ *= (1.f - a);
-    }
-    const float fc[3] = {r + occ * P.bg0, g + occ * P.bg1, bl + occ * P.bg2};
-    const float m = 1.f - occ;
-    float* ge = P.ep_g_env + (size_t)view * 4 * plane + pix;
-    float gm = 0.f;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const float ec = ep_e[c];
-      const float rc = fc[c] * m + (1.f - m) * ec;
-      const float diff = rc - ep_t[c];
-      ep_sq += diff * diff;
-      if (P.ep_rec) P.ep_rec[(size_t)view * 3 * plane + (size_t)c * plane + pix] = rc;
-      const float gr = 2.f * diff * P.ep_inv_count;
-      ep_g[c] = gr * m;
-      ge[(size_t)c * plane] = gr * (1.f - m);
-      gm += gr * (fc[c] - ec);
-    }
-    ep_g[3] = gm;
-    if (!P.ep_skip_env_alpha) ge[3 * plane] = 0.f;
-  }
-  blocks_epilogue_backward(P, S, lA, lV, live, n_saved, p, ep_g, lane, warp);
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) ep_sq += __shfl_xor_sync(0xffffffffu, ep_sq, off);
-  if (lane == 0 && ep_sq != 0.f) {
-    const unsigned cta = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    atomicAdd(&P.ep_partials[(cta * (NT / 32) + warp) & P.ep_part_mask], ep_sq * P.ep_inv_count);
-  }
-  if (has_alpha && P.g_faces_alpha) {
-    __syncthreads();
-    for (int i = tid; i < P.n_alpha; i += NT) {
-      const float v = s_galpha[i];
-      if (v != 0.f) atomicAdd(&P.g_faces_alpha[(size_t)view * P.alpha_stride + i], v);
-    }
-  }
+                  want_alpha, BLOCKS || (want_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX), s_galpha, P.sigma > 0.f && P.g_tri != nullptr, lane);
 }
 
 // One thread per pixel.  Pass 1 streams the pixel's saved fragment records {slot, u, v, signed distance} front to back,
@@ -2508,33 +2097,27 @@ static size_t bary_flag_count(const DbwRenderSettings& s) {
   return (size_t)g.x * g.y * g.z;
 }
 
-// dynamic shared memory of the raster kernels: K list entries (forward) / K saved scalars (backward) of 20 B per thread
-static size_t frag_smem_bytes(int K, int NT, int M, int n_alpha = 0) {
-  return (size_t)K * NT * (sizeof(float4) + sizeof(float)) + (size_t)M * sizeof(int4) + (n_alpha <= 512 ? (size_t)n_alpha * sizeof(float) : 0);
+// dynamic shared memory of the raster kernels: K list entries (forward) / K saved scalars (backward) of 20 B per thread, the
+// map table, and `alpha_tables` arrays of n_alpha floats (the opacity sums, then the opacity table) when they fit
+static size_t frag_smem_bytes(int K, int NT, int M, int n_alpha = 0, int alpha_tables = 1) {
+  return (size_t)K * NT * (sizeof(float4) + sizeof(float)) + (size_t)M * sizeof(int4) +
+         (n_alpha <= DBW_ALPHA_SMEM_MAX ? (size_t)alpha_tables * n_alpha * sizeof(float) : 0);
 }
 
-template <int NT>
+// BLOCKS: blocks_loss_kernel, whose dispatch guarantees ep_grad and n_alpha <= DBW_ALPHA_SMEM_MAX
+template <int NT, bool BLOCKS = false>
 static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st) {
+  static_assert(!BLOCKS || NT == 128, "blocks_loss_kernel runs 128 threads");
   const dim3 grid(P.B, (P.W + TILE_W - 1) / TILE_W, (P.H + NT / 16 - 1) / (NT / 16));       // see centre_out()
-  const size_t smem = frag_smem_bytes(P.K, NT, P.M, P.ep_grad && P.faces_alpha && P.g_faces_alpha ? P.n_alpha : 0);
+  const size_t smem = BLOCKS ? frag_smem_bytes(P.K, NT, P.M, P.faces_alpha ? P.n_alpha : 0, 2)
+                             : frag_smem_bytes(P.K, NT, P.M, P.ep_grad && P.faces_alpha && P.g_faces_alpha ? P.n_alpha : 0);
   auto go = [&](auto kern) -> cudaError_t {
     if (smem > 40 * 1024) { cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); if (e != cudaSuccess) return e; }
     kern<<<grid, NT, smem, st>>>(P);
     return cudaSuccess;
   };
+  if (BLOCKS) return go(blocks_loss_kernel);
   return P.ep_target ? go(raster_forward_kernel<NT, true>) : go(raster_forward_kernel<NT, false>);
-}
-
-static cudaError_t launch_blocks_loss(const RasterParams& P, cudaStream_t st) {
-  const dim3 grid(P.B, (P.W + TILE_W - 1) / TILE_W, (P.H + BL_NT / 16 - 1) / (BL_NT / 16));       // see centre_out()
-  const size_t smem = (size_t)P.K * BL_NT * (sizeof(float4) + sizeof(float)) + (size_t)P.M * sizeof(int4) +
-                      (P.faces_alpha ? 2 * (size_t)P.n_alpha * sizeof(float) : 0);
-  if (smem > 40 * 1024) {
-    const cudaError_t e = cudaFuncSetAttribute(blocks_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-  }
-  blocks_loss_kernel<<<grid, BL_NT, smem, st>>>(P);
-  return cudaSuccess;
 }
 
 // the backward scratch and the gradients a loss-epilogue forward computes itself (dbw_render_forward_loss_grad)
@@ -2673,7 +2256,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
       cudaError_t e;
       if (blocks_loss) {
         ScopedTimer bl_timer(2, K, st);
-        e = launch_blocks_loss(P, st);
+        e = launch_forward<128, true>(P, st);
       } else {
         e = K <= 4 ? launch_forward<DBW_FWD_NT_SMALLK>(P, st) : launch_forward<DBW_FWD_NT>(P, st);
       }

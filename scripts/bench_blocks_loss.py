@@ -6,27 +6,18 @@ kernels alternate, `--repeat` runs of `--steps` eager training steps each; per s
     graph-replayed step of each build.)
 Prints one JSON line per workload with the card's name and power limit, the medians and the min..max spread.
 
---ablate also builds the library once per global-load removal that blocks_loss_kernel leaves out by default (DESIGN §6:
-they made it slower), into a temporary directory, and runs the same comparison with each:
-  DBW_BL_STAGE_UV=1                      UV records staged with the face records
-  DBW_BL_STAGE_UV=1 DBW_BL_EDGE_SMEM=1   ... and the suffix pass's edges read from the staged face records
-  DBW_BL_BOX_SMEM=0                      the box reject recomputed from the staged vertices (no s_bbox)
-
-  python scripts/bench_blocks_loss.py [--workload dtu bmvs] [--repeat N] [--steps S] [--ablate]"""
+  python scripts/bench_blocks_loss.py [--workload dtu bmvs] [--repeat N] [--steps S]"""
 import argparse
 import json
 import os
 import statistics
 import subprocess
 import sys
-import tempfile
-from concurrent.futures import ThreadPoolExecutor
 from copy import deepcopy
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.join(HERE, '..')
 sys.path.insert(0, ROOT)
-ABLATIONS = (('DBW_BL_STAGE_UV=1',), ('DBW_BL_STAGE_UV=1', 'DBW_BL_EDGE_SMEM=1'), ('DBW_BL_BOX_SMEM=0',))
 
 
 def card():
@@ -100,40 +91,15 @@ def measure(workload, repeat, steps):
     return out
 
 
-def build_variant(flags, outdir):
-    """the library with the macro definitions `flags` (nvcc, the Makefile's flags), into outdir"""
-    csrc = os.path.join(ROOT, 'differentiable-blocksworld_b200', 'csrc')
-    so = os.path.join(outdir, 'libdbw_render_' + '_'.join(f.lower().replace('=', '') for f in flags) + '.so')
-    nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-    srcs = ['dbw_render.cu', 'dbw_scene.cu', 'dbw_comm.cu', 'dbw_eval.cu', 'dbw_knn.cu', 'dbw_lpips.cu', 'dbw_optim.cu']
-    subprocess.check_call([nvcc, '-O3', '-std=c++17', '-lineinfo', '-prec-div=false', '-gencode', 'arch=compute_90a,code=sm_90a',
-                           '-Xcompiler', '-fPIC', '-shared', *[f'-D{f}' for f in flags], *srcs, '-o', so], cwd=csrc)
-    return so
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--workload', nargs='+', default=['dtu', 'bmvs'], choices=['dtu', 'bmvs'])
     ap.add_argument('--repeat', type=int, default=3)
     ap.add_argument('--steps', type=int, default=20)
-    ap.add_argument('--ablate', action='store_true')
-    ap.add_argument('--variant', default='default', help=argparse.SUPPRESS)
     args = ap.parse_args()
-    if args.ablate:
-        with tempfile.TemporaryDirectory() as tmp:
-            with ThreadPoolExecutor(len(ABLATIONS)) as ex:
-                libs = list(ex.map(lambda f: build_variant(f, tmp), ABLATIONS))
-            for flags, so in [(None, None)] + list(zip(ABLATIONS, libs)):
-                env = dict(os.environ)
-                if so:
-                    env['DBW_RENDER_LIB'] = so
-                cmd = [sys.executable, os.path.abspath(__file__), '--repeat', str(args.repeat), '--steps', str(args.steps),
-                       '--variant', ' '.join(flags) if flags else 'default', '--workload', *args.workload]
-                subprocess.check_call(cmd, env=env)
-        return
     c = card()
     for wl in args.workload:
-        line = {'workload': wl, 'variant': args.variant, 'card': c, 'repeat': args.repeat, 'steps_per_run': args.steps}
+        line = {'workload': wl, 'card': c, 'repeat': args.repeat, 'steps_per_run': args.steps}
         line.update(measure(wl, args.repeat, args.steps))
         print(json.dumps(line), flush=True)
 

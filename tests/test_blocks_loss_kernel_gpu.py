@@ -1,5 +1,5 @@
-"""GPU: the coarse phase's blocks loss pass in its own kernel (blocks_loss_kernel) against the generic
-raster_forward_kernel<128, true> it replaces (dbw_debug_generic_blocks_loss(1)), on the same inputs.  The loss and the
+"""GPU: the coarse phase's blocks loss pass in its own kernel (blocks_loss_kernel, the BLOCKS instantiation of the forward
+body) against the generic raster_forward_kernel<128, true> (dbw_debug_generic_blocks_loss(1)), on the same inputs.  The loss and the
 environment's gradient image are bit-identical; the leaf gradients agree to the rounding of the atomics' order (1e-6 of
 each array's largest magnitude, or 4x the spread of two generic runs).  The generic kernel itself is pinned to the
 two-kernel path by test_fused_blocks_grad_gpu.py and to the float64 oracle by test_epilogue_matrix_gpu.py."""
