@@ -49,35 +49,45 @@ Dims dims_of(int64_t B, int H, int W) {
 int64_t align64(int64_t n) { return (n + 63) & ~int64_t(63); }        // floats: 256-byte aligned regions
 int64_t head_chunks(int H, int W) { return ((int64_t)H * W + HEAD_PIX - 1) / HEAD_PIX; }
 
-// workspace layout, in floats: rec activations of the 13 layers (only its 5 taps when no backward follows), the 5 taps of
-// imgs, two scratch tensors of B*H*W*64 (pool outputs and the intermediates not kept in the forward, the running gradient
-// in the backward), the head partials, the seed the forward used (the contract is stated in include/dbw_render.h)
+// levels: bit k requests level k (relu1_2 .. relu5_3); LPIPS requests all five
+constexpr int ALL_LEVELS = 31;
+bool wants(int levels, int k) { return (levels >> k) & 1; }
+int deepest(int levels) { int L = 0; for (int k = 0; k < 5; ++k) if (wants(levels, k)) L = k; return L; }   // 0-based
+
+// workspace layout, in floats (the contract is stated in include/dbw_render.h): rec's activations through the deepest
+// requested level (only its requested taps when no backward follows), imgs' requested taps, two scratch tensors of
+// B*H*W*64 (pool outputs and the intermediates not kept in the forward, the running gradient in the backward), the head
+// partials of the requested levels, then a region of `tail_floats`: LPIPS's seed the forward used and the target cache's
+// miss count, or the VGG term's constants
 struct Layout {
-  int64_t act[LP_LAYERS], tap0[5], s0, s1, partials, seed, total;
+  int64_t act[LP_LAYERS], tap0[5], s0, s1, partials, tail, total;
   int64_t chunks[5], part_off[5];
 };
 
-bool is_tap_layer(int l) { return l == 1 || l == 3 || l == 6 || l == 9 || l == 12; }
-
-Layout layout_of(const Dims& d, bool save) {
+Layout layout_of(const Dims& d, int levels, bool save, int64_t tail_floats) {
   Layout L; int64_t o = 0;
+  const int last = LP_TAP_LAYER[deepest(levels)];
   for (int l = 0; l < LP_LAYERS; ++l) {
     L.act[l] = -1;
-    if (!save && !is_tap_layer(l)) continue;
-    L.act[l] = o; o += align64(d.B * d.H[LP_LEVEL[l]] * d.W[LP_LEVEL[l]] * LP_COUT[l]);
+    const int lv = LP_LEVEL[l];
+    if (l > last || (!save && !(LP_TAP_LAYER[lv] == l && wants(levels, lv)))) continue;
+    L.act[l] = o; o += align64(d.B * d.H[lv] * d.W[lv] * LP_COUT[l]);
   }
-  for (int k = 0; k < 5; ++k) { L.tap0[k] = o; o += align64(d.B * d.H[k] * d.W[k] * LP_TAP_C[k]); }
+  for (int k = 0; k < 5; ++k) {
+    L.tap0[k] = -1;
+    if (wants(levels, k)) { L.tap0[k] = o; o += align64(d.B * d.H[k] * d.W[k] * LP_TAP_C[k]); }
+  }
   const int64_t big = align64(d.B * d.H[0] * d.W[0] * 64);
   L.s0 = o; o += big;
   L.s1 = o; o += big;
   L.partials = o;
   int64_t p = 0;
   for (int k = 0; k < 5; ++k) {
-    L.chunks[k] = head_chunks(d.H[k], d.W[k]);
+    L.chunks[k] = wants(levels, k) ? head_chunks(d.H[k], d.W[k]) : 0;
     L.part_off[k] = p; p += d.B * L.chunks[k];
   }
   o += align64(p);
-  L.seed = o; o += 64;
+  L.tail = o; o += align64(tail_floats);
   L.total = o;
   return L;
 }
@@ -495,8 +505,8 @@ __global__ void __launch_bounds__(256) lpips_head_backward_kernel(const float* _
   }
 }
 
-// value[b] = sum over taps of (sum of the tap's partials, in chunk order) / (H_k W_k); then the seed is saved for the
-// backward and advanced
+// value[b] = sum over the requested levels k, in order, of (sum of the level's partials, in chunk order) / (H_k W_k); the
+// levels not requested have no chunks.  Then, with a seed (LPIPS), the seed is saved for the backward and advanced.
 struct PartDesc { int64_t off[5], chunks[5]; float inv_hw[5]; };
 
 __global__ void lpips_reduce_kernel(const float* __restrict__ partials, PartDesc pd, int B, float* __restrict__ value,
@@ -504,6 +514,7 @@ __global__ void lpips_reduce_kernel(const float* __restrict__ partials, PartDesc
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     float v = 0.f;
     for (int k = 0; k < 5; ++k) {
+      if (pd.chunks[k] == 0) continue;
       const float* p = partials + pd.off[k] + (int64_t)b * pd.chunks[k];
       float s = 0.f;
       for (int64_t c = 0; c < pd.chunks[k]; ++c) s += p[c];
@@ -511,7 +522,7 @@ __global__ void lpips_reduce_kernel(const float* __restrict__ partials, PartDesc
     }
     value[b] = v;
   }
-  if (threadIdx.x == 0) { *seed_used = *seed; *seed = *seed + 1u; }
+  if (seed && threadIdx.x == 0) { *seed_used = *seed; *seed = *seed + 1u; }
 }
 
 __global__ void lpips_prepare_kernel(const float* __restrict__ w, float* __restrict__ fwd, float* __restrict__ bwd, int Cin, int Cout) {
@@ -601,22 +612,6 @@ __global__ void vgg_relu_mask_kernel(const float4* __restrict__ act, float4* __r
   float4 v = g[i];
   v.x = a.x > 0.f ? v.x : 0.f; v.y = a.y > 0.f ? v.y : 0.f; v.z = a.z > 0.f ? v.z : 0.f; v.w = a.w > 0.f ? v.w : 0.f;
   g[i] = v;
-}
-
-// value[b] = sum over the requested levels k, in order, of (sum of the level's partials, in chunk order) / (H_k W_k); the
-// levels not requested have no chunks
-__global__ void vgg_reduce_kernel(const float* __restrict__ partials, PartDesc pd, int B, float* __restrict__ value) {
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    float v = 0.f;
-    for (int k = 0; k < 5; ++k) {
-      if (pd.chunks[k] == 0) continue;
-      const float* p = partials + pd.off[k] + (int64_t)b * pd.chunks[k];
-      float s = 0.f;
-      for (int64_t c = 0; c < pd.chunks[k]; ++c) s += p[c];
-      v += s * pd.inv_hw[k];
-    }
-    value[b] = v;
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ target cache
@@ -835,43 +830,77 @@ int check_head_args(const char* what, int64_t B, int H, int W, int C, int tap) {
   return 0;
 }
 
-int check_dims(const char* what, int64_t B, int H, int W) {
-  if (B < 1 || B > 65535 || H < 16 || W < 16 || H > 32767 || W > 32767 || B * H * W * 64 >= ((int64_t)1 << 40) ||
+// B, H, W for the trunk through the deepest of `levels` (its tap at least 1x1) and the conv kernels' int32 pixel indices;
+// a level mask outside 1..31 fails too
+int check_sizes(const char* what, int64_t B, int H, int W, int levels) {
+  if (levels < 1 || levels > ALL_LEVELS) return dbw_fail_(what, cudaSuccess);
+  const int min_hw = 1 << deepest(levels);
+  if (B < 1 || B > 65535 || H < min_hw || W < min_hw || H > 32767 || W > 32767 || B * H * W * 64 >= ((int64_t)1 << 40) ||
       B * H * W >= ((int64_t)1 << 31) - CV_BM)
     return dbw_fail_(what, cudaSuccess);
   return 0;
 }
 
-// the conv weights, the input transform and the prepared copies (all dbw_lpips_prepare_weights needs)
-bool trunk_ok(const DbwLpipsNet* net) {
-  if (!net || !net->shift || !net->scale || !net->prepared) return false;
+// what a caller reads of net: the conv weights and their prepared copies, the input transform when `transform`, the lin
+// weights when `lin`
+bool net_ok(const DbwLpipsNet* net, bool transform, bool lin) {
+  if (!net || !net->prepared || (transform && (!net->shift || !net->scale))) return false;
   for (int l = 0; l < LP_LAYERS; ++l) if (!net->conv_w[l] || !net->conv_b[l]) return false;
+  for (int k = 0; k < 5; ++k) if (lin && !net->lin_w[k]) return false;
   return true;
 }
 
-bool net_ok(const DbwLpipsNet* net) {
-  if (!trunk_ok(net)) return false;
-  for (int k = 0; k < 5; ++k) if (!net->lin_w[k]) return false;
-  return true;
+// what differs between the two terms on the trunk: LPIPS (every level, the normalised head with the learned lin weights,
+// dropout, the 2x - 1 option, an optional target cache for in0) and the VGG feature loss (the requested levels, either head,
+// constant weights and input transform read from the workspace)
+struct Term {
+  int levels;
+  bool normalized;                    // lpips_head_* with lin[k], else vgg_head_plain_* with w[k]
+  const float* lin[5];
+  float w[5];
+  int train;                          // dropout keyed by *seed: the device seed in the forward, the one it saved in the backward
+  uint32_t* seed;
+  int normalize;                      // x -> 2x - 1, then (x - shift) / scale
+  const float *shift, *scale;
+  const DbwLpipsTargetCache* cache;   // NULL, or in0's target cache with the route and hit count of the cached calls
+  int32_t* route;
+  int32_t* n_hits;
+};
+
+constexpr int64_t LPIPS_TAIL = 64;    // the seed the forward used, then the target cache's miss count
+
+Term lpips_term(const DbwLpipsNet* net, int normalize, int train, uint32_t* seed, const DbwLpipsTargetCache* cache = nullptr,
+                int32_t* route = nullptr, int32_t* n_hits = nullptr) {
+  Term t{ALL_LEVELS, true, {}, {}, train, seed, normalize, net->shift, net->scale, cache, route, n_hits};
+  for (int k = 0; k < 5; ++k) t.lin[k] = net->lin_w[k];
+  return t;
 }
 
-// layers 0..last of one image batch x: out[l] receives layer l's activation, the pool before level k writes pool_out[k]
-// (S0 without pool_out).  With route and count (the miss chain), only the images of route[s][1] for slots s < *count,
-// compacted in slot order.
-int trunk(const DbwLpipsNet* net, const float* x, float* const* out, float* S0, const Dims& d, int normalize, cudaStream_t st,
-          const int32_t* route = nullptr, const int* count = nullptr, int last = LP_LAYERS - 1, float* const* pool_out = nullptr) {
+// consts: what vgg_consts_kernel wrote, in the workspace's last region
+Term vgg_term(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* consts) {
+  Term t{opt->levels, opt->normalize_features != 0, {}, {}, 0, nullptr, 0, net->shift, net->scale, nullptr, nullptr, nullptr};
+  // the first layer applies (x - shift) / scale: the ImageNet statistics, or the identity of the constants
+  if (!opt->normalize_input) { t.shift = consts + 5 * 512; t.scale = consts + 5 * 512 + 4; }
+  for (int k = 0; k < 5; ++k) { t.lin[k] = consts + 512 * k; t.w[k] = opt->sum_channels ? 1.f : 1.f / (float)LP_TAP_C[k]; }
+  return t;
+}
+
+// layers 0..last of one image batch x, through the term's input transform: out[l] receives layer l's activation, the pool
+// before level k writes pool_out[k].  With route and count (the miss chain), only the images of route[s][1] for slots
+// s < *count, compacted in slot order.
+int trunk(const DbwLpipsNet* net, const Term& t, const float* x, float* const* out, float* const* pool_out, const Dims& d, int last,
+          cudaStream_t st, const int32_t* route = nullptr, const int* count = nullptr) {
   const float* prep = (const float*)net->prepared;
   const int64_t B = d.B;
-  if (const int rc = conv_first(x, net->conv_w[0], net->conv_b[0], net->shift, net->scale, normalize, out[0], B, d.H[0], d.W[0], st,
+  if (const int rc = conv_first(x, net->conv_w[0], net->conv_b[0], t.shift, t.scale, t.normalize, out[0], B, d.H[0], d.W[0], st,
                                 route, count))
     return rc;
   const float* cur = out[0];
   for (int l = 1; l <= last; ++l) {
     const int lv = LP_LEVEL[l];
     if (lv != LP_LEVEL[l - 1]) {
-      float* po = pool_out ? pool_out[lv] : S0;
-      if (const int rc = pool(cur, po, B, d.H[lv - 1], d.W[lv - 1], LP_CIN[l], st, count)) return rc;
-      cur = po;
+      if (const int rc = pool(cur, pool_out[lv], B, d.H[lv - 1], d.W[lv - 1], LP_CIN[l], st, count)) return rc;
+      cur = pool_out[lv];
     }
     if (const int rc = conv3x3(cur, prep + wfwd_off(l), net->conv_b[l], nullptr, out[l], B, d.H[lv], d.W[lv], LP_CIN[l], LP_COUT[l], 1,
                                st, count))
@@ -881,165 +910,9 @@ int trunk(const DbwLpipsNet* net, const float* x, float* const* out, float* S0, 
   return 0;
 }
 
-// imgs keeps only its taps: the other layers alternate between the scratch tensors (pool outputs go to S0)
-void imgs_outputs(float* S0, float* S1, float* const* T, float** out) {
-  float* o[LP_LAYERS] = {S1, T[0], S1, T[1], S1, S0, T[2], S1, S0, T[3], S1, S0, T[4]};
-  for (int l = 0; l < LP_LAYERS; ++l) out[l] = o[l];
-}
-
-bool cache_ok(const DbwLpipsTargetCache* c) { return c && c->arena && c->N >= 1 && c->N < ((int64_t)1 << 31); }
-
-// the whole forward; cache: NULL, or the target cache (route and n_hits as dbw_lpips_forward_cached takes them)
-int forward_impl(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const float* in0, const float* in1, int64_t B, int H, int W,
-                 int normalize, int train, int save_for_backward, uint32_t* seed, float* value, int32_t* route, int32_t* n_hits,
-                 void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  const Dims d = dims_of(B, H, W);
-  const bool save = save_for_backward != 0;
-  const Layout L = layout_of(d, save);
-  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_forward: workspace too small", cudaSuccess);
-  float* ws = (float*)workspace;
-  float *S0 = ws + L.s0, *S1 = ws + L.s1, *T[5];
-  for (int k = 0; k < 5; ++k) T[k] = ws + L.tap0[k];
-  float* out0[LP_LAYERS];
-  imgs_outputs(S0, S1, T, out0);
-  // rec keeps every activation for the backward, or like imgs only its taps
-  float* out1[LP_LAYERS];
-  for (int l = 0; l < LP_LAYERS; ++l) out1[l] = L.act[l] >= 0 ? ws + L.act[l] : out0[l];
-  const float* cache_tap[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  if (cache) {
-    // look imgs up (fingerprint partials in S1, the miss count beside the seed), then run its chain over the misses only:
-    // their taps land in the first n_miss images of tap0
-    const CacheLayout C = cache_layout_of(cache->N, H, W);
-    const float* arena = (const float*)cache->arena;
-    for (int k = 0; k < 5; ++k) cache_tap[k] = arena + C.tap[k];
-    const int64_t n = 3 * (int64_t)H * W;
-    uint64_t* part = (uint64_t*)S1;
-    int* n_miss = (int*)(ws + L.seed) + 1;
-    lpips_fingerprint_kernel<<<dim3(FP_CHUNKS, (unsigned)B), 256, 0, st>>>(in0, n, part);
-    LP_LAUNCH_CK("lpips_fingerprint_kernel");
-    lpips_lookup_kernel<<<(unsigned)B, LOOKUP_THREADS, 0, st>>>(in0, n, part, (const uint64_t*)(arena + C.fp), arena + C.img, cache->N,
-                                                                route);
-    LP_LAUNCH_CK("lpips_lookup_kernel");
-    lpips_route_kernel<<<1, 32, 0, st>>>(route, B, n_miss, n_hits);
-    LP_LAUNCH_CK("lpips_route_kernel");
-    if (const int rc = trunk(net, in0, out0, S0, d, normalize, st, route, n_miss)) return rc;
-  } else if (const int rc = trunk(net, in0, out0, S0, d, normalize, st)) {
-    return rc;
-  }
-  if (const int rc = trunk(net, in1, out1, S0, d, normalize, st)) return rc;
-  for (int k = 0; k < 5; ++k)
-    if (const int rc = head_forward(T[k], out1[LP_TAP_LAYER[k]], net->lin_w[k], B, d.H[k], d.W[k], LP_TAP_C[k], k, train, seed,
-                                    ws + L.partials + L.part_off[k], st, cache ? route : nullptr, cache_tap[k]))
-      return rc;
-  PartDesc pd;
-  for (int k = 0; k < 5; ++k) { pd.off[k] = L.part_off[k]; pd.chunks[k] = L.chunks[k]; pd.inv_hw[k] = 1.f / (float)(d.H[k] * d.W[k]); }
-  lpips_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value, seed, (uint32_t*)(ws + L.seed));
-  LP_LAUNCH_CK("lpips_reduce_kernel");
-  return 0;
-}
-
-int backward_impl(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const int32_t* route, const float* grad_value, int64_t B,
-                  int H, int W, int normalize, int train, float* grad_in1, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  const Dims d = dims_of(B, H, W);
-  const Layout L = layout_of(d, true);
-  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_backward: workspace too small", cudaSuccess);
-  float* ws = (float*)workspace;
-  const float* prep = (const float*)net->prepared;
-  const uint32_t* seed_used = (const uint32_t*)(ws + L.seed);
-  const float* cache_tap[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  if (cache) {
-    const CacheLayout C = cache_layout_of(cache->N, H, W);
-    for (int k = 0; k < 5; ++k) cache_tap[k] = (const float*)cache->arena + C.tap[k];
-  }
-  float* G[2] = {ws + L.s0, ws + L.s1};
-  int cur = 0;                        // G[cur] holds the gradient at the pre-activation of layer l
-  for (int l = LP_LAYERS - 1; l >= 1; --l) {
-    const int lv = LP_LEVEL[l];
-    const float* act = ws + L.act[l];
-    if (l == LP_TAP_LAYER[lv]) {
-      const bool deepest = lv == 4;
-      if (!deepest) {                 // G[cur] holds the gradient at the next pool's output: route it back to this tap
-        if (const int rc = pool_backward(act, G[cur], G[cur ^ 1], B, d.H[lv], d.W[lv], LP_COUT[l], st)) return rc;
-        cur ^= 1;
-      }
-      if (const int rc = head_backward(ws + L.tap0[lv], act, net->lin_w[lv], B, d.H[lv], d.W[lv], LP_TAP_C[lv], lv, train, seed_used,
-                                       grad_value, !deepest, G[cur], st, cache ? route : nullptr, cache_tap[lv]))
-        return rc;
-    }
-    // input gradient of layer l; masked by the ReLU below unless a pool sits in between
-    const bool after_pool = LP_LEVEL[l - 1] != lv;
-    if (const int rc = conv3x3(G[cur], prep + wbwd_off(l), nullptr, after_pool ? nullptr : ws + L.act[l - 1], G[cur ^ 1], B,
-                               d.H[lv], d.W[lv], LP_COUT[l], LP_CIN[l], 0, st))
-      return rc;
-    cur ^= 1;
-  }
-  return dgrad_last(G[cur], net->conv_w[0], net->scale, normalize, grad_in1, B, H, W, st);
-}
-
-int check_cache(const char* what, const DbwLpipsTargetCache* cache, int H, int W, int normalize) {
-  if (!cache_ok(cache)) return dbw_fail_(what, cudaSuccess);
-  if (cache->H != H || cache->W != W || (cache->normalize != 0) != (normalize != 0)) return dbw_fail_(what, cudaSuccess);
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------------ VGG feature loss (host)
-bool vgg_wants(int levels, int k) { return (levels >> k) & 1; }
-int vgg_deepest(int levels) { int L = 0; for (int k = 0; k < 5; ++k) if (vgg_wants(levels, k)) L = k; return L; }   // 0-based
-
-// workspace layout, in floats (stated in include/dbw_render.h): rec's activations through the deepest level (only its
-// requested taps when no backward follows), imgs' requested taps, two scratch tensors of B*H*W*64, the head partials of the
-// requested levels, the constants of vgg_consts_kernel
-struct VggLayout {
-  int64_t act[LP_LAYERS], tap0[5], s0, s1, partials, consts, total;
-  int64_t chunks[5], part_off[5];
-};
-
-VggLayout vgg_layout_of(const Dims& d, int levels, bool save) {
-  VggLayout L; int64_t o = 0;
-  const int last = LP_TAP_LAYER[vgg_deepest(levels)];
-  for (int l = 0; l < LP_LAYERS; ++l) {
-    L.act[l] = -1;
-    const int lv = LP_LEVEL[l];
-    if (l > last || (!save && !(LP_TAP_LAYER[lv] == l && vgg_wants(levels, lv)))) continue;
-    L.act[l] = o; o += align64(d.B * d.H[lv] * d.W[lv] * LP_COUT[l]);
-  }
-  for (int k = 0; k < 5; ++k) {
-    L.tap0[k] = -1;
-    if (vgg_wants(levels, k)) { L.tap0[k] = o; o += align64(d.B * d.H[k] * d.W[k] * LP_TAP_C[k]); }
-  }
-  const int64_t big = align64(d.B * d.H[0] * d.W[0] * 64);
-  L.s0 = o; o += big;
-  L.s1 = o; o += big;
-  L.partials = o;
-  int64_t p = 0;
-  for (int k = 0; k < 5; ++k) {
-    L.chunks[k] = vgg_wants(levels, k) ? head_chunks(d.H[k], d.W[k]) : 0;
-    L.part_off[k] = p; p += d.B * L.chunks[k];
-  }
-  o += align64(p);
-  L.consts = o; o += align64(VGG_CONSTS);
-  L.total = o;
-  return L;
-}
-
-int check_vgg_args(const char* what, int64_t B, int H, int W, const DbwVggLossOptions* opt) {
-  if (!opt || opt->levels < 1 || opt->levels > 31) return dbw_fail_(what, cudaSuccess);
-  const int min_hw = 1 << vgg_deepest(opt->levels);
-  if (B < 1 || B > 65535 || H < min_hw || W < min_hw || H > 32767 || W > 32767 || B * H * W * 64 >= ((int64_t)1 << 40) ||
-      B * H * W >= ((int64_t)1 << 31) - CV_BM)
-    return dbw_fail_(what, cudaSuccess);
-  return 0;
-}
-
-bool vgg_net_ok(const DbwLpipsNet* net, const DbwVggLossOptions* opt) {
-  if (!net || !net->prepared || (opt->normalize_input && (!net->shift || !net->scale))) return false;
-  for (int l = 0; l < LP_LAYERS; ++l) if (!net->conv_w[l] || !net->conv_b[l]) return false;
-  return true;
-}
-
 // the outputs of one chain through layer `last`: keep[l] where given, else (as for the pools) whichever scratch tensor the
 // layer does not read
-void vgg_chain_outputs(float* const* keep, int last, float* S0, float* S1, float** out, float** pool_out) {
+void chain_outputs(float* const* keep, int last, float* S0, float* S1, float** out, float** pool_out) {
   const float* cur = nullptr;
   for (int l = 0; l <= last; ++l) {
     if (l > 0 && LP_LEVEL[l] != LP_LEVEL[l - 1]) {
@@ -1050,6 +923,8 @@ void vgg_chain_outputs(float* const* keep, int last, float* S0, float* S1, float
     cur = out[l];
   }
 }
+
+bool cache_ok(const DbwLpipsTargetCache* c) { return c && c->arena && c->N >= 1 && c->N < ((int64_t)1 << 31); }
 
 // the plain head of C channels (64, 128, 256 or 512): partials (B, head_chunks(H, W)) as head_forward writes them
 int head_plain_forward(const float* f0, const float* f1, float w, int64_t B, int H, int W, int C, float* part, cudaStream_t st) {
@@ -1079,81 +954,88 @@ int head_plain_backward(const float* f0, const float* f1, float w, int64_t B, in
   return 0;
 }
 
-int vgg_head_forward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
-                     float* part, cudaStream_t st) {
-  if (normalized) return head_forward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, part, st);
-  return head_plain_forward(f0, f1, w, B, H, W, LP_TAP_C[k], part, st);
-}
-
-int vgg_head_backward(const float* f0, const float* f1, const float* lin, float w, bool normalized, int64_t B, int H, int W, int k,
-                      const float* grad_value, int accumulate, float* g, cudaStream_t st) {
-  if (normalized) return head_backward(f0, f1, lin, B, H, W, LP_TAP_C[k], k, 0, nullptr, grad_value, accumulate, g, st);
-  return head_plain_backward(f0, f1, w, B, H, W, LP_TAP_C[k], grad_value, accumulate, g, st);
-}
-
-float vgg_head_weight(const DbwVggLossOptions* opt, int k) { return opt->sum_channels ? 1.f : 1.f / (float)LP_TAP_C[k]; }
-
-int vgg_forward_impl(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* in0, const float* in1, int64_t B, int H, int W,
-                     int save_for_backward, float* value, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  const Dims d = dims_of(B, H, W);
-  const int levels = opt->levels, last = LP_TAP_LAYER[vgg_deepest(levels)];
-  const VggLayout L = vgg_layout_of(d, levels, save_for_backward != 0);
-  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_vgg_loss_forward: workspace too small", cudaSuccess);
-  float* ws = (float*)workspace;
-  float *S0 = ws + L.s0, *S1 = ws + L.s1, *consts = ws + L.consts;
-  vgg_consts_kernel<<<1, 256, 0, st>>>(consts, opt->sum_channels);
-  LP_LAUNCH_CK("vgg_consts_kernel");
-  // the first layer applies (x - shift) / scale: the ImageNet statistics, or the identity of the constants
-  DbwLpipsNet n = *net;
-  if (!opt->normalize_input) { n.shift = consts + 5 * 512; n.scale = consts + 5 * 512 + 4; }
+// the whole forward into a workspace of layout L: the target cache's lookup of in0, in0's chain (over the misses only when
+// cached), in1's chain, the heads of the requested levels, one reduction
+int forward_impl(const DbwLpipsNet* net, const Term& t, const float* in0, const float* in1, const Dims& d, const Layout& L,
+                 float* ws, float* value, cudaStream_t st) {
+  const int64_t B = d.B;
+  const int last = LP_TAP_LAYER[deepest(t.levels)];
+  // imgs keeps only its requested taps; rec every activation for the backward, or like imgs only its taps
   float* keep0[LP_LAYERS] = {};
   float* keep1[LP_LAYERS] = {};
   for (int l = 0; l <= last; ++l) {
     const int lv = LP_LEVEL[l];
-    if (LP_TAP_LAYER[lv] == l && vgg_wants(levels, lv)) keep0[l] = ws + L.tap0[lv];
+    if (LP_TAP_LAYER[lv] == l && wants(t.levels, lv)) keep0[l] = ws + L.tap0[lv];
     if (L.act[l] >= 0) keep1[l] = ws + L.act[l];
   }
   float *out0[LP_LAYERS], *out1[LP_LAYERS], *pool0[5], *pool1[5];
-  vgg_chain_outputs(keep0, last, S0, S1, out0, pool0);
-  vgg_chain_outputs(keep1, last, S0, S1, out1, pool1);
-  if (const int rc = trunk(&n, in0, out0, S0, d, 0, st, nullptr, nullptr, last, pool0)) return rc;
-  if (const int rc = trunk(&n, in1, out1, S0, d, 0, st, nullptr, nullptr, last, pool1)) return rc;
+  chain_outputs(keep0, last, ws + L.s0, ws + L.s1, out0, pool0);
+  chain_outputs(keep1, last, ws + L.s0, ws + L.s1, out1, pool1);
+  const float* cache_tap[5] = {};
+  if (t.cache) {
+    // look imgs up (fingerprint partials in S1, the miss count beside the seed), then run its chain over the misses only:
+    // their taps land in the first n_miss images of tap0
+    const CacheLayout C = cache_layout_of(t.cache->N, d.H[0], d.W[0]);
+    const float* arena = (const float*)t.cache->arena;
+    for (int k = 0; k < 5; ++k) cache_tap[k] = arena + C.tap[k];
+    const int64_t n = 3 * (int64_t)d.H[0] * d.W[0];
+    uint64_t* part = (uint64_t*)(ws + L.s1);
+    int* n_miss = (int*)(ws + L.tail) + 1;
+    lpips_fingerprint_kernel<<<dim3(FP_CHUNKS, (unsigned)B), 256, 0, st>>>(in0, n, part);
+    LP_LAUNCH_CK("lpips_fingerprint_kernel");
+    lpips_lookup_kernel<<<(unsigned)B, LOOKUP_THREADS, 0, st>>>(in0, n, part, (const uint64_t*)(arena + C.fp), arena + C.img,
+                                                                t.cache->N, t.route);
+    LP_LAUNCH_CK("lpips_lookup_kernel");
+    lpips_route_kernel<<<1, 32, 0, st>>>(t.route, B, n_miss, t.n_hits);
+    LP_LAUNCH_CK("lpips_route_kernel");
+    if (const int rc = trunk(net, t, in0, out0, pool0, d, last, st, t.route, n_miss)) return rc;
+  } else if (const int rc = trunk(net, t, in0, out0, pool0, d, last, st)) {
+    return rc;
+  }
+  if (const int rc = trunk(net, t, in1, out1, pool1, d, last, st)) return rc;
   PartDesc pd;
   for (int k = 0; k < 5; ++k) {
     pd.off[k] = L.part_off[k]; pd.chunks[k] = L.chunks[k]; pd.inv_hw[k] = 1.f / (float)(d.H[k] * d.W[k]);
-    if (!vgg_wants(levels, k)) continue;
-    if (const int rc = vgg_head_forward(ws + L.tap0[k], out1[LP_TAP_LAYER[k]], consts + 512 * k, vgg_head_weight(opt, k),
-                                        opt->normalize_features != 0, B, d.H[k], d.W[k], k, ws + L.partials + L.part_off[k], st))
+    if (!wants(t.levels, k)) continue;
+    const float *f0 = ws + L.tap0[k], *f1 = out1[LP_TAP_LAYER[k]];
+    float* part = ws + L.partials + L.part_off[k];
+    if (const int rc = t.normalized ? head_forward(f0, f1, t.lin[k], B, d.H[k], d.W[k], LP_TAP_C[k], k, t.train, t.seed, part, st,
+                                                   t.route, cache_tap[k])
+                                    : head_plain_forward(f0, f1, t.w[k], B, d.H[k], d.W[k], LP_TAP_C[k], part, st))
       return rc;
   }
-  vgg_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value);
-  LP_LAUNCH_CK("vgg_reduce_kernel");
+  lpips_reduce_kernel<<<1, 256, 0, st>>>(ws + L.partials, pd, (int)B, value, t.seed, t.seed ? (uint32_t*)(ws + L.tail) : nullptr);
+  LP_LAUNCH_CK("lpips_reduce_kernel");
   return 0;
 }
 
-int vgg_backward_impl(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B, int H, int W,
-                      float* grad_in1, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  const Dims d = dims_of(B, H, W);
-  const int levels = opt->levels, last = LP_TAP_LAYER[vgg_deepest(levels)];
-  const VggLayout L = vgg_layout_of(d, levels, true);
-  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_vgg_loss_backward: workspace too small", cudaSuccess);
-  float* ws = (float*)workspace;
+int backward_impl(const DbwLpipsNet* net, const Term& t, const float* grad_value, const Dims& d, const Layout& L, float* ws,
+                  float* grad_in1, cudaStream_t st) {
+  const int64_t B = d.B;
+  const int last = LP_TAP_LAYER[deepest(t.levels)];
   const float* prep = (const float*)net->prepared;
-  const float* consts = ws + L.consts;
+  const float* cache_tap[5] = {};
+  if (t.cache) {
+    const CacheLayout C = cache_layout_of(t.cache->N, d.H[0], d.W[0]);
+    for (int k = 0; k < 5; ++k) cache_tap[k] = (const float*)t.cache->arena + C.tap[k];
+  }
   float* G[2] = {ws + L.s0, ws + L.s1};
   int cur = 0;                        // G[cur] holds the gradient at the pre-activation of layer l
   for (int l = last; l >= 1; --l) {
     const int lv = LP_LEVEL[l];
     const float* act = ws + L.act[l];
     if (l == LP_TAP_LAYER[lv]) {
-      const bool deepest = l == last;
-      if (!deepest) {                 // G[cur] holds the gradient at the next pool's output: route it back to this tap
+      const bool bottom = l == last;
+      if (!bottom) {                  // G[cur] holds the gradient at the next pool's output: route it back to this tap
         if (const int rc = pool_backward(act, G[cur], G[cur ^ 1], B, d.H[lv], d.W[lv], LP_COUT[l], st)) return rc;
         cur ^= 1;
       }
-      if (vgg_wants(levels, lv)) {
-        if (const int rc = vgg_head_backward(ws + L.tap0[lv], act, consts + 512 * lv, vgg_head_weight(opt, lv),
-                                             opt->normalize_features != 0, B, d.H[lv], d.W[lv], lv, grad_value, !deepest, G[cur], st))
+      if (wants(t.levels, lv)) {
+        const float* f0 = ws + L.tap0[lv];
+        if (const int rc = t.normalized ? head_backward(f0, act, t.lin[lv], B, d.H[lv], d.W[lv], LP_TAP_C[lv], lv, t.train, t.seed,
+                                                        grad_value, !bottom, G[cur], st, t.route, cache_tap[lv])
+                                        : head_plain_backward(f0, act, t.w[lv], B, d.H[lv], d.W[lv], LP_TAP_C[lv], grad_value, !bottom,
+                                                              G[cur], st))
           return rc;
       } else {                        // the deepest level is always requested
         const int64_t n4 = B * d.H[lv] * d.W[lv] * LP_COUT[l] / 4;
@@ -1170,8 +1052,34 @@ int vgg_backward_impl(const DbwLpipsNet* net, const DbwVggLossOptions* opt, cons
       return rc;
     cur ^= 1;
   }
-  const float* scale = opt->normalize_input ? net->scale : consts + 5 * 512 + 4;
-  return dgrad_last(G[cur], net->conv_w[0], scale, 0, grad_in1, B, H, W, st);
+  return dgrad_last(G[cur], net->conv_w[0], t.scale, t.normalize, grad_in1, B, d.H[0], d.W[0], st);
+}
+
+// LPIPS's forward and backward, with or without the target cache
+int lpips_forward(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const float* in0, const float* in1, int64_t B, int H,
+                  int W, int normalize, int train, int save_for_backward, uint32_t* seed, float* value, int32_t* route,
+                  int32_t* n_hits, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const Dims d = dims_of(B, H, W);
+  const Layout L = layout_of(d, ALL_LEVELS, save_for_backward != 0, LPIPS_TAIL);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_forward: workspace too small", cudaSuccess);
+  return forward_impl(net, lpips_term(net, normalize, train, seed, cache, route, n_hits), in0, in1, d, L, (float*)workspace, value,
+                      st);
+}
+
+int lpips_backward(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const int32_t* route, const float* grad_value, int64_t B,
+                   int H, int W, int normalize, int train, float* grad_in1, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const Dims d = dims_of(B, H, W);
+  const Layout L = layout_of(d, ALL_LEVELS, true, LPIPS_TAIL);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_backward: workspace too small", cudaSuccess);
+  float* ws = (float*)workspace;
+  return backward_impl(net, lpips_term(net, normalize, train, (uint32_t*)(ws + L.tail), cache, (int32_t*)route), grad_value, d, L, ws,
+                       grad_in1, st);
+}
+
+int check_cache(const char* what, const DbwLpipsTargetCache* cache, int H, int W, int normalize) {
+  if (!cache_ok(cache)) return dbw_fail_(what, cudaSuccess);
+  if (cache->H != H || cache->W != W || (cache->normalize != 0) != (normalize != 0)) return dbw_fail_(what, cudaSuccess);
+  return 0;
 }
 
 }  // namespace
@@ -1179,16 +1087,16 @@ int vgg_backward_impl(const DbwLpipsNet* net, const DbwVggLossOptions* opt, cons
 // ------------------------------------------------------------------------------------------------ C-ABI
 extern "C" int dbw_lpips_workspace_bytes(int64_t B, int32_t H, int32_t W, int32_t save_for_backward, size_t* workspace_bytes,
                                          size_t* prepared_bytes) {
-  if (const int rc = check_dims("dbw_lpips_workspace_bytes: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)",
-                                B, H, W)) return rc;
+  if (const int rc = check_sizes("dbw_lpips_workspace_bytes: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)",
+                                B, H, W, ALL_LEVELS)) return rc;
   if (!workspace_bytes || !prepared_bytes) return dbw_fail_("dbw_lpips_workspace_bytes: null pointer argument", cudaSuccess);
-  *workspace_bytes = (size_t)layout_of(dims_of(B, H, W), save_for_backward != 0).total * 4;
+  *workspace_bytes = (size_t)layout_of(dims_of(B, H, W), ALL_LEVELS, save_for_backward != 0, LPIPS_TAIL).total * 4;
   *prepared_bytes = (size_t)wprep_total() * 4;
   return 0;
 }
 
 extern "C" int dbw_lpips_prepare_weights(const DbwLpipsNet* net, void* stream) {
-  if (!trunk_ok(net)) return dbw_fail_("dbw_lpips_prepare_weights: null pointer argument", cudaSuccess);
+  if (!net_ok(net, true, false)) return dbw_fail_("dbw_lpips_prepare_weights: null pointer argument", cudaSuccess);
   cudaStream_t st = (cudaStream_t)stream;
   float* p = (float*)net->prepared;
   for (int l = 1; l < LP_LAYERS; ++l) {
@@ -1203,27 +1111,29 @@ extern "C" int dbw_lpips_prepare_weights(const DbwLpipsNet* net, void* stream) {
 extern "C" int dbw_lpips_forward(const DbwLpipsNet* net, const float* in0, const float* in1, int64_t B, int32_t H, int32_t W,
                                  int32_t normalize, int32_t train, int32_t save_for_backward, uint32_t* seed, float* value,
                                  void* workspace, size_t workspace_bytes, void* stream) {
-  if (const int rc = check_dims("dbw_lpips_forward: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B, H, W))
+  if (const int rc = check_sizes("dbw_lpips_forward: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B, H, W,
+                                  ALL_LEVELS))
     return rc;
-  if (!net_ok(net) || !in0 || !in1 || !seed || !value || !workspace)
+  if (!net_ok(net, true, true) || !in0 || !in1 || !seed || !value || !workspace)
     return dbw_fail_("dbw_lpips_forward: null pointer argument", cudaSuccess);
-  return forward_impl(net, nullptr, in0, in1, B, H, W, normalize, train, save_for_backward, seed, value, nullptr, nullptr, workspace,
-                      workspace_bytes, (cudaStream_t)stream);
+  return lpips_forward(net, nullptr, in0, in1, B, H, W, normalize, train, save_for_backward, seed, value, nullptr, nullptr, workspace,
+                       workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int dbw_lpips_backward(const DbwLpipsNet* net, const float* grad_value, int64_t B, int32_t H, int32_t W,
                                   int32_t normalize, int32_t train, float* grad_in1, void* workspace, size_t workspace_bytes,
                                   void* stream) {
-  if (const int rc = check_dims("dbw_lpips_backward: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B, H, W))
+  if (const int rc = check_sizes("dbw_lpips_backward: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B, H, W,
+                                  ALL_LEVELS))
     return rc;
-  if (!net_ok(net) || !grad_value || !grad_in1 || !workspace)
+  if (!net_ok(net, true, true) || !grad_value || !grad_in1 || !workspace)
     return dbw_fail_("dbw_lpips_backward: null pointer argument", cudaSuccess);
-  return backward_impl(net, nullptr, nullptr, grad_value, B, H, W, normalize, train, grad_in1, workspace, workspace_bytes,
-                       (cudaStream_t)stream);
+  return lpips_backward(net, nullptr, nullptr, grad_value, B, H, W, normalize, train, grad_in1, workspace, workspace_bytes,
+                        (cudaStream_t)stream);
 }
 
 extern "C" int dbw_lpips_cache_bytes(int32_t H, int32_t W, size_t* bytes_per_image) {
-  if (const int rc = check_dims("dbw_lpips_cache_bytes: bad sizes (16 <= H, W <= 32767)", 1, H, W)) return rc;
+  if (const int rc = check_sizes("dbw_lpips_cache_bytes: bad sizes (16 <= H, W <= 32767)", 1, H, W, ALL_LEVELS)) return rc;
   if (!bytes_per_image) return dbw_fail_("dbw_lpips_cache_bytes: null pointer argument", cudaSuccess);
   *bytes_per_image = (size_t)cache_layout_of(1, H, W).total * 4;
   return 0;
@@ -1232,16 +1142,17 @@ extern "C" int dbw_lpips_cache_bytes(int32_t H, int32_t W, size_t* bytes_per_ima
 extern "C" int dbw_lpips_cache_targets(const DbwLpipsNet* net, const float* imgs, const DbwLpipsTargetCache* cache, int64_t chunk,
                                        void* workspace, size_t workspace_bytes, void* stream) {
   if (!cache) return dbw_fail_("dbw_lpips_cache_targets: null pointer argument", cudaSuccess);
-  if (const int rc = check_dims("dbw_lpips_cache_targets: bad sizes (1 <= chunk <= 65535, 16 <= H, W <= 32767, chunk*H*W < 2^31 - 128)",
-                                chunk, cache->H, cache->W))
+  if (const int rc = check_sizes("dbw_lpips_cache_targets: bad sizes (1 <= chunk <= 65535, 16 <= H, W <= 32767, chunk*H*W < 2^31 - 128)",
+                                chunk, cache->H, cache->W, ALL_LEVELS))
     return rc;
-  if (!net_ok(net) || !imgs || !cache_ok(cache) || !workspace)
+  if (!net_ok(net, true, true) || !imgs || !cache_ok(cache) || !workspace)
     return dbw_fail_("dbw_lpips_cache_targets: null pointer argument or bad cache (arena, 1 <= N < 2^31)", cudaSuccess);
   const int H = cache->H, W = cache->W;
-  const Layout L = layout_of(dims_of(chunk, H, W), false);
+  const Layout L = layout_of(dims_of(chunk, H, W), ALL_LEVELS, false, LPIPS_TAIL);
   if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_lpips_cache_targets: workspace too small", cudaSuccess);
   cudaStream_t st = (cudaStream_t)stream;
   const CacheLayout C = cache_layout_of(cache->N, H, W);
+  const Term t = lpips_term(net, cache->normalize, 0, nullptr);
   float* arena = (float*)cache->arena;
   float* ws = (float*)workspace;
   const int64_t n = 3 * (int64_t)H * W;
@@ -1258,11 +1169,11 @@ extern "C" int dbw_lpips_cache_targets(const DbwLpipsNet* net, const float* imgs
     LP_LAUNCH_CK("lpips_fingerprint_kernel");
     lpips_fingerprint_sum_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, st>>>(part, nb, (uint64_t*)(arena + C.fp) + n0);
     LP_LAUNCH_CK("lpips_fingerprint_sum_kernel");
-    float* T[5];
-    for (int k = 0; k < 5; ++k) T[k] = arena + C.tap[k] + n0 * d.H[k] * d.W[k] * LP_TAP_C[k];
-    float* out[LP_LAYERS];
-    imgs_outputs(ws + L.s0, ws + L.s1, T, out);
-    if (const int rc = trunk(net, img + n0 * n, out, ws + L.s0, d, cache->normalize, st)) return rc;
+    float* keep[LP_LAYERS] = {};
+    for (int k = 0; k < 5; ++k) keep[LP_TAP_LAYER[k]] = arena + C.tap[k] + n0 * d.H[k] * d.W[k] * LP_TAP_C[k];
+    float *out[LP_LAYERS], *pool_out[5];
+    chain_outputs(keep, LP_LAYERS - 1, ws + L.s0, ws + L.s1, out, pool_out);
+    if (const int rc = trunk(net, t, img + n0 * n, out, pool_out, d, LP_LAYERS - 1, st)) return rc;
   }
   return 0;
 }
@@ -1271,31 +1182,31 @@ extern "C" int dbw_lpips_forward_cached(const DbwLpipsNet* net, const DbwLpipsTa
                                         int64_t B, int32_t H, int32_t W, int32_t normalize, int32_t train, int32_t save_for_backward,
                                         uint32_t* seed, float* value, int32_t* route, int32_t* n_hits, void* workspace,
                                         size_t workspace_bytes, void* stream) {
-  if (const int rc = check_dims("dbw_lpips_forward_cached: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B,
-                                H, W))
+  if (const int rc = check_sizes("dbw_lpips_forward_cached: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B,
+                                H, W, ALL_LEVELS))
     return rc;
-  if (!net_ok(net) || !in0 || !in1 || !seed || !value || !route || !workspace)
+  if (!net_ok(net, true, true) || !in0 || !in1 || !seed || !value || !route || !workspace)
     return dbw_fail_("dbw_lpips_forward_cached: null pointer argument", cudaSuccess);
   if (const int rc = check_cache("dbw_lpips_forward_cached: bad cache (NULL arena, N < 1, or another H, W or normalize)", cache, H, W,
                                  normalize))
     return rc;
-  return forward_impl(net, cache, in0, in1, B, H, W, normalize, train, save_for_backward, seed, value, route, n_hits, workspace,
-                      workspace_bytes, (cudaStream_t)stream);
+  return lpips_forward(net, cache, in0, in1, B, H, W, normalize, train, save_for_backward, seed, value, route, n_hits, workspace,
+                       workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int dbw_lpips_backward_cached(const DbwLpipsNet* net, const DbwLpipsTargetCache* cache, const int32_t* route,
                                          const float* grad_value, int64_t B, int32_t H, int32_t W, int32_t normalize, int32_t train,
                                          float* grad_in1, void* workspace, size_t workspace_bytes, void* stream) {
-  if (const int rc = check_dims("dbw_lpips_backward_cached: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B,
-                                H, W))
+  if (const int rc = check_sizes("dbw_lpips_backward_cached: bad sizes (1 <= B <= 65535, 16 <= H, W <= 32767, B*H*W < 2^31 - 128)", B,
+                                H, W, ALL_LEVELS))
     return rc;
-  if (!net_ok(net) || !route || !grad_value || !grad_in1 || !workspace)
+  if (!net_ok(net, true, true) || !route || !grad_value || !grad_in1 || !workspace)
     return dbw_fail_("dbw_lpips_backward_cached: null pointer argument", cudaSuccess);
   if (const int rc = check_cache("dbw_lpips_backward_cached: bad cache (NULL arena, N < 1, or another H, W or normalize)", cache, H, W,
                                  normalize))
     return rc;
-  return backward_impl(net, cache, route, grad_value, B, H, W, normalize, train, grad_in1, workspace, workspace_bytes,
-                       (cudaStream_t)stream);
+  return lpips_backward(net, cache, route, grad_value, B, H, W, normalize, train, grad_in1, workspace, workspace_bytes,
+                        (cudaStream_t)stream);
 }
 
 // single layers, for tests and per-layer timing (scripts/bench_lpips.py)
@@ -1361,27 +1272,39 @@ extern "C" int dbw_lpips_head_backward(const float* f0, const float* f1, const f
 
 extern "C" int dbw_vgg_loss_workspace_bytes(int64_t B, int32_t H, int32_t W, const DbwVggLossOptions* opt, int32_t save_for_backward,
                                             size_t* workspace_bytes) {
-  if (const int rc = check_vgg_args("dbw_vgg_loss_workspace_bytes: bad options or sizes " VGG_SIZES, B, H, W, opt)) return rc;
+  if (const int rc = check_sizes("dbw_vgg_loss_workspace_bytes: bad options or sizes " VGG_SIZES, B, H, W, opt ? opt->levels : 0))
+    return rc;
   if (!workspace_bytes) return dbw_fail_("dbw_vgg_loss_workspace_bytes: null pointer argument", cudaSuccess);
-  *workspace_bytes = (size_t)vgg_layout_of(dims_of(B, H, W), opt->levels, save_for_backward != 0).total * 4;
+  *workspace_bytes = (size_t)layout_of(dims_of(B, H, W), opt->levels, save_for_backward != 0, VGG_CONSTS).total * 4;
   return 0;
 }
 
 extern "C" int dbw_vgg_loss_forward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* in0, const float* in1, int64_t B,
                                     int32_t H, int32_t W, int32_t save_for_backward, float* value, void* workspace,
                                     size_t workspace_bytes, void* stream) {
-  if (const int rc = check_vgg_args("dbw_vgg_loss_forward: bad options or sizes " VGG_SIZES, B, H, W, opt)) return rc;
-  if (!vgg_net_ok(net, opt) || !in0 || !in1 || !value || !workspace)
+  if (const int rc = check_sizes("dbw_vgg_loss_forward: bad options or sizes " VGG_SIZES, B, H, W, opt ? opt->levels : 0)) return rc;
+  if (!net_ok(net, opt->normalize_input, false) || !in0 || !in1 || !value || !workspace)
     return dbw_fail_("dbw_vgg_loss_forward: null pointer argument", cudaSuccess);
-  return vgg_forward_impl(net, opt, in0, in1, B, H, W, save_for_backward, value, workspace, workspace_bytes, (cudaStream_t)stream);
+  const Dims d = dims_of(B, H, W);
+  const Layout L = layout_of(d, opt->levels, save_for_backward != 0, VGG_CONSTS);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_vgg_loss_forward: workspace too small", cudaSuccess);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  vgg_consts_kernel<<<1, 256, 0, st>>>(ws + L.tail, opt->sum_channels);
+  LP_LAUNCH_CK("vgg_consts_kernel");
+  return forward_impl(net, vgg_term(net, opt, ws + L.tail), in0, in1, d, L, ws, value, st);
 }
 
 extern "C" int dbw_vgg_loss_backward(const DbwLpipsNet* net, const DbwVggLossOptions* opt, const float* grad_value, int64_t B,
                                      int32_t H, int32_t W, float* grad_in1, void* workspace, size_t workspace_bytes, void* stream) {
-  if (const int rc = check_vgg_args("dbw_vgg_loss_backward: bad options or sizes " VGG_SIZES, B, H, W, opt)) return rc;
-  if (!vgg_net_ok(net, opt) || !grad_value || !grad_in1 || !workspace)
+  if (const int rc = check_sizes("dbw_vgg_loss_backward: bad options or sizes " VGG_SIZES, B, H, W, opt ? opt->levels : 0)) return rc;
+  if (!net_ok(net, opt->normalize_input, false) || !grad_value || !grad_in1 || !workspace)
     return dbw_fail_("dbw_vgg_loss_backward: null pointer argument", cudaSuccess);
-  return vgg_backward_impl(net, opt, grad_value, B, H, W, grad_in1, workspace, workspace_bytes, (cudaStream_t)stream);
+  const Dims d = dims_of(B, H, W);
+  const Layout L = layout_of(d, opt->levels, true, VGG_CONSTS);
+  if (workspace_bytes < (size_t)L.total * 4) return dbw_fail_("dbw_vgg_loss_backward: workspace too small", cudaSuccess);
+  float* ws = (float*)workspace;
+  return backward_impl(net, vgg_term(net, opt, ws + L.tail), grad_value, d, L, ws, grad_in1, (cudaStream_t)stream);
 }
 
 // the plain head alone, for tests: the launchers of the whole term

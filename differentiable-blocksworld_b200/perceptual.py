@@ -154,7 +154,98 @@ def _stream(dev):
     return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
-class LPIPS(nn.Module):
+def _strip(sd, prefixes):
+    """sd with each of `prefixes` that some key carries stripped, in order (the keys without it dropped)"""
+    sd = dict(sd)
+    for prefix in prefixes:
+        if any(k.startswith(prefix) for k in sd):
+            sd = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
+    return sd
+
+
+class _Trunk(nn.Module):
+    """What LPIPS and PerceptualLoss share: torchvision's VGG16 convolutions on the kernels of csrc/dbw_lpips.cu, their TF32
+    copies in `prepared`, loading their weights, and the checks on the two images.  A subclass names its convolutions
+    (`_convs`), its input transform (`_transform`) and its lin weights (`_lins`)."""
+
+    def __init__(self):
+        super().__init__()
+        self.register_buffer('prepared', torch.zeros(0), persistent=False)
+        self._prepared_key = None
+
+    def _lins(self):
+        return []
+
+    @classmethod
+    def _load(cls, sd, shapes, **options):
+        """an instance holding sd's entries of `shapes`; raises on a missing or misshapen key"""
+        missing = [k for k in shapes if k not in sd]
+        if missing:
+            raise KeyError(f'{cls.__name__}.from_state_dict: missing keys {missing}')
+        bad = [(k, tuple(sd[k].shape), s) for k, s in shapes.items() if tuple(sd[k].shape) != s]
+        if bad:
+            raise ValueError(f'{cls.__name__}.from_state_dict: misshapen keys (key, got, want) {bad}')
+        m = cls(**options)
+        m.load_state_dict({k: sd[k] for k in shapes}, strict=True)
+        return m
+
+    @classmethod
+    def _features(cls, vgg16_pth, prefix):
+        """{prefix + 'slice{s}.{i}.weight' / '.bias': torchvision's `features.{i}.*`} of its vgg16 state dict"""
+        vgg = torch.load(vgg16_pth, map_location='cpu', weights_only=True)
+        sd = {}
+        for s, i, _, _ in CONVS:
+            for n in ('weight', 'bias'):
+                if f'features.{i}.{n}' not in vgg:
+                    raise KeyError(f'{cls.__name__}.from_files: {vgg16_pth} lacks features.{i}.{n}')
+                sd[f'{prefix}slice{s}.{i}.{n}'] = vgg[f'features.{i}.{n}']
+        return sd
+
+    def _net_struct(self):
+        net = _lib.DbwLpipsNet()
+        for i, c in enumerate(self._convs()):
+            net.conv_w[i], net.conv_b[i] = c.weight.data_ptr(), c.bias.data_ptr()
+        for k, w in enumerate(self._lins()):
+            net.lin_w[k] = w.data_ptr()
+        shift, scale = self._transform()
+        net.shift, net.scale = shift.data_ptr(), scale.data_ptr()
+        net.prepared = self.prepared.data_ptr()
+        return net
+
+    def _prepare(self):
+        """(re)write the TF32 forward and input-gradient weight copies when a weight tensor was replaced or modified"""
+        convs = self._convs()
+        params = [c.weight for c in convs] + [c.bias for c in convs] + self._lins() + list(self._transform())
+        key = tuple((p.data_ptr(), p._version) for p in params)
+        if key == self._prepared_key:
+            return
+        for p in params:
+            if not (p.is_cuda and p.dtype == torch.float32 and p.is_contiguous()):
+                raise DbwError(f'{type(self).__name__}: weights must be contiguous CUDA float32 tensors (call .cuda() on the module)')
+        ws, prep = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        check(_lib.lib().dbw_lpips_workspace_bytes(1, 16, 16, 0, ctypes.byref(ws), ctypes.byref(prep)), 'dbw_lpips_workspace_bytes')
+        dev = params[0].device
+        if self.prepared.numel() * 4 != prep.value or self.prepared.device != dev:
+            self.prepared = torch.empty(prep.value // 4, dtype=torch.float32, device=dev)
+        check(_lib.lib().dbw_lpips_prepare_weights(ctypes.byref(self._net_struct()), _stream(dev)), 'dbw_lpips_prepare_weights')
+        self._prepared_key = key
+
+    def _check_images(self, target, rendering, names, min_hw, why):
+        """target and rendering: (B,3,H,W) CUDA float32 images of one shape, H and W >= min_hw, target without a gradient"""
+        who = type(self).__name__
+        if target.requires_grad:
+            raise DbwError(f'{who}: {names[0]} requires a gradient; only {names[1]} (the rendering) is differentiated')
+        if not (torch.is_tensor(target) and torch.is_tensor(rendering) and target.is_cuda and rendering.is_cuda):
+            raise DbwError(f'{who}: expected CUDA tensors (there is no CPU fallback)')
+        if target.dtype != torch.float32 or rendering.dtype != torch.float32:
+            raise DbwError(f'{who}: expected float32 images, got {target.dtype} / {rendering.dtype}')
+        if target.shape != rendering.shape or rendering.dim() != 4 or rendering.shape[1] != 3:
+            raise DbwError(f'{who}: expected two (B,3,H,W) images of one shape, got {tuple(target.shape)} / {tuple(rendering.shape)}')
+        if min(rendering.shape[2:]) < min_hw:
+            raise DbwError(f'{who}: H and W must be >= {min_hw} {why}, got {tuple(rendering.shape[2:])}')
+
+
+class LPIPS(_Trunk):
     """lpips.LPIPS(net='vgg', version='0.1') with the lin-layer dropout lpips builds by default; forward(in0, in1,
     normalize=False) -> (B,1,1,1).  `in0` must not require a gradient.  Build it with `from_state_dict` or `from_files`;
     a bare LPIPS() has torchvision's default random initialisation (tests only)."""
@@ -170,8 +261,6 @@ class LPIPS(nn.Module):
             p.requires_grad_(False)
         # the dropout seed (uint32 bits in an int32), advanced on the device by every forward; not part of lpips's state
         self.register_buffer('seed', torch.zeros(1, dtype=torch.int32), persistent=False)
-        self.register_buffer('prepared', torch.zeros(0), persistent=False)
-        self._prepared_key = None
         self._target_cache = None
 
     # ------------------------------------------------------------------ construction
@@ -179,40 +268,23 @@ class LPIPS(nn.Module):
     def from_state_dict(cls, sd):
         """from an lpips-named state dict; a `perceptual_loss.loss.` or `module.` prefix is stripped.  Either of the
         `lin{k}` / `lins.{k}` spellings suffices.  Raises on a missing or misshapen key."""
-        sd = dict(sd)
-        for prefix in ('module.', 'perceptual_loss.loss.'):
-            if any(k.startswith(prefix) for k in sd):
-                sd = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
+        sd = _strip(sd, ('module.', 'perceptual_loss.loss.'))
         for k in range(5):
             a, b = f'lin{k}.model.1.weight', f'lins.{k}.model.1.weight'
             if a not in sd and b in sd:
                 sd[a] = sd[b]
             if b not in sd and a in sd:
                 sd[b] = sd[a]
-        shapes = state_dict_shapes()
-        missing = [k for k in shapes if k not in sd]
-        if missing:
-            raise KeyError(f'LPIPS.from_state_dict: missing keys {missing}')
-        bad = [(k, tuple(sd[k].shape), s) for k, s in shapes.items() if tuple(sd[k].shape) != s]
-        if bad:
-            raise ValueError(f'LPIPS.from_state_dict: misshapen keys (key, got, want) {bad}')
-        m = cls()
-        m.load_state_dict({k: sd[k] for k in shapes}, strict=True)
-        return m
+        return cls._load(sd, state_dict_shapes())
 
     @classmethod
     def from_files(cls, vgg16_pth, lin_pth):
         """from torchvision's vgg16 state dict (`features.N.weight` / `.bias`) and lpips's `weights/v0.1/vgg.pth`
         (`lin{k}.model.1.weight`)"""
-        vgg = torch.load(vgg16_pth, map_location='cpu', weights_only=True)
+        sd = cls._features(vgg16_pth, 'net.')
         lin = torch.load(lin_pth, map_location='cpu', weights_only=True)
-        sd = {'scaling_layer.shift': torch.tensor(SHIFT)[None, :, None, None],
-              'scaling_layer.scale': torch.tensor(SCALE)[None, :, None, None]}
-        for s, i, _, _ in CONVS:
-            for n in ('weight', 'bias'):
-                if f'features.{i}.{n}' not in vgg:
-                    raise KeyError(f'LPIPS.from_files: {vgg16_pth} lacks features.{i}.{n}')
-                sd[f'net.slice{s}.{i}.{n}'] = vgg[f'features.{i}.{n}']
+        sd.update({'scaling_layer.shift': torch.tensor(SHIFT)[None, :, None, None],
+                   'scaling_layer.scale': torch.tensor(SCALE)[None, :, None, None]})
         for k in range(5):
             key = f'lin{k}.model.1.weight'
             if key not in lin:
@@ -226,37 +298,14 @@ class LPIPS(nn.Module):
         check(_lib.lib().dbw_lpips_workspace_bytes(B, H, W, int(save), ctypes.byref(ws), ctypes.byref(prep)), 'dbw_lpips_workspace_bytes')
         return ws.value, prep.value
 
-    def _weights(self):
-        convs = self.net.convs()
-        return ([c.weight for c in convs], [c.bias for c in convs], [getattr(self, f'lin{k}').model[1].weight for k in range(5)])
+    def _convs(self):
+        return self.net.convs()
 
-    def _net_struct(self):
-        ws, bs, ls = self._weights()
-        net = _lib.DbwLpipsNet()
-        for i in range(13):
-            net.conv_w[i], net.conv_b[i] = ws[i].data_ptr(), bs[i].data_ptr()
-        for k in range(5):
-            net.lin_w[k] = ls[k].data_ptr()
-        net.shift, net.scale = self.scaling_layer.shift.data_ptr(), self.scaling_layer.scale.data_ptr()
-        net.prepared = self.prepared.data_ptr()
-        return net
+    def _transform(self):
+        return self.scaling_layer.shift, self.scaling_layer.scale
 
-    def _prepare(self):
-        """(re)write the TF32 forward and input-gradient weight copies when a weight tensor was replaced or modified"""
-        ws, bs, ls = self._weights()
-        params = ws + bs + ls + [self.scaling_layer.shift, self.scaling_layer.scale]
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if key == self._prepared_key:
-            return
-        for p in params:
-            if not (p.is_cuda and p.dtype == torch.float32 and p.is_contiguous()):
-                raise DbwError('LPIPS: weights must be contiguous CUDA float32 tensors (call .cuda() on the module)')
-        nbytes = self._bytes(1, 16, 16)[1]
-        if self.prepared.numel() * 4 != nbytes or self.prepared.device != ws[0].device:
-            self.prepared = torch.empty(nbytes // 4, dtype=torch.float32, device=ws[0].device)
-        check(_lib.lib().dbw_lpips_prepare_weights(ctypes.byref(self._net_struct()), _stream(ws[0].device)),
-              'dbw_lpips_prepare_weights')
-        self._prepared_key = key
+    def _lins(self):
+        return [getattr(self, f'lin{k}').model[1].weight for k in range(5)]
 
     # ------------------------------------------------------------------ target cache
     def target_cache_bytes(self, H, W, N=1):
@@ -310,16 +359,7 @@ class LPIPS(nn.Module):
         return c
 
     def forward(self, in0, in1, normalize=False):
-        if in0.requires_grad:
-            raise DbwError('LPIPS: in0 requires a gradient; only in1 (the rendering) is differentiated')
-        if not (in0.is_cuda and in1.is_cuda):
-            raise DbwError('LPIPS: expected CUDA tensors (there is no CPU fallback)')
-        if in0.dtype != torch.float32 or in1.dtype != torch.float32:
-            raise DbwError(f'LPIPS: expected float32 images, got {in0.dtype} / {in1.dtype}')
-        if in0.shape != in1.shape or in1.dim() != 4 or in1.shape[1] != 3:
-            raise DbwError(f'LPIPS: expected two (B,3,H,W) images of one shape, got {tuple(in0.shape)} / {tuple(in1.shape)}')
-        if min(in1.shape[2:]) < 16:
-            raise DbwError(f'LPIPS: H and W must be >= 16 (relu5_3 at least 1x1), got {tuple(in1.shape[2:])}')
+        self._check_images(in0, in1, ('in0', 'in1'), 16, '(relu5_3 at least 1x1)')
         self._prepare()
         # rec's activations are kept only when a backward can follow (not under no_grad, as in quantitative_eval)
         save = torch.is_grad_enabled() and in1.requires_grad
@@ -368,7 +408,7 @@ class _VggLossFunction(torch.autograd.Function):
         return None, grad, None, None
 
 
-class PerceptualLoss(nn.Module):
+class PerceptualLoss(_Trunk):
     """The reference's VGG16 feature-reconstruction loss (`PerceptualLoss`, src/model/loss.py:66-111; `perceptual_name:
     perceptual`) on the sm_90a kernels of csrc/dbw_lpips.cu.  forward(imgs, rec) -> scalar, differentiable in `rec` only:
     with `normalize_input`, (x - mean_rgb) / std_rgb; torchvision's VGG16 features only through the deepest of
@@ -402,39 +442,19 @@ class PerceptualLoss(nn.Module):
             self.add_module(f'slice{s}', getattr(vgg, f'slice{s}'))
         for p in self.parameters():
             p.requires_grad_(False)
-        self.register_buffer('prepared', torch.zeros(0), persistent=False)
-        self._prepared_key = None
 
     # ------------------------------------------------------------------ construction
     @classmethod
     def from_state_dict(cls, sd, **options):
         """from a state dict with the reference's names; a `perceptual_loss.` or `module.` prefix is stripped.  Raises on a
         missing or misshapen key."""
-        sd = dict(sd)
-        for prefix in ('module.', 'perceptual_loss.'):
-            if any(k.startswith(prefix) for k in sd):
-                sd = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
-        shapes = vgg_loss_state_dict_shapes()
-        missing = [k for k in shapes if k not in sd]
-        if missing:
-            raise KeyError(f'PerceptualLoss.from_state_dict: missing keys {missing}')
-        bad = [(k, tuple(sd[k].shape), s) for k, s in shapes.items() if tuple(sd[k].shape) != s]
-        if bad:
-            raise ValueError(f'PerceptualLoss.from_state_dict: misshapen keys (key, got, want) {bad}')
-        m = cls(**options)
-        m.load_state_dict({k: sd[k] for k in shapes}, strict=True)
-        return m
+        return cls._load(_strip(sd, ('module.', 'perceptual_loss.')), vgg_loss_state_dict_shapes(), **options)
 
     @classmethod
     def from_files(cls, vgg16_pth, **options):
         """from torchvision's vgg16 state dict (`features.N.weight` / `.bias`), the file LPIPS.from_files also reads"""
-        vgg = torch.load(vgg16_pth, map_location='cpu', weights_only=True)
-        sd = {'mean_rgb': torch.tensor(MEAN_RGB), 'std_rgb': torch.tensor(STD_RGB)}
-        for s, i, _, _ in CONVS:
-            for n in ('weight', 'bias'):
-                if f'features.{i}.{n}' not in vgg:
-                    raise KeyError(f'PerceptualLoss.from_files: {vgg16_pth} lacks features.{i}.{n}')
-                sd[f'slice{s}.{i}.{n}'] = vgg[f'features.{i}.{n}']
+        sd = cls._features(vgg16_pth, '')
+        sd.update({'mean_rgb': torch.tensor(MEAN_RGB), 'std_rgb': torch.tensor(STD_RGB)})
         return cls.from_state_dict(sd, **options)
 
     # ------------------------------------------------------------------ device plumbing
@@ -454,45 +474,12 @@ class PerceptualLoss(nn.Module):
     def _convs(self):
         return [getattr(getattr(self, f'slice{s}'), str(i)) for s, i, _, _ in CONVS]
 
-    def _net_struct(self):
-        net = _lib.DbwLpipsNet()
-        for i, c in enumerate(self._convs()):
-            net.conv_w[i], net.conv_b[i] = c.weight.data_ptr(), c.bias.data_ptr()
-        net.shift, net.scale = self.mean_rgb.data_ptr(), self.std_rgb.data_ptr()
-        net.prepared = self.prepared.data_ptr()
-        return net
-
-    def _prepare(self):
-        """(re)write the TF32 forward and input-gradient weight copies when a weight tensor was replaced or modified"""
-        convs = self._convs()
-        params = [c.weight for c in convs] + [c.bias for c in convs] + [self.mean_rgb, self.std_rgb]
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if key == self._prepared_key:
-            return
-        for p in params:
-            if not (p.is_cuda and p.dtype == torch.float32 and p.is_contiguous()):
-                raise DbwError('PerceptualLoss: weights must be contiguous CUDA float32 tensors (call .cuda() on the module)')
-        ws, prep = ctypes.c_size_t(0), ctypes.c_size_t(0)
-        check(_lib.lib().dbw_lpips_workspace_bytes(1, 16, 16, 0, ctypes.byref(ws), ctypes.byref(prep)), 'dbw_lpips_workspace_bytes')
-        dev = params[0].device
-        if self.prepared.numel() * 4 != prep.value or self.prepared.device != dev:
-            self.prepared = torch.empty(prep.value // 4, dtype=torch.float32, device=dev)
-        check(_lib.lib().dbw_lpips_prepare_weights(ctypes.byref(self._net_struct()), _stream(dev)), 'dbw_lpips_prepare_weights')
-        self._prepared_key = key
+    def _transform(self):
+        return self.mean_rgb, self.std_rgb
 
     def per_image(self, imgs, rec):
         """(B,) float32: each image's value, whose batch mean forward() returns"""
-        if imgs.requires_grad:
-            raise DbwError('PerceptualLoss: imgs requires a gradient; only rec (the rendering) is differentiated')
-        if not (torch.is_tensor(imgs) and torch.is_tensor(rec) and imgs.is_cuda and rec.is_cuda):
-            raise DbwError('PerceptualLoss: expected CUDA tensors (there is no CPU fallback)')
-        if imgs.dtype != torch.float32 or rec.dtype != torch.float32:
-            raise DbwError(f'PerceptualLoss: expected float32 images, got {imgs.dtype} / {rec.dtype}')
-        if imgs.shape != rec.shape or rec.dim() != 4 or rec.shape[1] != 3:
-            raise DbwError(f'PerceptualLoss: expected two (B,3,H,W) images of one shape, got {tuple(imgs.shape)} / {tuple(rec.shape)}')
-        if min(rec.shape[2:]) < 2 ** (self.max_level - 1):
-            raise DbwError(f'PerceptualLoss: H and W must be >= {2 ** (self.max_level - 1)} for level {self.max_level}, '
-                           f'got {tuple(rec.shape[2:])}')
+        self._check_images(imgs, rec, ('imgs', 'rec'), 2 ** (self.max_level - 1), f'for level {self.max_level}')
         self._prepare()
         # rec's activations are kept only when a backward can follow (not under no_grad)
         save = torch.is_grad_enabled() and rec.requires_grad

@@ -30,7 +30,7 @@ eta = 2^-150, every bound evaluated in float64 from the same float32 operands an
   plain_head_bwd  k = 2w (gv / HW): 2w is exact, gv / HW and the product one rounding each; k (u1 - f0) adds one for the
                   difference and one for the product; the accumulate (or the FMA it may be fused into) one of the result.
                   Bound 2 (4u |k (u1 - f0)| + u |k (u1 - f0) + g_in| + eta), then * [u1 > 0], exact.
-  vgg_value       vgg_reduce_kernel: each requested level's partials summed in chunk order (chunks_k - 1 roundings), the fp32
+  vgg_value       lpips_reduce_kernel: each requested level's partials summed in chunk order (chunks_k - 1 roundings), the fp32
                   1 / (H_k W_k) and the product (2), the levels in order (up to 5): tests/test_lpips_matrix_gpu.py's value
                   bound 2 (chunks_k + 7) u sum_k sum_c |partial_c| / (H_k W_k) over the requested levels.
 
