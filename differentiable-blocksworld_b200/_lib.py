@@ -78,6 +78,17 @@ class DbwAdamGroup(ctypes.Structure):
 ADAM_MAX_SEGMENTS, ADAM_MAX_GROUPS = 64, 8
 
 
+class DbwRegularisers(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ('texture_bkg', 'texture_ground', 'textures', 'S', 'R_6d', 'T', 'sq_eps',
+                                               'alpha_full', 'unit_samples')] \
+             + [(n, ctypes.c_int32) for n in ('n_blocks', 'n_points', 'env_size', 'txt_size', 'terms', 'tv_norm', 'coarse')] \
+             + [(n, ctypes.c_float) for n in ('ratio_block_scene', 'scale_min', 'w_parsimony', 'w_tv', 'w_overlap')]
+
+
+REG_PARSIMONY, REG_TV, REG_OVERLAP = 1, 2, 4                  # DBW_REG_* of include/dbw_render.h
+REG_TV_NORMS = {'l2': 0, 'l1': 1, 'l2sq': 2}                  # DBW_REG_TV_NORM_*
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -99,7 +110,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generi
            'dbw_lpips_cache_bytes', 'dbw_lpips_cache_targets', 'dbw_lpips_forward_cached', 'dbw_lpips_backward_cached',
            'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward', 'dbw_vgg_head_forward',
            'dbw_vgg_head_backward',
-           'dbw_adam_step', 'dbw_viz_workspace_bytes', 'dbw_render_forward_viz']
+           'dbw_adam_step', 'dbw_viz_workspace_bytes', 'dbw_render_forward_viz',
+           'dbw_regularisers_workspace_bytes', 'dbw_regularisers_forward', 'dbw_regularisers_backward']
 
 _lib = None
 
@@ -193,6 +205,10 @@ def lib():
         L.dbw_vgg_head_forward.argtypes = [vp, vp, ctypes.c_float, i64, i32, i32, i32, vp, vp]
         L.dbw_vgg_head_backward.argtypes = [vp, vp, ctypes.c_float, i64, i32, i32, i32, vp, i32, vp, vp]
         L.dbw_adam_step.argtypes = [vp, i32, i64, ctypes.POINTER(DbwAdamGroup), i32, vp, vp, vp]
+        rp = ctypes.POINTER(DbwRegularisers)
+        L.dbw_regularisers_workspace_bytes.argtypes = [rp, ctypes.POINTER(sz)]
+        L.dbw_regularisers_forward.argtypes = [rp] + [vp] * 4 + [sz, vp]
+        L.dbw_regularisers_backward.argtypes = [rp] + [vp] * 12 + [sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

@@ -101,7 +101,8 @@ class DifferentiableBlocksWorld(nn.Module):
                                                           'scale_weight', 'tv_weight', 'overlap_weight')}
         self.loss_weights = {k: w for k, w in weights.items() if w > 0}
         self.loss_names = [f'loss_{k}' for k in self.loss_weights] + ['loss_total']
-        self.tv_norm = L.TV_NORMS[loss['tv_type']]
+        self.tv_type = loss['tv_type']
+        self.tv_norm = L.TV_NORMS[self.tv_type]
         self.criterion = {'mse': nn.MSELoss, 'l2': nn.MSELoss, 'l1': nn.L1Loss}[loss['name']]()
         if 'perceptual' in self.loss_weights:
             # LPIPS is a VGG16 conv network (cuDNN / tensor cores): outside the render hot path (SURVEY 8a row a13);
@@ -642,7 +643,8 @@ class DifferentiableBlocksWorld(nn.Module):
     def compute_losses(self, imgs, rec, rgb_loss=None):
         coarse = self.is_live('coarse_learning')
         w = self.loss_weights
-        if 'tv' in w or 'overlap' in w:
+        on_device = self.textures.is_cuda          # the regularisers run in the library's kernels, from the leaves
+        if ('tv' in w or 'overlap' in w) and not on_device:
             self._refresh_reg_state()
         terms = {}
         if 'rgb' in w:
@@ -650,6 +652,11 @@ class DifferentiableBlocksWorld(nn.Module):
             terms['rgb'] = rgb if w['rgb'] == 1 else w['rgb'] * rgb
         if 'perceptual' in w and self.perceptual_loss is not None:
             terms['perceptual'] = w['perceptual'] * (1 if coarse else 0.1) * self.perceptual_loss(imgs, rec)
+        if on_device and any(k in w for k in ('parsimony', 'tv', 'overlap')):
+            terms.update(L.regularisers(self.texture_bkg, self.texture_ground, self.textures, self.S, self.R_6d, self.T, self.sq_eps,
+                                        self._alpha_full, w, self.tv_type, coarse, self.ratio_block_scene, self.scale_min,
+                                        generator=self.noise_generator, unit_samples=self.overlap_samples_buffer))
+            return self._total(terms, imgs)
         if 'parsimony' in w:
             terms['parsimony'] = w['parsimony'] * L.parsimony(self._alpha_full, coarse)
         if 'tv' in w:
@@ -658,6 +665,10 @@ class DifferentiableBlocksWorld(nn.Module):
             S, R, T = self._blocks_SRT
             terms['overlap'] = w['overlap'] * L.overlap(S, R, T, *self._blocks_eps, self._alpha_full, self.ratio_block_scene,
                                                         coarse, generator=self.noise_generator, unit_samples=self.overlap_samples_buffer)
+        return self._total(terms, imgs)
+
+    def _total(self, terms, imgs):
+        w = self.loss_weights
         vals = list(terms.values())
         total = vals[0] if vals else torch.zeros((), device=imgs.device)
         for v in vals[1:]:

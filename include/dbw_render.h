@@ -694,6 +694,61 @@ typedef struct DbwAdamGroup { double beta1, beta2, eps, weight_decay; } DbwAdamG
 int dbw_adam_step(const DbwAdamSegment* segments, int32_t n_segments, int64_t n_total, const DbwAdamGroup* groups,
                   int32_t n_groups, const float* lr, int64_t* step, void* stream);
 
+/*
+ * Regularisers: the parameter-only terms of the objective (src/model/dbw.py:373-405), each multiplied by its weight, straight
+ * from the leaf parameters:
+ *   parsimony  w_p  * mean_k safe_pow(alpha_full_k, 0.5)                                   (coarse phase only)
+ *   tv         w_tv * f * (TV(bkg) + TV_u-periodic(blocks) + f TV(ground)),  f = 1 coarse, 0.1 fine; TV of a stack of maps
+ *              sigmoid(logits) = mean of the norm of the v differences + mean of the norm of the u differences (the blocks'
+ *              sums over blocks first, then means over one map)
+ *   overlap    w_ov * mean_points clamp(sum_k sigmoid(-sdf_k(point) / 0.005) alpha_full_k - 1.95, min=0)      (coarse only)
+ *              with the points ((2 u - 1) ratio S_b) R_b + T_b of every block b from `unit_samples`, and sdf_k the as_sdf=2
+ *              superquadric implicit in block k's frame; S = exp(S) + scale_min, R = rotation_6d_to_matrix(R_6d),
+ *              (e1, e2) = sigmoid(sq_eps) * 1.8 + 0.1.  The points carry no gradient.
+ * The sigmoid texture maps are never materialised.  A term is on when its bit is set in `terms`.
+ *
+ * Deterministic (no float atomics: per-CTA partials summed in a fixed order) and capturable (no allocation, no host read).
+ * Forward: 2 launches.  Backward: at most 2 (1 when only tv is on).  The workspace is caller-owned device memory of at least
+ * the size dbw_regularisers_workspace_bytes returns; forward and backward of one call may share it.
+ *
+ *   out_*   DEVICE fp32 scalars, written for the terms that are on (the others may be null).
+ *   g_out_* DEVICE fp32 upstream gradients of the three outputs, read on the device (null for terms that are off).
+ *   g_*     DEVICE fp32 gradients of the leaves, WRITTEN (not accumulated): g_texture_* (full resolution) when tv is on,
+ *           g_S, g_R_6d, g_T, g_sq_eps when overlap is on, g_alpha_full when parsimony or overlap is on.  Any may be null: it
+ *           is then not written.
+ */
+#define DBW_REG_PARSIMONY 1
+#define DBW_REG_TV 2
+#define DBW_REG_OVERLAP 4
+#define DBW_REG_TV_NORM_L2 0
+#define DBW_REG_TV_NORM_L1 1
+#define DBW_REG_TV_NORM_L2SQ 2
+typedef struct DbwRegularisers {
+  const float* texture_bkg;      /* (env_size, env_size, 3) logits                                                          */
+  const float* texture_ground;   /* (env_size, env_size, 3) logits                                                          */
+  const float* textures;         /* (n_blocks, txt_size, txt_size, 3) logits                                                */
+  const float* S;                /* (n_blocks, 3) log-scales                                                                */
+  const float* R_6d;             /* (n_blocks, 6)                                                                           */
+  const float* T;                /* (n_blocks, 3)                                                                           */
+  const float* sq_eps;           /* (n_blocks, 2) exponent logits                                                           */
+  const float* alpha_full;       /* (n_blocks) opacities as the opacity path hands them over (kills folded in)              */
+  const float* unit_samples;     /* (n_blocks, n_points, 3) U(0,1) draws                                                    */
+  int32_t n_blocks, n_points, env_size, txt_size;
+  int32_t terms;                 /* DBW_REG_* bits                                                                          */
+  int32_t tv_norm;               /* DBW_REG_TV_NORM_*                                                                       */
+  int32_t coarse;                /* 1: coarse phase (tv factor 1), 0: fine (factor 0.1)                                     */
+  float ratio_block_scene, scale_min;
+  float w_parsimony, w_tv, w_overlap;
+} DbwRegularisers;
+
+int dbw_regularisers_workspace_bytes(const DbwRegularisers* r, size_t* bytes);
+int dbw_regularisers_forward(const DbwRegularisers* r, float* out_parsimony, float* out_tv, float* out_overlap, void* workspace,
+                             size_t workspace_bytes, void* stream);
+int dbw_regularisers_backward(const DbwRegularisers* r, const float* g_out_parsimony, const float* g_out_tv,
+                              const float* g_out_overlap, float* g_texture_bkg, float* g_texture_ground, float* g_textures,
+                              float* g_S, float* g_R_6d, float* g_T, float* g_sq_eps, float* g_alpha_full, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
