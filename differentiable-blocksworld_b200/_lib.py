@@ -89,6 +89,15 @@ REG_PARSIMONY, REG_TV, REG_OVERLAP = 1, 2, 4                  # DBW_REG_* of inc
 REG_TV_NORMS = {'l2': 0, 'l1': 1, 'l2sq': 2}                  # DBW_REG_TV_NORM_*
 
 
+class DbwPhongShading(ctypes.Structure):
+    _fields_ = [('light', ctypes.c_int32)] + [(n, ctypes.c_float * 3) for n in ('ambient_color', 'diffuse_color', 'specular_color',
+                                                                               'direction', 'ka', 'kd', 'ks')] \
+             + [('shininess', ctypes.c_float)]
+
+
+LIGHTS = {'ambient': 0, 'directional': 1, 'point': 2}        # DBW_LIGHT_* of include/dbw_render.h
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -111,7 +120,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generi
            'dbw_vgg_loss_workspace_bytes', 'dbw_vgg_loss_forward', 'dbw_vgg_loss_backward', 'dbw_vgg_head_forward',
            'dbw_vgg_head_backward',
            'dbw_adam_step', 'dbw_viz_workspace_bytes', 'dbw_render_forward_viz',
-           'dbw_regularisers_workspace_bytes', 'dbw_regularisers_forward', 'dbw_regularisers_backward']
+           'dbw_regularisers_workspace_bytes', 'dbw_regularisers_forward', 'dbw_regularisers_backward',
+           'dbw_vertex_face_list', 'dbw_vertex_normals', 'dbw_render_forward_phong']
 
 _lib = None
 
@@ -209,6 +219,10 @@ def lib():
         L.dbw_regularisers_workspace_bytes.argtypes = [rp, ctypes.POINTER(sz)]
         L.dbw_regularisers_forward.argtypes = [rp] + [vp] * 4 + [sz, vp]
         L.dbw_regularisers_backward.argtypes = [rp] + [vp] * 12 + [sz, vp]
+        L.dbw_vertex_face_list.argtypes = [vp, i32, i32, vp, vp, vp]
+        L.dbw_vertex_normals.argtypes = [vp, vp, i32, vp, vp, vp, vp]
+        L.dbw_render_forward_phong.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [ctypes.POINTER(DbwPhongShading), i32, vp, i32,
+                                                                                          vp, vp, vp, sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

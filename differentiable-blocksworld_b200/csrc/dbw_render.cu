@@ -31,6 +31,7 @@
 #include "dbw_fraglist.cuh"
 #include "dbw_camera.cuh"
 #include "dbw_viz_math.cuh"
+#include "dbw_shade_math.cuh"
 
 // ------------------------------------------------------------------------------------------------ error plumbing
 static thread_local char g_err[512] = "";
@@ -1147,8 +1148,61 @@ __device__ __forceinline__ HardShade hard_shade(const RasterParams& P, const int
   return w;
 }
 
-template <bool VIZ>
-__device__ __forceinline__ void hard_forward_body(const RasterParams& P, const VizOut& Z) {
+// Inputs of the Phong-shaded variants (dbw_render_forward_phong): a kernel argument of their own, so that RasterParams -- and
+// with it every other kernel -- is unchanged.
+struct PhongIn {
+  const float* verts;        // (V,3) world-space vertices
+  const float* normals;      // (V,3) vertex normals (dbw_vertex_normals)
+  const int* faces;          // (F,3)
+  const float* R; const float* T;   // (B,3,3), (B,3): the per-view light direction and camera centre
+  DbwPhongShading light;
+};
+// hard_shade with the texel Phong-shaded: vertex normal and world position interpolated with the same barycentrics bu as the
+// texture coordinates.  A copy of hard_shade rather than a branch in it, so that the existing kernels keep their code.
+__device__ __forceinline__ HardShade hard_shade_phong(const RasterParams& P, const PhongIn& L, const int4* s_desc, int view,
+                                                      int best_slot, f3 best_bc) {
+  const size_t gs = (size_t)view * 2 * P.F + best_slot;
+  f3 bu = best_bc;
+  if (__float_as_int(__ldg(&P.rec[gs * 4 + 2]).w) & 1) {
+    const float* cv = P.conv + gs * 9;
+    bu.x = best_bc.x * cv[0] + best_bc.y * cv[3] + best_bc.z * cv[6];
+    bu.y = best_bc.x * cv[1] + best_bc.y * cv[4] + best_bc.z * cv[7];
+    bu.z = best_bc.x * cv[2] + best_bc.y * cv[5] + best_bc.z * cv[8];
+  }
+  const float4 q0 = __ldg(&P.rec2[gs * 2]), q1 = __ldg(&P.rec2[gs * 2 + 1]);
+  HardShade w;
+  w.u = bu.x * q0.x + bu.y * q0.z + bu.z * q1.x;
+  w.v = bu.x * q0.y + bu.y * q0.w + bu.z * q1.y;
+  w.map_id = __float_as_int(q1.z);
+  Texel4 tx;
+  fetch_color(P, w.u, w.v, s_desc[w.map_id], tx);
+  const int face = best_slot >= P.F ? best_slot - P.F : best_slot;
+  w.a = 1.f;
+  if (P.faces_alpha) w.a *= __ldg(&P.faces_alpha[alpha_index(P, view, face)]);
+  const int i0 = __ldg(L.faces + 3 * face), i1 = __ldg(L.faces + 3 * face + 1), i2 = __ldg(L.faces + 3 * face + 2);
+  DbwVec3 n, p;
+  n.x = bu.x * __ldg(L.normals + 3 * i0) + bu.y * __ldg(L.normals + 3 * i1) + bu.z * __ldg(L.normals + 3 * i2);
+  n.y = bu.x * __ldg(L.normals + 3 * i0 + 1) + bu.y * __ldg(L.normals + 3 * i1 + 1) + bu.z * __ldg(L.normals + 3 * i2 + 1);
+  n.z = bu.x * __ldg(L.normals + 3 * i0 + 2) + bu.y * __ldg(L.normals + 3 * i1 + 2) + bu.z * __ldg(L.normals + 3 * i2 + 2);
+  p.x = bu.x * __ldg(L.verts + 3 * i0) + bu.y * __ldg(L.verts + 3 * i1) + bu.z * __ldg(L.verts + 3 * i2);
+  p.y = bu.x * __ldg(L.verts + 3 * i0 + 1) + bu.y * __ldg(L.verts + 3 * i1 + 1) + bu.z * __ldg(L.verts + 3 * i2 + 1);
+  p.z = bu.x * __ldg(L.verts + 3 * i0 + 2) + bu.y * __ldg(L.verts + 3 * i1 + 2) + bu.z * __ldg(L.verts + 3 * i2 + 2);
+  float Rv[9], Tv[3];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) Rv[k] = __ldg(L.R + 9 * view + k);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) Tv[k] = __ldg(L.T + 3 * view + k);
+  DbwVec3 light, camera;
+  shade_view_setup(L.light, Rv, Tv, light, camera);
+  const DbwVec3 c = shade_phong(L.light, shade_v3(tx.color.x, tx.color.y, tx.color.z), n, p, light, camera);
+  w.color.x = c.x; w.color.y = c.y; w.color.z = c.z;
+  return w;
+}
+
+// PHONG: the Phong-shaded variants (phong_hard_forward_kernel, phong_resolve_hard_viz_kernel), which shade the winner with
+// hard_shade_phong; the code of the other instantiations is unchanged.
+template <bool VIZ, bool PHONG = false>
+__device__ __forceinline__ void hard_forward_body(const RasterParams& P, const VizOut& Z, const PhongIn& L = PhongIn{}) {
   __shared__ float4 s_bbox[HARD_CAP];
   __shared__ float4 s_rec[HARD_CAP * 4];
   __shared__ int s_slot[HARD_CAP];
@@ -1233,7 +1287,7 @@ __device__ __forceinline__ void hard_forward_body(const RasterParams& P, const V
     // every lane takes part in the resolve's shuffles: a sample outside the image belongs to a frame pixel outside it
     float c[4] = {P.bg0, P.bg1, P.bg2, 0.f};
     if (live && best_j >= 0) {
-      const HardShade w = hard_shade(P, s_desc, view, best_slot, best_bc);
+      const HardShade w = PHONG ? hard_shade_phong(P, L, s_desc, view, best_slot, best_bc) : hard_shade(P, s_desc, view, best_slot, best_bc);
       const float occ = 1.f - w.a;
       c[0] = w.a * w.color.x + occ * P.bg0; c[1] = w.a * w.color.y + occ * P.bg1; c[2] = w.a * w.color.z + occ * P.bg2; c[3] = w.a;
     }
@@ -1248,6 +1302,14 @@ __device__ __forceinline__ void hard_forward_body(const RasterParams& P, const V
     o[0] = P.bg0; o[plane] = P.bg1; o[2 * plane] = P.bg2; o[3 * plane] = 0.f;
     if (P.nfrag) P.nfrag[(size_t)view * plane + pix] = 0;
     if (P.topk) P.topk[(size_t)view * plane + pix] = -1;
+    return;
+  }
+  if constexpr (PHONG) {         // no fragment records: a phong render has no backward
+    const HardShade w = hard_shade_phong(P, L, s_desc, view, best_slot, best_bc);
+    if (P.topk) P.topk[(size_t)view * plane + pix] = best_slot;
+    const float occ = 1.f - w.a;
+    o[0] = w.a * w.color.x + occ * P.bg0; o[plane] = w.a * w.color.y + occ * P.bg1; o[2 * plane] = w.a * w.color.z + occ * P.bg2;
+    o[3 * plane] = w.a;
     return;
   }
   // texture coordinates of the winner (its record is read back from global memory: the tile list may have been recycled)
@@ -1289,6 +1351,14 @@ __global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const R
 // The resolving variant renders the VizMeshRenderer frame (hard render on the 4H x 4W sample grid, avg_pool2d(., 4)) without
 // the sample image: a warp's 8 x 4 samples are the 4 x 4 samples of two frame pixels, which its lanes sum in registers.
 __global__ void __launch_bounds__(HARD_NT, 5) resolve_hard_viz_kernel(const RasterParams P, const VizOut Z) { hard_forward_body<true>(P, Z); }
+
+// Phong-shaded hard render (dbw_render_forward_phong, factor 1) and its resolving variant (factor 4)
+__global__ void __launch_bounds__(HARD_NT, 5) phong_hard_forward_kernel(const RasterParams P, const PhongIn L) {
+  hard_forward_body<false, true>(P, VizOut{}, L);
+}
+__global__ void __launch_bounds__(HARD_NT, 5) phong_resolve_hard_viz_kernel(const RasterParams P, const VizOut Z, const PhongIn L) {
+  hard_forward_body<true, true>(P, Z, L);
+}
 
 // The 16 samples of a frame pixel are lanes (g + c) + 8 r, r, c in [0, 4), g = 0 or 4.  Each sum runs in avg_pool2d's order
 // (dbw_viz_math.cuh), so the frame equals avg_pool2d(render at 4H x 4W, 4) bit for bit.
@@ -2127,7 +2197,8 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream, const EpilogueGrad* eg = nullptr, const VizOut* viz = nullptr);
+                               void* stream, const EpilogueGrad* eg = nullptr, const VizOut* viz = nullptr,
+                               const PhongIn* phong = nullptr);
 
 extern "C" int dbw_render_forward(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                   const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
@@ -2179,7 +2250,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream, const EpilogueGrad* eg, const VizOut* viz) {
+                               void* stream, const EpilogueGrad* eg, const VizOut* viz, const PhongIn* phong) {
   if (validate(s)) return -1;
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || (!out_rgba && !eg && !viz) || !workspace)
     return fail("dbw_render_forward: null pointer argument");
@@ -2237,7 +2308,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   {
     ScopedTimer timer(0, K, st);
     // a hard single-layer render without distances has its own kernel (dbw_debug_generic_kernel_only(1): the generic one)
-    const bool hard = viz || (K == 1 && s->sigma == 0.f && s->blur_radius == 0.f && !out_dists && !ep && !g_no_hard_kernel);
+    const bool hard = viz || phong || (K == 1 && s->sigma == 0.f && s->blur_radius == 0.f && !out_dists && !ep && !g_no_hard_kernel);
     if (!hard && w.cbin_list) {
       coarse_bin_kernel<<<dim3(B, w.cbin_nx * w.cbin_ny), 256, 0, st>>>(w.bbox, w.view_flags, F, s->height, s->width, w.cbin_nx,
                                                                         w.cbin_ny, w.cbin_count, w.cbin_list);
@@ -2247,7 +2318,9 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
     }
     if (hard) {
       const dim3 grid(P.B, (P.W + 15) / 16, (P.H + 15) / 16);
-      if (viz) resolve_hard_viz_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *viz);
+      if (phong && viz) phong_resolve_hard_viz_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *viz, *phong);
+      else if (phong) phong_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *phong);
+      else if (viz) resolve_hard_viz_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *viz);
       else raster_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P);
     } else {
       // the coarse phase's blocks loss pass (K > 4) has a kernel of its own; anything it does not serve takes the generic one
@@ -2301,6 +2374,39 @@ extern "C" int dbw_render_forward_viz(const DbwRenderSettings* s, const float* v
   const VizOut viz = {bkg, bkg && bkg_views > 1 ? (int)(3 * plane) : 0, out_rgba, out_rgb8};
   return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, nullptr, nullptr,
                              workspace, workspace_bytes, face_shade, nullptr, nullptr, stream, nullptr, &viz);
+}
+
+// ------------------------------------------------------------------------------------------------ phong hard render
+extern "C" int dbw_render_forward_phong(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
+                                        const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
+                                        const float* T, const float* faces_alpha, const float* verts_world, const float* normals,
+                                        const DbwPhongShading* shading, int32_t factor, const float* bkg, int32_t bkg_views,
+                                        float* out_rgba, uint8_t* out_rgb8, void* workspace, size_t workspace_bytes, void* stream) {
+  if (validate(s)) return -1;
+  const char* why = nullptr;
+  if (factor == 1) {
+    if (s->faces_per_pixel != 1 || s->sigma != 0.f || s->blur_radius != 0.f) why = "a hard render needs faces_per_pixel = 1, sigma = 0, blur_radius = 0";
+    else if (s->save_fragment_state) why = "no fragment records are written (save_fragment_state must be 0)";
+    else if (bkg || out_rgb8) why = "bkg and out_rgb8 belong to factor 4";
+    else if (!out_rgba) why = "null out_rgba";
+  } else {
+    why = viz_unsupported(*s, factor);
+    if (!why && !out_rgba && !out_rgb8) why = "out_rgba and out_rgb8 are both NULL";
+    if (!why && bkg && bkg_views != 1 && bkg_views != s->n_views) why = "bkg_views must be 1 or n_views";
+  }
+  if (!why && !shading) why = "null shading";
+  if (!why && (shading->light < DBW_LIGHT_AMBIENT || shading->light > DBW_LIGHT_POINT)) why = "unknown light type";
+  if (!why && (!verts_world || !normals || !R || !T)) why = "verts_world, normals, R and T are required";
+  if (why) { char msg[192]; snprintf(msg, sizeof(msg), "dbw_render_forward_phong: %s", why); return fail(msg); }
+  const PhongIn phong = {verts_world, normals, faces, R, T, *shading};
+  if (factor == 1)
+    return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, out_rgba, nullptr,
+                               workspace, workspace_bytes, nullptr, nullptr, nullptr, stream, nullptr, nullptr, &phong);
+  const size_t plane = (size_t)(s->height / factor) * (s->width / factor);
+  if (3 * plane > (size_t)INT32_MAX) return fail("dbw_render_forward_phong: frame too large");
+  const VizOut viz = {bkg, bkg && bkg_views > 1 ? (int)(3 * plane) : 0, out_rgba, out_rgb8};
+  return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, nullptr, nullptr,
+                             workspace, workspace_bytes, nullptr, nullptr, nullptr, stream, nullptr, &viz, &phong);
 }
 
 // adds the cell-gradient copies of the backward scratch into g_maps, times *scale (NULL = 1)

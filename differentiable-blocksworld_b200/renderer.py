@@ -2,7 +2,10 @@
 `forward(meshes, R, T, viz_purpose=False, **kwargs) -> (B,4,H,W)`, same `update_cameras(device=, K=)` /
 `.cameras.K` probe (src/model/dbw.py:204-208) -- but the whole MeshRasterizer + LayeredShader + layered_rgb_blend
 stack behind it is ONE pair of hand-written sm_90a kernels reached through the C-ABI of include/dbw_render.h.
-There is no CPU / PyTorch fallback: a missing library or a non-CUDA tensor raises."""
+There is no CPU / PyTorch fallback: a missing library or a non-CUDA tensor raises.
+Shading types: 'raw' with ambient lights (training), 'flat' with a directional light (renderer_light), and 'phong' with
+ambient, directional or point lights for hard single-layer renders (sigma 0, faces_per_pixel 1, and every viz_purpose
+render); soft phong, gouraud and any backward through a lit render raise NotImplementedError."""
 import ctypes
 from copy import deepcopy
 
@@ -12,7 +15,7 @@ from torch import nn
 from torch.nn import functional as F
 
 from . import _lib
-from ._lib import DbwMapDesc, DbwRenderSettings, DbwError
+from ._lib import DbwMapDesc, DbwRenderSettings, DbwError, DbwPhongShading
 
 LAYERED_SHADER = True
 SHADING_TYPE = 'raw'
@@ -372,6 +375,125 @@ def render_scene_viz(verts, faces, faces_uvs, face_map, maps, map_table_host, R,
     return (rgba, rgb8) if frames_u8 else rgba
 
 
+# ------------------------------------------------------------------ phong shading
+# PyTorch3D's defaults: DirectionalLights / PointLights, AmbientLights (white), Materials (the reference passes none)
+LIGHT_DEFAULTS = {'ambient_color': (0.5, 0.5, 0.5), 'diffuse_color': (0.3, 0.3, 0.3), 'specular_color': (0.2, 0.2, 0.2),
+                  'direction': (0., 1., 0.), 'location': (0., 1., 0.)}
+AMBIENT_LIGHT_COLOR = (1., 1., 1.)
+MATERIAL_DEFAULTS = {'ambient_color': (1., 1., 1.), 'diffuse_color': (1., 1., 1.), 'specular_color': (1., 1., 1.), 'shininess': 64.}
+
+
+def phong_shading(lights=None, materials=None):
+    """DbwPhongShading of PyTorch3D lights given as the reference's Renderer takes them ({'name': 'ambient' | 'directional' |
+    'point', colours, direction / location}, one light) and of Materials kwargs (ambient_color, diffuse_color, specular_color,
+    shininess), each defaulting as in PyTorch3D"""
+    lights, materials = dict(lights or {}), dict(materials or {})
+    name = lights.pop('name', 'ambient')
+    if name not in _lib.LIGHTS:
+        raise NotImplementedError(f'lights name={name!r}: only ambient, directional and point lights are implemented')
+    vec = lambda v: [float(x) for x in (v.detach().cpu() if torch.is_tensor(v) else torch.tensor(v, dtype=torch.float64)).reshape(-1, 3)[0]]
+    sh = DbwPhongShading()
+    sh.light = _lib.LIGHTS[name]
+    defaults = dict(LIGHT_DEFAULTS, ambient_color=AMBIENT_LIGHT_COLOR) if name == 'ambient' else LIGHT_DEFAULTS
+    for k in ('ambient_color', 'diffuse_color', 'specular_color'):
+        getattr(sh, k)[:] = vec(lights.get(k, defaults[k])) if name != 'ambient' or k == 'ambient_color' else [0., 0., 0.]
+    sh.direction[:] = vec(lights.get('location' if name == 'point' else 'direction', defaults['direction']))
+    for field, k in (('ka', 'ambient_color'), ('kd', 'diffuse_color'), ('ks', 'specular_color')):
+        getattr(sh, field)[:] = vec(materials.get(k, MATERIAL_DEFAULTS[k]))
+    sh.shininess = float(materials.get('shininess', MATERIAL_DEFAULTS['shininess']))
+    return sh
+
+
+def vertex_face_list(faces, n_verts):
+    """(vf_end (V), vf_faces (3F)) int32: the faces of vertex v, in ascending order, are vf_faces[vf_end[v-1] : vf_end[v]]
+    (dbw_vertex_face_list).  faces (F,3) int32 on the device."""
+    faces = faces.to(torch.int32).contiguous()
+    vf_end = torch.empty(n_verts, dtype=torch.int32, device=faces.device)
+    vf_faces = torch.empty(faces.numel(), dtype=torch.int32, device=faces.device)
+    _lib.check(_lib.lib().dbw_vertex_face_list(_c(faces), faces.shape[0], n_verts, _c(vf_end), _c(vf_faces), _stream()),
+               'dbw_vertex_face_list')
+    return vf_end, vf_faces
+
+
+@torch.no_grad()
+def vertex_normals(verts, faces, vf=None):
+    """Meshes.verts_normals_packed of one mesh: (V,3) unit area-weighted vertex normals (eps 1e-6), summed in a fixed order
+    (bit-reproducible).  vf: vertex_face_list(faces, V), built here when not given."""
+    if not verts.is_cuda:
+        raise DbwError('the CUDA renderer needs CUDA tensors (there is no CPU fallback)')
+    verts, faces = verts.detach().contiguous().float(), faces.to(torch.int32).contiguous()
+    vf_end, vf_faces = vertex_face_list(faces, verts.shape[0]) if vf is None else vf
+    out = torch.empty_like(verts)
+    _lib.check(_lib.lib().dbw_vertex_normals(_c(verts), _c(faces), verts.shape[0], _c(vf_end), _c(vf_faces), _c(out), _stream()),
+               'dbw_vertex_normals')
+    return out
+
+
+class _PhongFn(torch.autograd.Function):
+    """a phong render (dbw_render_forward_phong) in the autograd graph: its backward refuses, as the flat-shaded one does"""
+
+    @staticmethod
+    def forward(ctx, verts, maps, faces_alpha, R, T, run):
+        return run()
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise NotImplementedError('phong-shaded renders are a visualisation path: no backward')
+
+
+def render_scene_phong(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, intr, image_size, shading, factor=1,
+                       z_clip=None, detach_bary=False, clip_inside=True, background=(0., 0., 0.), faces_alpha=None,
+                       perspective_correct=True, bkg=None, frames_u8=False, normals=None):
+    """The hard single-layer render (faces_per_pixel 1, sigma 0) with every pixel Phong-shaded (dbw_render_forward_phong).
+    Arguments as render_scene; shading: a DbwPhongShading (phong_shading()); normals: vertex_normals(verts, faces), computed
+    here when None.  factor 1: rgba (B,4,H,W) of image_size.  factor 4: render_scene_viz's frames of image_size (the render
+    at 4H x 4W resolved 4x4 in the kernel), with bkg and frames_u8 as there.  No gradient: a backward raises."""
+    if factor not in (1, 4):
+        raise DbwError('factor must be 1 (plain hard render) or 4 (the resolving render)')
+    if not verts.is_cuda:
+        raise DbwError('the CUDA renderer needs CUDA tensors (there is no CPU fallback)')
+    dev = verts.device
+    H, W = image_size
+    B = R.shape[0]
+    normals = vertex_normals(verts, faces) if normals is None else normals
+
+    def run():
+        with torch.no_grad():
+            vw, Rc, Tc = verts.detach().contiguous().float(), R.detach().contiguous().float(), T.detach().contiguous().float()
+            v_in, i_in, ndc = vw, intr, False
+            if torch.is_tensor(intr):             # per-view intrinsics: the kernel rasterizes the projected vertices
+                v_in, i_in, ndc = project_verts(vw, Rc, Tc, intr).contiguous(), (1., 1., 0., 0.), True
+            L = _lib.lib()
+            cfg, map_table = scene_settings(v_in, faces, maps, map_table_host, B, i_in, (H * factor, W * factor), 0.0, 1, z_clip,
+                                            detach_bary, clip_inside, background, faces_alpha, perspective_correct, ndc,
+                                            blur_radius=0.0)
+            ws_bytes, bwd = ctypes.c_size_t(0), ctypes.c_size_t(0)
+            if factor == 4:
+                _lib.check(L.dbw_viz_workspace_bytes(ctypes.byref(cfg), 4, ctypes.byref(ws_bytes)), 'dbw_viz_workspace_bytes')
+            else:
+                _lib.check(L.dbw_workspace_bytes(ctypes.byref(cfg), ctypes.byref(ws_bytes), ctypes.byref(bwd)), 'dbw_workspace_bytes')
+            ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
+            n_bkg, bk = 0, None
+            if bkg is not None:
+                bk = bkg.to(device=dev, dtype=torch.float32).reshape(-1, 3, H, W).contiguous()
+                n_bkg = bk.shape[0]
+            rgba = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)
+            rgb8 = torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev) if frames_u8 else None
+            # converted copies are held until the launch is enqueued
+            args = [v_in.contiguous().float(), faces.to(torch.int32).contiguous(), faces_uvs.contiguous().float(),
+                    face_map.to(torch.int32).contiguous(), maps.contiguous().float(), map_table, Rc, Tc,
+                    faces_alpha.detach().contiguous().float() if faces_alpha is not None else None, vw, normals.contiguous().float()]
+            _lib.check(L.dbw_render_forward_phong(ctypes.byref(cfg), *[_c(a) for a in args], ctypes.byref(shading), factor, _c(bk),
+                                                  n_bkg, _c(rgba), _c(rgb8), _c(ws), ws.numel(), _stream()), 'dbw_render_forward_phong')
+            return (rgba, rgb8) if frames_u8 else rgba
+
+    if factor == 1 and (bkg is not None or frames_u8):
+        raise DbwError('bkg and frames_u8 belong to the resolving render (factor 4)')
+    if frames_u8:
+        return run()
+    return _PhongFn.apply(verts, maps, faces_alpha, R, T, run)
+
+
 class Renderer(nn.Module):
     def __init__(self, img_size, **kwargs):
         super().__init__()
@@ -392,6 +514,7 @@ class Renderer(nn.Module):
         self.shading_type = kwargs.pop('shading_type', SHADING_TYPE)
         self.detach_bary = kwargs.pop('detach_bary', False)
         assert len(kwargs) == 0, kwargs
+        self._vf = None             # (int32 faces, vertex -> face list) of the last phong render's topology
         self.blur_radius = float(np.log(1. / 1e-4 - 1.) * self.sigma)                # renderer.py:51
 
     def init_cameras(self, **kwargs):
@@ -437,9 +560,30 @@ class Renderer(nn.Module):
         maps, table = meshes.textures.packed_maps()
         return verts, faces, fvu, fmap, maps, table
 
+    def _phong_normals(self, verts, faces):
+        """vertex_normals of the scene, through a vertex -> face list kept while the faces tensor is unchanged (its storage is
+        held with it, so that no other faces can take its address)"""
+        key = (faces.data_ptr(), tuple(faces.shape), faces.stride(), faces._version, verts.shape[0], str(faces.device))
+        if self._vf is None or self._vf[0] != key:
+            f32 = faces.to(torch.int32).contiguous()
+            self._vf = (key, faces, f32, vertex_face_list(f32, verts.shape[0]))
+        return vertex_normals(verts, self._vf[2], self._vf[3])
+
+    def _phong(self, meshes, R, T, K, factor, faces_alpha=None, bkg=None, frames_u8=False):
+        """LayeredShader(shading_type='phong') over the hard single-layer render: render_scene_phong with this renderer's
+        lights, PyTorch3D's default materials and the scene's vertex normals"""
+        verts, faces, fvu, fmap, maps, table = self._scene(meshes)
+        intr = K if K is not None else self.cameras.intrinsics()
+        return render_scene_phong(verts, faces, fvu, fmap, maps, table, R, T, intr, self.img_size, phong_shading(self.light_kwargs),
+                                  factor, self.z_clip, self.detach_bary, self.clip_inside, self.background_color, faces_alpha,
+                                  self.perspective_correct, bkg=bkg, frames_u8=frames_u8, normals=self._phong_normals(verts, faces))
+
     def _shade(self, verts, faces, R):
         """the per-(view, face) flat-shading multiplier of a lit renderer, None for the raw one"""
         lit = self.light_kwargs.get('name', 'ambient') == 'directional'
+        if self.shading_type == 'gouraud':
+            raise NotImplementedError('shading_type=gouraud: PyTorch3D interpolates vertex colours (TexturesVertex), which a '
+                                      'texture-mapped scene does not have')
         if self.shading_type not in ('raw', 'flat') or (lit != (self.shading_type == 'flat')):
             raise NotImplementedError(f'shading_type={self.shading_type} with lights={self.light_kwargs.get("name", "ambient")}: '
                                       'only raw+ambient (training) and flat+directional (renderer_light) are implemented')
@@ -447,6 +591,14 @@ class Renderer(nn.Module):
 
     def forward(self, meshes, R, T, viz_purpose=False, **kwargs):
         faces_alpha, K = kwargs.get('faces_alpha'), kwargs.get('K')
+        if self.shading_type == 'phong':
+            if viz_purpose:          # VizMeshRenderer's frame, resolved in the kernel: the bits of avg_pool2d(render at 4x, 4)
+                with torch.no_grad():
+                    return self._phong(meshes, R, T, K, 4, faces_alpha)
+            if self.sigma != 0 or self.faces_per_pixel != 1:
+                raise NotImplementedError(f'soft phong shading (sigma={self.sigma}, faces_per_pixel={self.faces_per_pixel}) is not '
+                                          'implemented: phong renders are hard and single-layer (sigma=0, faces_per_pixel=1)')
+            return self._phong(meshes, R, T, K, 1, faces_alpha)
         verts, faces, fvu, fmap, maps, table = self._scene(meshes)
         H, W = self.img_size
         intr = K if K is not None else self.cameras.intrinsics()      # K (B,4,4): each view with its own intrinsics
@@ -467,6 +619,8 @@ class Renderer(nn.Module):
         """forward(meshes, R, T, viz_purpose=True, K=K) -- the same bits -- in one resolving kernel that never writes the 4x
         supersampled image (render_scene_viz): rgba (B,4,H,W), RGB composited over bkg ((3,H,W) or (1 | B,3,H,W)) when given;
         with frames_u8 also the (B,H,W,3) uint8 frames a video encoder takes.  No gradient."""
+        if self.shading_type == 'phong':
+            return self._phong(meshes, R, T, K, 4, bkg=bkg, frames_u8=frames_u8)
         verts, faces, fvu, fmap, maps, table = self._scene(meshes)
         intr = K if K is not None else self.cameras.intrinsics()
         return render_scene_viz(verts, faces, fvu, fmap, maps, table, R, T, intr, self.img_size, self.z_clip, self.detach_bary,

@@ -3,9 +3,11 @@ src/utils/image.py:61-115), with PyTorch3D's look-at cameras.
 
 Every frame is VizMeshRenderer's (hard render at 4H x 4W, box-filtered 4x4), made by `Renderer.render_viz`: the resolving
 kernel never writes the 16x sample image, so a chunk of frames costs its H x W outputs plus the scene's face records.
+With eye_light=True an unlit renderer is swapped for a Phong-shaded one lit from the camera, as in the reference.
 Chunks are sized by a byte budget (CHUNK_BYTES, or `chunk_bytes=`) instead of the reference's fixed 10 frames; the frames
 do not depend on the chunk size.  Videos are written with OpenCV (`mp4v`, RGB -> BGR), GIFs with PIL."""
 import math
+from copy import deepcopy
 from pathlib import Path
 
 import numpy as np
@@ -82,9 +84,30 @@ def get_circle_traj(dist=1, a_scale=15, e_scale=15, N_views=50):
 
 
 # ------------------------------------------------------------------ frames
-def _refuse_eye_light(eye_light):
-    if eye_light:
-        raise NotImplementedError('eye_light=True needs phong shading, which this renderer does not implement')
+# the lights of the eye_light renders (renderer.py:303-305 and :345-348): a directional light fixed to the camera, no specular
+EYE_LIGHT_ROTATED = {'name': 'directional', 'direction': [[0, 0, -1]], 'ambient_color': [[0.6, 0.6, 0.6]],
+                     'diffuse_color': [[0.4, 0.4, 0.4]], 'specular_color': [[0., 0., 0.]]}
+EYE_LIGHT_VIEWS = {'name': 'directional', 'direction': [DIRECTION_LIGHT], 'ambient_color': [[0.7, 0.7, 0.7]],
+                   'diffuse_color': [[0.4, 0.4, 0.4]], 'specular_color': [[0., 0., 0.]]}
+
+
+def _eye_light(renderer, img_size, lights):
+    """the reference's eye_light swap: an unlit (ambient) renderer is replaced by a Phong-shaded, single-layer one with the
+    given lights and its other settings; a lit renderer is kept"""
+    if renderer.light_kwargs.get('name', 'ambient') != 'ambient':
+        return renderer
+    kwargs = renderer.init_kwargs
+    kwargs['lights'] = deepcopy(lights)
+    kwargs['shading_type'] = 'phong'
+    kwargs['faces_per_pixel'] = 1
+    return Renderer(img_size, **kwargs)
+
+
+def _check_mesh(mesh, who):
+    """the helpers render a Meshes (one joined scene): anything else is refused before a renderer or a device is set up --
+    NotImplementedError, as for the other input structures dbw_b200 does not provide for (pointcloud.py)"""
+    if not (hasattr(mesh, 'get_mesh_verts_faces') and hasattr(mesh, 'textures')):
+        raise NotImplementedError(f'{who}: rendering a {type(mesh).__name__} is not implemented (pass a Meshes with TexturesUV)')
 
 
 def _device():
@@ -138,14 +161,19 @@ def _to_u8(rgb):
 
 
 def _rotated_setup(mesh, n_views, elev, dist, R, T, bkg, renderer, rend_kwargs, eye_light, device):
-    _refuse_eye_light(eye_light)
+    _check_mesh(mesh, 'render_rotated_views')
+    if eye_light and R is not None:
+        raise NotImplementedError('render_rotated_views: eye_light=True with a given R (as in the reference)')
     img_size = VIZ_IMG_SIZE if renderer is None else renderer.img_size
     device = _device() if device is None else device
     rend_kwargs = {} if rend_kwargs is None else rend_kwargs
     if renderer is not None:          # a fresh renderer with the given one's settings and camera (renderer.py:297-300)
         rend_kwargs = renderer.init_kwargs
         rend_kwargs.setdefault('cameras', {})['K'] = renderer.cameras.K
-    renderer = Renderer(img_size, **rend_kwargs).to(device)
+    renderer = Renderer(img_size, **rend_kwargs)
+    if eye_light:
+        renderer = _eye_light(renderer, img_size, EYE_LIGHT_ROTATED)
+    renderer = renderer.to(device)
     elev, dist = 0 if R is not None else elev, 0 if T is not None else dist
     R = R.to(device) if R is not None else torch.eye(3, device=device)
     T = T.to(device) if T is not None else torch.zeros(3, device=device)
@@ -164,10 +192,12 @@ def render_rotated_views(mesh, n_views=50, elev=30, dist=2.5, R=None, T=None, bk
 
 
 def _views_setup(mesh, img_size, renderer, rend_kwargs, eye_light, device, bkg):
-    _refuse_eye_light(eye_light)
+    _check_mesh(mesh, 'render_views')
     device = _device() if device is None else device
     if renderer is None:
         renderer = Renderer(img_size or VIZ_IMG_SIZE, **({} if rend_kwargs is None else rend_kwargs))
+    if eye_light:
+        renderer = _eye_light(renderer, renderer.img_size, EYE_LIGHT_VIEWS)
     mesh, renderer = mesh.to(device), renderer.to(device)
     return mesh, renderer, _fit_bkg(bkg, renderer.img_size)
 

@@ -188,6 +188,57 @@ int dbw_render_backward(const DbwRenderSettings* settings, const float* verts, c
                         void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
 
 /*
+ * Phong shading (PyTorch3D phong_shading as the reference's LayeredShader calls it, src/model/renderer.py:187-238; its
+ * eye_light views, renderer.py:301-310,343-351).  Forward only: there is no backward of a phong render.
+ *
+ * Vertex normals = Meshes.verts_normals_packed: each vertex sums the area-weighted normals (v2 - v1) x (v0 - v1) of its
+ * incident faces, then the sum is normalised with eps 1e-6 (a vertex without faces gets 0).  The sums run in a fixed order
+ * through a vertex -> face list built once per topology, with no float atomics: two calls give the same bits.
+ *   dbw_vertex_face_list  faces (F,3) int32 -> vf_end (V) int32 and vf_faces (3F) int32: the faces of vertex v are
+ *                         vf_faces[v ? vf_end[v-1] : 0 .. vf_end[v]) in ascending order (a face listed once per corner
+ *                         on v).  Corners outside [0, V) are skipped.
+ *   dbw_vertex_normals    verts (V,3) world, faces and the list -> normals (V,3)
+ */
+int dbw_vertex_face_list(const int32_t* faces, int32_t n_faces, int32_t n_verts, int32_t* vf_end, int32_t* vf_faces,
+                         void* stream);
+int dbw_vertex_normals(const float* verts, const int32_t* faces, int32_t n_verts, const int32_t* vf_end,
+                       const int32_t* vf_faces, float* normals, void* stream);
+
+#define DBW_LIGHT_AMBIENT 0        /* AmbientLights: colour = ka * ambient_color * texel                                      */
+#define DBW_LIGHT_DIRECTIONAL 1    /* DirectionalLights; `direction` is re-expressed per view as direction @ R^T (renderer.py:87-97) */
+#define DBW_LIGHT_POINT 2          /* PointLights; `direction` holds the location, fixed in the world                         */
+
+/* One light and the materials (PyTorch3D's Lights / Materials, one entry each).  PyTorch3D's defaults: ambient 0.5,
+ * diffuse 0.3, specular 0.2, direction / location (0, 1, 0) (AmbientLights: ambient 1); ka = kd = ks = 1, shininess 64. */
+typedef struct DbwPhongShading {
+  int32_t light;              /* DBW_LIGHT_*                                                                        */
+  float ambient_color[3], diffuse_color[3], specular_color[3];
+  float direction[3];         /* directional: direction in the world; point: location in the world                   */
+  float ka[3], kd[3], ks[3];  /* Materials ambient_color, diffuse_color, specular_color                              */
+  float shininess;
+} DbwPhongShading;
+
+/*
+ * Hard single-layer render (faces_per_pixel = 1, sigma = 0, blur_radius = 0) with each pixel's winning fragment Phong-shaded:
+ *   n = bary . normals[faces[f]],  p = bary . verts_world[faces[f]]   (the fragment's barycentrics w.r.t. the original face,
+ *   after z-clipping),  colour = (ka La + kd diffuse(n, p)) * texel + ks specular(n, p, camera centre -T @ R^T, shininess),
+ * then blended like dbw_render_forward's (faces_alpha, background).  Arguments up to faces_alpha are dbw_render_forward's;
+ * R and T are required even with verts_are_ndc (they place the light and the camera centre).
+ *   verts_world  (V,3) world-space vertices (with verts_are_ndc, `verts` is the projected input and cannot supply them)
+ *   normals      (V,3) dbw_vertex_normals of verts_world
+ *   factor 1     out_rgba (B,4,height,width); bkg and out_rgb8 must be NULL; workspace: dbw_workspace_bytes' fwd_bytes
+ *   factor 4     the resolving render of dbw_render_forward_viz (same outputs, same guarantees: avg_pool2d's order, the
+ *                background composite, the uint8 frames); workspace: dbw_viz_workspace_bytes()
+ * save_fragment_state must be 0; view_rows is refused with factor 4.
+ */
+int dbw_render_forward_phong(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
+                             const float* faces_uvs, const int32_t* face_map, const float* maps,
+                             const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                             const float* verts_world, const float* normals, const DbwPhongShading* shading, int32_t factor,
+                             const float* bkg, int32_t bkg_views, float* out_rgba, uint8_t* out_rgb8, void* workspace,
+                             size_t workspace_bytes, void* stream);
+
+/*
  * Fused compositing + RGB loss of the decoupled scene (src/model/dbw.py:223 and :366-367):
  *   rec = rgb_fg * a_fg + (1 - a_fg) * rgb_env ;  loss = weight * mean((imgs - rec)^2)
  * fg, env: (B,4,H,W) outputs of dbw_render_forward; imgs (B,3,H,W).  Writes rec (B,3,H,W) (may be NULL), adds
