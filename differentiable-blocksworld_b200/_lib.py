@@ -121,7 +121,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generi
            'dbw_vgg_head_backward',
            'dbw_adam_step', 'dbw_viz_workspace_bytes', 'dbw_render_forward_viz',
            'dbw_regularisers_workspace_bytes', 'dbw_regularisers_forward', 'dbw_regularisers_backward',
-           'dbw_vertex_face_list', 'dbw_vertex_normals', 'dbw_render_forward_phong']
+           'dbw_vertex_face_list', 'dbw_vertex_normals', 'dbw_render_forward_phong',
+           'dbw_image_scores_workspace_bytes', 'dbw_image_scores']
 
 _lib = None
 
@@ -223,6 +224,9 @@ def lib():
         L.dbw_vertex_normals.argtypes = [vp, vp, i32, vp, vp, vp, vp]
         L.dbw_render_forward_phong.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 11 + [ctypes.POINTER(DbwPhongShading), i32, vp, i32,
                                                                                           vp, vp, vp, sz, vp]
+        L.dbw_image_scores_workspace_bytes.restype = sz
+        L.dbw_image_scores_workspace_bytes.argtypes = [i32, i32, i32]
+        L.dbw_image_scores.argtypes = [i32, i32, i32, vp, vp, ctypes.POINTER(ctypes.c_float), vp, vp, vp, sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

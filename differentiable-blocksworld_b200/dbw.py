@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import _lib, geometry as G, losses as L
+from . import _lib, geometry as G, losses as L, metrics as M
 from .renderer import Renderer, render_scene, _c, _stream
 from .fused_loss import ScenePass, scene_mse
 from .scene_ops import (scene_geometry_passes, block_opacities, scene_atlases, scene_texture_cells, atlases_from_cells,
@@ -696,8 +696,11 @@ class DifferentiableBlocksWorld(nn.Module):
     @torch.no_grad()
     def quantitative_eval(self, loader, device, hard_inference=True):
         """the columns of final_scores.tsv (dbw.py:464-493): n_blocks, L_tot, L_rec, PSNR, SSIM, LPIPS, alpha_k -- hard 4x
-        supersampled renders of the opaque blocks over a loader.  LPIPS is NaN when no perceptual network is installed, or
-        when the installed term is the VGG feature loss (perceptual.PerceptualLoss), which is not an LPIPS score."""
+        supersampled renders of the opaque blocks (resolved in the raster kernel, Renderer.render_viz) over a loader.  LPIPS
+        is NaN when no perceptual network is installed, or when the installed term is the VGG feature loss
+        (perceptual.PerceptualLoss), which is not an LPIPS score.  As the reference's AverageMeters, every column is the
+        mean of its per-batch values weighted by the batch size: PSNR is that of each batch's mean squared error, SSIM
+        1 - mean(1 - SSIM) over each batch's views.  The scores stay on the device until one host read at the end."""
         from .perceptual import PerceptualLoss
         self.eval()
         opacities = self.get_opacities()
@@ -705,22 +708,27 @@ class DifferentiableBlocksWorld(nn.Module):
         perceptual = getattr(self, 'perceptual_loss', None)
         if isinstance(perceptual, PerceptualLoss):
             perceptual = None
-        sums, count = dict(L_tot=0.0, L_rec=0.0, PSNR=0.0, SSIM=0.0, LPIPS=0.0), 0
+        sums, count = torch.zeros(5, dtype=torch.float64, device=device), 0          # L_tot, L_rec, PSNR, SSIM, LPIPS
         for inp, labels in loader:
             inp = {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in inp.items()}
             self._install_cameras(inp)
             imgs, n = inp['imgs'], len(inp['imgs'])
-            rec = (self.renderer(scene.extend(n), inp['R'], inp['T'], viz_purpose=True, K=self._view_K(inp))[:, :3] if hard_inference
+            rec = (self.renderer.render_viz(scene.extend(n), inp['R'], inp['T'], K=self._view_K(inp))[:, :3] if hard_inference
                    else self.predict(inp, labels, filter_transparent=True))
             losses = self.compute_losses(imgs, rec)
-            sums['L_tot'] += float(losses['total']) * n
-            sums['L_rec'] += float(sum(losses[k] for k in ('rgb', 'perceptual') if k in losses)) * n
-            sums['PSNR'] += float(-10.0 * torch.log10(F.mse_loss(imgs, rec))) * n
-            sums['SSIM'] += float(L.ssim(imgs, rec).mean()) * n
-            sums['LPIPS'] += (float(perceptual(imgs, rec)) if perceptual is not None else float('nan')) * n
+            se, ssim = M.image_scores(imgs, rec)
+            rec_terms = [losses[k] for k in ('rgb', 'perceptual') if k in losses]
+            row = [losses['total'], sum(rec_terms) if rec_terms else imgs.new_zeros(()), M.psnr_of(se, imgs[0].numel()),
+                   1 - (1 - ssim).mean(), perceptual(imgs, rec) if perceptual is not None else imgs.new_zeros(())]
+            sums += torch.stack([v.detach().double().reshape(()) for v in row]) * n
             count += n
-        return OrderedDict([('n_blocks', int((opacities > 0.5).sum()))] + [(k, v / max(count, 1)) for k, v in sums.items()]
-                           + [(f'alpha{k}', a.item()) for k, a in enumerate(opacities)])
+        values = torch.cat([sums / max(count, 1), opacities.to(sums)]).tolist()
+        scores, alphas = values[:5], values[5:]
+        if perceptual is None and count:
+            scores[4] = float('nan')
+        return OrderedDict([('n_blocks', sum(a > 0.5 for a in alphas))]
+                           + list(zip(('L_tot', 'L_rec', 'PSNR', 'SSIM', 'LPIPS'), scores))
+                           + [(f'alpha{k}', a) for k, a in enumerate(alphas)])
 
     @torch.no_grad()
     def qualitative_eval(self, loader, device, path=None, NV=240, n_inputs=10):

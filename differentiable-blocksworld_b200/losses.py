@@ -155,7 +155,8 @@ def regularisers(texture_bkg, texture_ground, textures, S, R_6d, T, sq_eps, alph
 def ssim(img1, img2, window_size=11, sigma=1.5):
     """mean structural similarity of two (B,C,H,W) images in [0,1] with the Gaussian window of the reference's evaluation
     (`SSIMLoss(padding=False)`, src/model/loss.py:113-155: 11 taps, sigma 1.5, C1 = 0.01^2, C2 = 0.03^2, 'valid' borders),
-    evaluated separably (two 1-D passes per moment instead of one 11x11 pass).  Returns (B,) = mean SSIM per image."""
+    evaluated separably (two 1-D passes per moment instead of one 11x11 pass).  Returns (B,) = mean SSIM per image.  The
+    PyTorch statement of the evaluation's SSIM; quantitative_eval computes it on the device with metrics.ssim."""
     C = img1.shape[1]
     x = torch.arange(window_size, dtype=img1.dtype, device=img1.device) - window_size // 2
     g = torch.exp(-x.pow(2) / (2 * sigma ** 2))

@@ -800,6 +800,26 @@ int dbw_regularisers_backward(const DbwRegularisers* r, const float* g_out_parsi
                               float* g_S, float* g_R_6d, float* g_T, float* g_sq_eps, float* g_alpha_full, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/*
+ * Image scores of the evaluation (src/model/dbw.py:464-493): per view b of two (n_views, 3, height, width) images,
+ *   se_sum[b]     sum over the view's 3 height width values of (imgs - rec)^2       (the numerator of nn.MSELoss)
+ *   ssim_mean[b]  mean of the valid-region SSIM map, 3 (height - 10) (width - 10) values: 1 - SSIMLoss(padding=False)[b]
+ *                 (src/model/loss.py:119-156), 11x11 Gaussian window, C1 = 0.01^2, C2 = 0.03^2
+ * The window is separable and applied as an 11-tap pass along rows then columns.  Deterministic (no float atomics: per-tile
+ * partials summed in a fixed order) and capturable (no allocation, no host read).  2 launches.
+ *
+ *   imgs, rec   DEVICE fp32 (n_views, 3, height, width), contiguous
+ *   window      HOST fp32 (11): the 1-D window, the reference's gaussian(11, 1.5) (float32 values normalised by their
+ *               float32 sum); copied into the kernel's arguments
+ *   se_sum, ssim_mean  DEVICE fp32 (n_views), written
+ *   workspace   caller-owned device memory of at least dbw_image_scores_workspace_bytes() bytes
+ * height or width below 11 is an error (the reference's map is then empty and its mean NaN), as is n_views outside
+ * 1..65535.  dbw_image_scores_workspace_bytes returns 0 for such sizes.
+ */
+size_t dbw_image_scores_workspace_bytes(int32_t n_views, int32_t height, int32_t width);
+int dbw_image_scores(int32_t n_views, int32_t height, int32_t width, const float* imgs, const float* rec, const float* window,
+                     float* se_sum, float* ssim_mean, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
