@@ -98,6 +98,11 @@ class DbwPhongShading(ctypes.Structure):
 LIGHTS = {'ambient': 0, 'directional': 1, 'point': 2}        # DBW_LIGHT_* of include/dbw_render.h
 
 
+class DbwAtlasJob(ctypes.Structure):
+    _fields_ = [('map', ctypes.c_void_p), ('h', ctypes.c_int32), ('w', ctypes.c_int32), ('x0', ctypes.c_int32),
+                ('y0', ctypes.c_int32), ('cell_w', ctypes.c_int32), ('cell_h', ctypes.c_int32)]
+
+
 class DbwMapDesc(ctypes.Structure):
     _fields_ = [('offset', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
                 ('reserved', ctypes.c_int32)]
@@ -122,7 +127,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generi
            'dbw_adam_step', 'dbw_viz_workspace_bytes', 'dbw_render_forward_viz',
            'dbw_regularisers_workspace_bytes', 'dbw_regularisers_forward', 'dbw_regularisers_backward',
            'dbw_vertex_face_list', 'dbw_vertex_normals', 'dbw_render_forward_phong',
-           'dbw_image_scores_workspace_bytes', 'dbw_image_scores']
+           'dbw_image_scores_workspace_bytes', 'dbw_image_scores',
+           'dbw_texture_atlas_workspace_bytes', 'dbw_texture_atlas_u8']
 
 _lib = None
 
@@ -227,6 +233,9 @@ def lib():
         L.dbw_image_scores_workspace_bytes.restype = sz
         L.dbw_image_scores_workspace_bytes.argtypes = [i32, i32, i32]
         L.dbw_image_scores.argtypes = [i32, i32, i32, vp, vp, ctypes.POINTER(ctypes.c_float), vp, vp, vp, sz, vp]
+        L.dbw_texture_atlas_workspace_bytes.restype = sz
+        L.dbw_texture_atlas_workspace_bytes.argtypes = [i32]
+        L.dbw_texture_atlas_u8.argtypes = [ctypes.POINTER(DbwAtlasJob), i32, i32, i32, vp, vp, sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

@@ -25,6 +25,7 @@ from .renderer import Renderer, render_scene, _c, _stream
 from .fused_loss import ScenePass, scene_mse
 from .scene_ops import (scene_geometry_passes, block_opacities, scene_atlases, scene_texture_cells, atlases_from_cells,
                         cell_map_table)
+from .export import save_mesh_as_obj
 from .structures import Meshes, TexturesUV, join_meshes_as_scene
 
 # accepted keys and defaults of the config sub-dicts (configs/*/*.yml -> model.{mesh,rend_optim,loss}); unknown keys are
@@ -732,7 +733,8 @@ class DifferentiableBlocksWorld(nn.Module):
 
     @torch.no_grad()
     def qualitative_eval(self, loader, device, path=None, NV=240, n_inputs=10):
-        """the outputs of dbw.py:495-554: texture maps, the scene as OBJ (with and without background), `gt.ply` (3000 points
+        """the outputs of dbw.py:495-554: texture maps, the scene as textured OBJ (`mesh_full.{obj,mtl,png}` with the background,
+        `mesh.{obj,mtl,png}` without it and with the reduced ground; export.save_mesh_as_obj), `gt.ply` (3000 points
         of loader.dataset.pc_gt, seed 123) when the dataset has a ground-truth cloud, `rotated_mesh.mp4` (NV frames around
         the scene), and per input view the hard reconstruction, its block-coloured edge overlays, the lit synthetic-colour
         render and the videos `{tag}_rec_traj.mp4` / `{tag}_rec_traj_syn.mp4` (NV frames along get_circle_traj about the
@@ -750,8 +752,8 @@ class DifferentiableBlocksWorld(nn.Module):
         for k, img in enumerate(torch.sigmoid(self.textures).permute(0, 3, 1, 2)):
             _save_png(img, path / 'textures' / f'block_{str(k).zfill(2)}.png')
         meshes = self.build_scene(filter_transparent=True)
-        _save_obj(meshes, path / 'mesh_full.obj')
-        _save_obj(self.build_scene(filter_transparent=True, w_bkg=False, reduce_ground=True), path / 'mesh.obj')
+        save_mesh_as_obj(meshes, path / 'mesh_full.obj')
+        save_mesh_as_obj(self.build_scene(filter_transparent=True, w_bkg=False, reduce_ground=True), path / 'mesh.obj')
         syn_blocks = self.build_blocks(filter_transparent=True, synthetic_colors=True, as_scene=True)
         if len(syn_blocks) == 0:
             return None
@@ -815,16 +817,6 @@ def _save_png(chw, path):
     from PIL import Image
     arr = (chw.detach().float().clamp(0, 1) * 255).permute(1, 2, 0).cpu().numpy().astype(np.uint8)
     Image.fromarray(arr).convert('RGB').save(path)
-
-
-def _save_obj(meshes, path):
-    """geometry-only Wavefront OBJ of the first mesh (the reference's textured export goes through PyTorch3D's save_obj)"""
-    verts, faces = meshes.get_mesh_verts_faces(0)
-    with open(path, 'w') as fh:
-        for v in verts.detach().cpu().tolist():
-            fh.write('v {:.6f} {:.6f} {:.6f}\n'.format(*v))
-        for f in (faces.detach().cpu() + 1).tolist():
-            fh.write('f {} {} {}\n'.format(*f))
 
 
 class PerceptualTerm(nn.Module):

@@ -820,6 +820,30 @@ size_t dbw_image_scores_workspace_bytes(int32_t n_views, int32_t height, int32_t
 int dbw_image_scores(int32_t n_views, int32_t height, int32_t width, const float* imgs, const float* rec, const float* window,
                      float* se_sum, float* ssim_mean, void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Texture atlas of the OBJ export (the texture_map of save_obj, src/utils/mesh.py:392-393): the maps of a scene quantised as
+ * (uint8)(x * 255.0f), the float32 product then truncation, and composed into one (atlas_h, atlas_w, 3) uint8 image.  One
+ * job per map; its cell, cell_w x cell_h texels from (x0 - 1, y0 - 1), holds the map at (x0, y0), a 1-texel gutter around it
+ * that replicates the map's edge texels, and zeros in the rest of the cell.  The cells must tile the atlas exactly (inside
+ * it, no overlap, areas summing to atlas_h atlas_w), so every atlas texel is written.  Values outside [0, 1] saturate to 0
+ * or 255, NaN gives 0.  One host-to-device copy of the job table into the workspace, then 1 launch.
+ *
+ *   jobs        HOST (n_jobs): each job's map is a DEVICE fp32 (h, w, 3) contiguous map
+ *   atlas       DEVICE uint8 (atlas_h, atlas_w, 3), written
+ *   workspace   caller-owned device memory of at least dbw_texture_atlas_workspace_bytes(n_jobs) bytes
+ * dbw_texture_atlas_workspace_bytes returns 0 for n_jobs < 1.
+ */
+typedef struct DbwAtlasJob {
+  const float* map;           /* DEVICE fp32 (h, w, 3)                                                              */
+  int32_t h, w;
+  int32_t x0, y0;             /* atlas column and row of the map's texel (0, 0)                                     */
+  int32_t cell_w, cell_h;     /* the region the job writes, from (x0 - 1, y0 - 1): at least (w + 2) x (h + 2)       */
+} DbwAtlasJob;
+
+size_t dbw_texture_atlas_workspace_bytes(int32_t n_jobs);
+int dbw_texture_atlas_u8(const DbwAtlasJob* jobs, int32_t n_jobs, int32_t atlas_h, int32_t atlas_w, uint8_t* atlas,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
