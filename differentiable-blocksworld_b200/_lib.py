@@ -108,6 +108,10 @@ class DbwMapDesc(ctypes.Structure):
                 ('reserved', ctypes.c_int32)]
 
 
+class DbwGatherField(ctypes.Structure):
+    _fields_ = [('src', ctypes.c_void_p), ('dst', ctypes.c_void_p), ('words_per_view', ctypes.c_int64)]
+
+
 EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generic_blocks_loss', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
            'dbw_render_forward_loss', 'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_camera_project', 'dbw_camera_project_backward',
@@ -128,7 +132,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generi
            'dbw_regularisers_workspace_bytes', 'dbw_regularisers_forward', 'dbw_regularisers_backward',
            'dbw_vertex_face_list', 'dbw_vertex_normals', 'dbw_render_forward_phong',
            'dbw_image_scores_workspace_bytes', 'dbw_image_scores',
-           'dbw_texture_atlas_workspace_bytes', 'dbw_texture_atlas_u8']
+           'dbw_texture_atlas_workspace_bytes', 'dbw_texture_atlas_u8',
+           'dbw_resample_u8_workspace_bytes', 'dbw_resample_u8', 'dbw_gather_views', 'dbw_subsample_points']
 
 _lib = None
 
@@ -236,6 +241,10 @@ def lib():
         L.dbw_texture_atlas_workspace_bytes.restype = sz
         L.dbw_texture_atlas_workspace_bytes.argtypes = [i32]
         L.dbw_texture_atlas_u8.argtypes = [ctypes.POINTER(DbwAtlasJob), i32, i32, i32, vp, vp, sz, vp]
+        L.dbw_resample_u8_workspace_bytes.argtypes = [i32] * 5 + [ctypes.POINTER(sz)]
+        L.dbw_resample_u8.argtypes = [i32, i32, i32, vp, i32, i32, vp, vp, sz, vp]
+        L.dbw_gather_views.argtypes = [i32, i32, vp, vp, i32, i32, vp, ctypes.POINTER(DbwGatherField), i32, vp]
+        L.dbw_subsample_points.argtypes = [i64, i32, vp, i32, i32, vp, ctypes.c_uint64, ctypes.c_uint64, i64, vp, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

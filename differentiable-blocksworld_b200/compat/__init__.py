@@ -14,7 +14,8 @@ own implementations), the point-cloud ops of the reference's 3-D evaluation (`kn
 k-NN kernels, the chamfer helpers and `chamfer_distance`, `sample_points_from_meshes`: dbw_b200/pointcloud.py), the
 look-at cameras `look_at_view_transform` / `look_at_rotation` (dbw_b200/views.py), the two `seaborn` / `matplotlib.colors`
 calls behind the block colour map (`utils/plot.py:77-87`).
-Everything else the reference imports at module load but only calls on its export / evaluation paths (PLY / OBJ I/O, the
+`load_ply` for point clouds (dtu_eval's PLY reader: the reference's DTUDataset reads its ground truth through it).
+Everything else the reference imports at module load but only calls on its export / evaluation paths (PLY writing, OBJ I/O, the
 SVD ICP, `Pointclouds`, Open3D, video writing, plotting, LPIPS weights) is a named placeholder that raises
 `NotImplementedError` when CALLED: the control plane stays out of scope (SURVEY 8), the import graph is satisfied."""
 import colorsys
@@ -98,6 +99,17 @@ def _ico_sphere(level=0, device=None):
     return m.to(device) if device is not None else m
 
 
+def _load_ply(f, *, path_manager=None):
+    """pytorch3d.io.load_ply for point clouds (the reference's DTU ground truth, dtu.py:47): (verts (V, 3) float32, faces (0, 3)
+    int64), on dtu_eval's PLY reader.  A file with faces is refused rather than returned without them."""
+    from ..dtu_eval import read_ply
+    with open(f, 'rb') as fh:
+        head = fh.read(1 << 16).split(b'end_header')[0].decode('ascii', 'replace').split('\n')
+    if any(l.split()[:2] == ['element', 'face'] and int(l.split()[2]) > 0 for l in head if len(l.split()) >= 3):
+        raise NotImplementedError(f'dbw_b200.compat load_ply reads point clouds; {f} has faces')
+    return torch.from_numpy(read_ply(f)).float(), torch.zeros(0, 3, dtype=torch.int64)
+
+
 def _pytorch3d():
     P = lambda n: _placeholder(f'pytorch3d.{n}')
     _module('pytorch3d', __version__='0.7.1+dbw_b200.compat')
@@ -113,7 +125,7 @@ def _pytorch3d():
             iterative_closest_point=P('ops.iterative_closest_point'), knn_points=PC.knn_points, knn_gather=PC.knn_gather)
     _module('pytorch3d.ops.subdivide_meshes', SubdivideMeshes=SubdivideMeshes)
     _module('pytorch3d.ops.knn', knn_points=PC.knn_points, knn_gather=PC.knn_gather)
-    _module('pytorch3d.io', save_ply=P('io.save_ply'), load_ply=P('io.load_ply'), save_obj=P('io.save_obj'),
+    _module('pytorch3d.io', save_ply=P('io.save_ply'), load_ply=_load_ply, save_obj=P('io.save_obj'),
             load_obj=P('io.load_obj'), load_objs_as_meshes=P('io.load_objs_as_meshes'))
     _module('pytorch3d.io.utils', _open_file=P('io.utils._open_file'))
     _module('pytorch3d.loss', mesh_normal_consistency=P('loss.mesh_normal_consistency'), chamfer_distance=PC.chamfer_distance)

@@ -18,7 +18,12 @@ learning rates are read on the device: a scheduler changes them between replays 
 Per-view intrinsics (model.set_per_view_intrinsics(True)): inp['K'] is one of the static inputs, copied in before each replay, so
 a batch with other intrinsics is rendered with them without a new capture.  Intrinsics gradients (a ViewParallel built with
 intrinsics=True, and a K that requires grad in example_inp): (fx, fy, px, py) of the full batch become one more static leaf
-beside the poses, and its summed gradient is back-propagated into the caller's K after the replay."""
+beside the poses, and its summed gradient is back-propagated into the caller's K after the replay.
+
+Captured gather (GraphedStep(views=data.DeviceViews)): the step's inputs are gathered from views resident on the device by a
+launch captured at the head of the graph, from a static buffer of B view indices.  run(items=...) writes the B dataset item
+indices of the batch there, one small host-to-device copy, and replays: no image crosses the bus.  The inputs are then exactly
+those DeviceLoader would have handed to run(inp).  Not combined with camera-pose gradients."""
 import torch
 
 from .optim import BucketAdam
@@ -27,7 +32,8 @@ from .renderer import intrinsics_of
 
 
 class GraphedStep:
-    def __init__(self, view_parallel, example_inp, n_total_views, warmup=3, capture_all_reduce=None, generator=None, optimizer=None):
+    def __init__(self, view_parallel, example_inp, n_total_views, warmup=3, capture_all_reduce=None, generator=None, optimizer=None,
+                 views=None):
         self.vp, self.model = view_parallel, view_parallel.model
         if optimizer is not None and not isinstance(optimizer, BucketAdam):
             raise TypeError('GraphedStep: only an optim.BucketAdam can be captured (its launch reads rates and counters on the device)')
@@ -50,6 +56,14 @@ class GraphedStep:
         self.n_total = n_total_views
         dev = example_inp['imgs'].device
         self.static_inp = {k: v.clone() for k, v in example_inp.items()}
+        self.views, self.view_index = views, None
+        if views is not None:
+            if self.pose is not None:
+                raise ValueError('GraphedStep: a captured gather (views=...) cannot be combined with camera-pose gradients')
+            if set(self.static_inp) != {'imgs', 'K', 'R', 'T'}:
+                raise ValueError(f"GraphedStep: with views=..., example_inp holds exactly imgs, K, R and T, got {sorted(self.static_inp)}")
+            self.view_index = torch.zeros(len(self.static_inp['imgs']), dtype=torch.int64, device=dev)
+            views.check_batch(self.static_inp, len(self.view_index))     # refuses buffers whose shapes or dtypes differ
         self.model.n_total_views = n_total_views
         # random inputs of a step are pre-drawn into buffers OWNED BY THIS STEP (a graph captures addresses): the opacity
         # noise (dbw.py:300-301) and the overlap term's sample points (dbw.py:393).  `generator` is shared by the steps of a
@@ -107,6 +121,8 @@ class GraphedStep:
         self.pose_grads = self.vp.pose_grads(self.pose) if self.pose is not None else None
 
     def _body(self):
+        if self.views is not None:
+            self.views.launch_gather(self.view_index, self.static_inp)
         losses, reduced = self.vp.local_step(self.static_inp, None, self.n_total, collective=self.capture_all_reduce, poses=self.pose)
         self.inside = self.vp.reduces_inside_backward(self.static_inp)      # the collective sits INSIDE the backward (parallel.GradSumPoint)
         if self.capture_all_reduce and not reduced:
@@ -161,13 +177,24 @@ class GraphedStep:
             if self._intrinsics_leaf and 'K' in inp:
                 self.pose[3].copy_(intrinsics_of(inp['K'].detach()), non_blocking=non_blocking)
 
-    def run(self, inp=None, non_blocking=True, all_reduce=True):
+    def run(self, inp=None, non_blocking=True, all_reduce=True, items=None):
         """inp: optional dict of (host or device) tensors for this step, copied into the static buffers.
         all_reduce=False skips the collective when it is issued after the replay (a captured one always runs).
         With an optimizer the replay also applies the update, at the learning rates param_groups hold now.
         With pose gradients, inp holds the full batch, and the summed pose gradient is back-propagated into the graph
-        behind inp['R'] / inp['T'] (without them, it stays in the static leaves' .grad)."""
+        behind inp['R'] / inp['T'] (without them, it stays in the static leaves' .grad).
+        items: with views=..., the dataset item indices of this step's batch, gathered inside the graph (a host sequence or
+        tensor; a CUDA tensor is read back to the host first, a synchronisation)."""
         self.check_poses(inp)
+        if self.views is not None and inp is not None:
+            raise ValueError('GraphedStep: this step gathers its inputs inside the graph; pass run(items=...), not inp')
+        if items is not None:
+            if self.views is None:
+                raise ValueError('GraphedStep: run(items=...) needs a step built with views=... (a captured gather)')
+            idx = self.views.item_views[torch.as_tensor(items, dtype=torch.int64).cpu()]
+            if idx.shape != self.view_index.shape:
+                raise ValueError(f'GraphedStep: {len(idx)} items, but the step was captured for {len(self.view_index)} views')
+            self.view_index.copy_(idx.pin_memory(), non_blocking=non_blocking)
         if self.optimizer is not None and not all_reduce and self.vp.world_size > 1:
             raise RuntimeError('GraphedStep: run(all_reduce=False) with an optimizer would update from gradients that are not summed')
         if inp is not None:

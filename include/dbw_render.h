@@ -844,6 +844,48 @@ size_t dbw_texture_atlas_workspace_bytes(int32_t n_jobs);
 int dbw_texture_atlas_u8(const DbwAtlasJob* jobs, int32_t n_jobs, int32_t atlas_h, int32_t atlas_w, uint8_t* atlas,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Training views (the reference's loaders, src/dataset/dtu.py:58-68, bmvs.py:49-59, dataset/__init__.py:9-26, held on the
+ * device).
+ *
+ * dbw_resample_u8: Pillow's Image.resize((out_w, out_h), BILINEAR) of n decoded RGB images, bit for bit (what torchvision's
+ * Resize runs on a PIL image).  Pillow's convolution resampler: the filter support scales with the downscale factor, the
+ * coefficients are normalised in double then stored with 22 fractional bits, rounded away from zero; a horizontal pass into a
+ * uint8 intermediate, then a vertical pass, except that an image taller than 100x its width and shrinking in height runs its
+ * vertical pass first, as Image.resize does; a pass whose size does not change is skipped (neither: a copy).  The host builds
+ * the coefficient tables and copies them into the workspace on the stream; the kernels do integer multiply-adds only.
+ *   src   DEVICE uint8 (n, in_h, in_w, 3);  dst  DEVICE uint8 (n, out_h, out_w, 3), written
+ *   workspace  caller-owned device memory of at least dbw_resample_u8_workspace_bytes(...) bytes
+ *
+ * dbw_gather_views: one batch in one launch, capturable (no host copy): for b < batch, v = idx[b] (read on the device),
+ *   imgs[b, c, y, x] = views[v, y, x, c] / 255.0f, the float32 division correctly rounded (torchvision's ToTensor), when
+ *   `views` is not NULL; and for each field, dst[b] = src[v], words_per_view 32-bit words copied bit for bit (K, R, T in any
+ *   4- or 8-byte dtype, or float images).  An index outside [0, n_views) fills that entry's outputs with NaN words.
+ *   idx   DEVICE int64 (batch);  views  DEVICE uint8 (n_views, height, width, 3) or NULL;  imgs  DEVICE fp32 (batch, 3, height, width)
+ *   fields  HOST (n_fields <= DBW_GATHER_MAX_FIELDS); their src / dst are DEVICE (n_views, words) / (batch, words)
+ *
+ * dbw_subsample_points: per batch entry b, out[b, j] = points[perm_b(j)] for j < n_out <= n_points, where perm_b is a keyed
+ *   pseudo-random permutation of [0, n_points) (cycle-walking Feistel network, key from (seed, step, idx[b])): a uniformly drawn
+ *   subset without duplicates, O(n_out) work.  A point is row_words 32-bit words, copied bit for bit.  This is not the stream of
+ *   the reference's torch.randperm.  An index outside [0, n_views) fills that entry with NaN words.
+ *   points  DEVICE (n_points, row_words words);  idx  DEVICE int64 (batch);  out  DEVICE (batch, n_out, row_words words)
+ */
+#define DBW_GATHER_MAX_FIELDS 4
+
+typedef struct DbwGatherField {
+  const void* src;            /* DEVICE (n_views, words_per_view) 32-bit words                                      */
+  void* dst;                  /* DEVICE (batch, words_per_view)                                                     */
+  int64_t words_per_view;
+} DbwGatherField;
+
+int dbw_resample_u8_workspace_bytes(int32_t n, int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, size_t* bytes);
+int dbw_resample_u8(int32_t n, int32_t in_h, int32_t in_w, const uint8_t* src, int32_t out_h, int32_t out_w, uint8_t* dst,
+                    void* workspace, size_t workspace_bytes, void* stream);
+int dbw_gather_views(int32_t n_views, int32_t batch, const int64_t* idx, const uint8_t* views, int32_t height, int32_t width,
+                     float* imgs, const DbwGatherField* fields, int32_t n_fields, void* stream);
+int dbw_subsample_points(int64_t n_points, int32_t row_words, const void* points, int32_t n_views, int32_t batch,
+                         const int64_t* idx, uint64_t seed, uint64_t step, int64_t n_out, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,7 +1,7 @@
 """Drives the reference's UNMODIFIED `src/trainer.py` (+ optimizer.py, scheduler.py, utils/*, configs/dtu/*.yml) on this repo's
 model, from a checkout of monniert/differentiable-blocksworld.
 
-    python scripts/ref_trainer_driver.py --reference /path/to/differentiable-blocksworld <run_dir> [--iters N] [--graphed]
+    python scripts/ref_trainer_driver.py --reference /path/to/differentiable-blocksworld <run_dir> [--iters N] [--graphed] [--device-data]
 
 What is swapped (INTEGRATION.md A, nothing in the reference tree is edited or copied):
   * `model.create_model`                 -> dbw_b200.dbw.create_model   (the drop-in)
@@ -9,6 +9,8 @@ What is swapped (INTEGRATION.md A, nothing in the reference tree is edited or co
   * missing third-party modules          -> dbw_b200.compat stand-ins
   * with --graphed (needs a GPU), also `optimizer.create_optimizer` -> dbw_b200.optim.create_optimizer, and the trainer's model
     becomes a dbw_b200.graph.GraphedModel: every `run_single_batch_train` is one replay of a captured step, update included
+  * with --device-data (needs a GPU), the synthetic views are served by dbw_b200.data.DeviceLoader: decoded once, resident on the
+    device, each batch one gather launch (dbw_b200.data.create_train_val_test_loader with this driver's dataset factory)
 
 With a GPU the model renders for real.  WITHOUT one the product renderer refuses to run -- there is
 no CPU fallback, by design -- so this driver replaces the model's three render entry points by parameter-touching dummies and
@@ -80,9 +82,12 @@ def main():
     ap.add_argument('--reference', required=True, help='checkout of monniert/differentiable-blocksworld')
     ap.add_argument('--iters', type=int, default=3)
     ap.add_argument('--graphed', action='store_true', help='train through a captured step with the update inside (needs a GPU)')
+    ap.add_argument('--device-data', action='store_true', help='serve the views from device memory (dbw_b200.data; needs a GPU)')
     args = ap.parse_args()
     if args.graphed and not torch.cuda.is_available():
         sys.exit('--graphed needs a GPU: a captured step has no stand-in')
+    if args.device_data and not torch.cuda.is_available():
+        sys.exit('--device-data needs a GPU: the views live in device memory')
     ref = os.path.abspath(args.reference)
     shimmed = compat.install()
     sys.path.insert(0, os.path.join(ref, 'src'))
@@ -90,6 +95,10 @@ def main():
     import model as ref_model
     ref_model.create_model = b200.create_model
     ref_dataset.create_train_val_test_loader = synthetic_loaders
+    if args.device_data:
+        from dbw_b200.data import create_train_val_test_loader
+        ref_dataset.create_train_val_test_loader = lambda cfg, rank=None, world_size=None: create_train_val_test_loader(
+            cfg, rank, world_size, get_dataset=lambda name: SyntheticViews)
     if args.graphed:
         import optimizer as ref_optimizer
         from dbw_b200.optim import create_optimizer
@@ -133,7 +142,8 @@ def main():
     T.save(epoch=1, batch=it)
     moved = sorted(n for n, p in T.model.named_parameters() if not torch.equal(p.detach(), before[n]))
     ckpt = torch.load(run_dir / 'model.pkl', map_location='cpu', weights_only=False)
-    out = {'shimmed': shimmed, 'stubbed_render': stubbed, 'graphed': args.graphed, 'optimizer': type(T.optimizer).__name__, 'device': str(T.device), 'loss_names': T.model.loss_names,
+    out = {'shimmed': shimmed, 'stubbed_render': stubbed, 'graphed': args.graphed, 'device_data': args.device_data,
+           'loader': type(T.train_loader).__name__, 'optimizer': type(T.optimizer).__name__, 'device': str(T.device), 'loss_names': T.model.loss_names,
            'param_groups': groups, 'lrs': lrs, 'moved': moved, 'cur_epoch': T.model.cur_epoch,
            'checkpoint_keys': sorted(ckpt['model_state'].keys()), 'model_name': ckpt['model_name'],
            'train_metrics_rows': len(open(run_dir / 'train_metrics.tsv').read().strip().splitlines()),
