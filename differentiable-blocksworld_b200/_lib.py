@@ -112,6 +112,14 @@ class DbwGatherField(ctypes.Structure):
     _fields_ = [('src', ctypes.c_void_p), ('dst', ctypes.c_void_p), ('words_per_view', ctypes.c_int64)]
 
 
+class DbwRansacResult(ctypes.Structure):
+    _fields_ = [('params', ctypes.c_float * 3), ('hypothesis', ctypes.c_int32), ('n_inliers', ctypes.c_int64),
+                ('n_improvements', ctypes.c_int32), ('reserved', ctypes.c_int32)]
+
+
+RANSAC_MAX_HYPOTHESES, RANSAC_MAX_SAMPLE = 2048, 64          # DBW_RANSAC_MAX_* of include/dbw_render.h
+
+
 EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generic_blocks_loss', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
            'dbw_render_forward_loss', 'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_camera_project', 'dbw_camera_project_backward',
@@ -133,7 +141,8 @@ EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generi
            'dbw_vertex_face_list', 'dbw_vertex_normals', 'dbw_render_forward_phong',
            'dbw_image_scores_workspace_bytes', 'dbw_image_scores',
            'dbw_texture_atlas_workspace_bytes', 'dbw_texture_atlas_u8',
-           'dbw_resample_u8_workspace_bytes', 'dbw_resample_u8', 'dbw_gather_views', 'dbw_subsample_points']
+           'dbw_resample_u8_workspace_bytes', 'dbw_resample_u8', 'dbw_gather_views', 'dbw_subsample_points',
+           'dbw_ransac_workspace_bytes', 'dbw_ransac_fit', 'dbw_ransac_count', 'dbw_ransac_select', 'dbw_ransac_filter']
 
 _lib = None
 
@@ -245,6 +254,11 @@ def lib():
         L.dbw_resample_u8.argtypes = [i32, i32, i32, vp, i32, i32, vp, vp, sz, vp]
         L.dbw_gather_views.argtypes = [i32, i32, vp, vp, i32, i32, vp, ctypes.POINTER(DbwGatherField), i32, vp]
         L.dbw_subsample_points.argtypes = [i64, i32, vp, i32, i32, vp, ctypes.c_uint64, ctypes.c_uint64, i64, vp, vp]
+        L.dbw_ransac_workspace_bytes.argtypes = [i64, i32, ctypes.POINTER(sz)]
+        L.dbw_ransac_fit.argtypes = [i64, vp, i32, i32, vp, vp, vp]
+        L.dbw_ransac_count.argtypes = [i64, vp, i32, vp, ctypes.c_float, vp, vp, sz, vp]
+        L.dbw_ransac_select.argtypes = [i32, i32, vp, vp, vp, vp]
+        L.dbw_ransac_filter.argtypes = [i64, vp, vp, ctypes.c_float, vp, vp, vp, vp, sz, vp]
         if L.dbw_sizeof_settings() != ctypes.sizeof(DbwRenderSettings):
             raise DbwError('DbwRenderSettings layout mismatch between the library and its ctypes mirror')
         if L.dbw_abi_version() != ABI_VERSION:

@@ -886,6 +886,52 @@ int dbw_gather_views(int32_t n_views, int32_t batch, const int64_t* idx, const u
 int dbw_subsample_points(int64_t n_points, int32_t row_words, const void* points, int32_t n_views, int32_t batch,
                          const int64_t* idx, uint64_t seed, uint64_t step, int64_t n_out, void* out, void* stream);
 
+/*
+ * RANSAC ground filter of the baseline preprocessing (the reference's Ransac(n_points=3, n_iter=100, batch_size=10,
+ * thresh=0.001) with LSLinearRegressor, src/utils/ransac.py, as src/dtu_3d_process.py:36-41 runs it): the plane
+ * z = a + b x + c y that the most points of a cloud lie within sqrt(thresh) of, in z.
+ *
+ * dbw_ransac_fit: per hypothesis h, (X^T X)^-1 X^T z of its n_sample points points[sample_idx[h n_sample + k]], X = [1, x, y],
+ *   in float64 (the inverse as adjugate / determinant), stored as float32 (a, b, c).  A singular X^T X (collinear or
+ *   repeated points: determinant exactly 0) gives NaN parameters, which count no inlier.  1 launch.
+ * dbw_ransac_count: counts[h] = #{i : (z_i - ((a + b x_i) + c y_i))^2 < thresh}, float32, each operation rounded on its own
+ *   (no FMA contraction); a point with a NaN coordinate is no inlier.  Integer CTA partials; the last CTA sums them.  1 launch
+ *   for all hypotheses (plus a 4-byte memset of the workspace's ticket).
+ * dbw_ransac_select: the reference's rule over rounds of batch_size hypotheses: a round's best is its first maximum, and it
+ *   replaces the running best only when strictly greater (the running best starts at 0 inliers).  `result` is the last such
+ *   best (best_models[-1]); hypothesis -1 when no hypothesis has an inlier (the reference then has no model).  1 launch.
+ * dbw_ransac_filter: the points that are NOT inliers of result's model, in input order (order-preserving compaction), into
+ *   `kept` (n_points rows at most; may be NULL), the inlier flags into `inlier` (may be NULL), and the kept count into
+ *   *n_kept.  A result with hypothesis -1 keeps every point.  3 launches.
+ *
+ *   points      DEVICE fp32 (n_points, 3) x y z;  sample_idx  DEVICE int64 (n_hyp, n_sample), each in [0, n_points)
+ *   params      DEVICE fp32 (n_hyp, 3);  counts  DEVICE int64 (n_hyp);  result  DEVICE DbwRansacResult
+ *   kept        DEVICE fp32 (n_points, 3);  inlier  DEVICE uint8 (n_points);  n_kept  DEVICE int64
+ *   workspace   caller-owned device memory of at least dbw_ransac_workspace_bytes(n_points, n_hyp) bytes
+ * n_points in [1, 2^31 - 1], n_hyp in [1, DBW_RANSAC_MAX_HYPOTHESES], n_sample in [3, DBW_RANSAC_MAX_SAMPLE], n_hyp a
+ * multiple of batch_size.
+ */
+#define DBW_RANSAC_MAX_HYPOTHESES 2048
+#define DBW_RANSAC_MAX_SAMPLE 64
+
+typedef struct DbwRansacResult {
+  float params[3];            /* a, b, c of the chosen hypothesis (NaN when there is none)                          */
+  int32_t hypothesis;         /* its index in [0, n_hyp), or -1                                                     */
+  int64_t n_inliers;          /* its count (0 when there is none)                                                   */
+  int32_t n_improvements;     /* how many times the running best was replaced (len(best_models))                   */
+  int32_t reserved;
+} DbwRansacResult;
+
+int dbw_ransac_workspace_bytes(int64_t n_points, int32_t n_hyp, size_t* bytes);
+int dbw_ransac_fit(int64_t n_points, const float* points, int32_t n_hyp, int32_t n_sample, const int64_t* sample_idx,
+                   float* params, void* stream);
+int dbw_ransac_count(int64_t n_points, const float* points, int32_t n_hyp, const float* params, float thresh, int64_t* counts,
+                     void* workspace, size_t workspace_bytes, void* stream);
+int dbw_ransac_select(int32_t n_hyp, int32_t batch_size, const int64_t* counts, const float* params, DbwRansacResult* result,
+                      void* stream);
+int dbw_ransac_filter(int64_t n_points, const float* points, const DbwRansacResult* result, float thresh, float* kept,
+                      uint8_t* inlier, int64_t* n_kept, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
