@@ -1673,7 +1673,7 @@ __device__ __forceinline__ void suffix_backward(const RasterParams& P, const flo
         const int bits = s_bits[k * stride], slot = bits & DBW_FRAG_SLOT_MASK;
         const int face = slot >= P.F ? slot - P.F : slot;
         if (want_alpha) { akey = alpha_index(P, alpha_in_smem ? 0 : view, face); aval = g_alpha * q.z; }
-        if (want_dist) {
+        if (want_dist && face >= P.n_static_faces) {        // a static face's vertices are constants
           // gradient w.r.t. the SIGNED squared distance: alpha = e(d) * fa, so fa * e = alpha
           const bool inside = !(bits & DBW_FRAG_OUTSIDE_BIT);
           float g_sd = 0.f;
