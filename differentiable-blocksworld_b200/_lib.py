@@ -121,6 +121,7 @@ RANSAC_MAX_HYPOTHESES, RANSAC_MAX_SAMPLE = 2048, 64          # DBW_RANSAC_MAX_* 
 
 
 EXPORTS = ['dbw_abi_version', 'dbw_debug_generic_kernel_only', 'dbw_debug_generic_blocks_loss', 'dbw_debug_keep_unread_outputs', 'dbw_sizeof_settings', 'dbw_last_error', 'dbw_workspace_bytes', 'dbw_render_forward', 'dbw_render_backward',
+           'dbw_render_forward_depth', 'dbw_render_backward_depth',
            'dbw_render_forward_loss', 'dbw_render_forward_loss_grad', 'dbw_render_backward_deferred',
            'dbw_camera_project', 'dbw_camera_project_backward',
            'dbw_composite_mse', 'dbw_composite_mse_backward', 'dbw_render_forward_host', 'dbw_host_arena_release', 'dbw_launch_count',
@@ -166,6 +167,8 @@ def lib():
         L.dbw_workspace_bytes.argtypes = [ctypes.POINTER(DbwRenderSettings), ctypes.POINTER(sz), ctypes.POINTER(sz)]
         L.dbw_render_forward.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, vp, vp, vp]
         L.dbw_render_backward.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz] + [vp] * 8 + [sz, vp]
+        L.dbw_render_forward_depth.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz] + [vp] * 5
+        L.dbw_render_backward_depth.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz] + [vp] * 10 + [sz, vp]
         L.dbw_render_forward_loss.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 12 + [sz, ctypes.POINTER(DbwLossEpilogue), vp]
         L.dbw_render_forward_loss_grad.argtypes = [ctypes.POINTER(DbwRenderSettings)] + [vp] * 10 + [sz, ctypes.POINTER(DbwLossEpilogue),
                                                                                                ctypes.c_int32, vp, sz, vp]

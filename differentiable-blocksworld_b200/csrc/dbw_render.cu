@@ -32,6 +32,7 @@
 #include "dbw_camera.cuh"
 #include "dbw_viz_math.cuh"
 #include "dbw_shade_math.cuh"
+#include "dbw_depth_math.cuh"
 
 // ------------------------------------------------------------------------------------------------ error plumbing
 static thread_local char g_err[512] = "";
@@ -641,6 +642,13 @@ struct RasterParams {
   // g_faces_alpha, which then point at the backward scratch
   int ep_grad;
 };
+// Depth outputs and their gradients (dbw_render_forward_depth / dbw_render_backward_depth): a kernel argument of the DEPTH
+// instantiations only, so that RasterParams -- and with it every other kernel -- is unchanged.
+struct DepthIO {
+  float* zbuf;               // (B,K,H,W) view-space depth of each kept fragment (-1 = empty) or NULL
+  float* depth;              // (B,1,H,W) the fragments' depths blended with the colour weights (background 0) or NULL
+  const float* g_zbuf; const float* g_depth;   // their gradients, multiplied by *grad_scale as read (either may be NULL)
+};
 
 // Raster CTAs: the 8x4-pixel patches of a CTA's warps tile a 16 x (NT / 16) pixel tile.  The backward kernels and the
 // K > 4 forward use 128 threads (finer scheduling granularity, less waiting on the slowest warp of a tile), the K <= 4
@@ -776,8 +784,12 @@ __device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4*
 // is staged in shared memory beside the opacity sums, so that the shading loop and the backward's pass 1 read no global
 // memory but the texels.  Every decision and every loss term is the generic instantiation's; the gradients differ only by
 // the order of their atomics.
-template <int NT, bool EP, bool BLOCKS>
-__device__ __forceinline__ void raster_forward_body(const RasterParams& P) {
+// DEPTH (depth_forward_kernel): also writes each kept fragment's depth (its pz, DepthIO.zbuf) and the depth blended with
+// the colour weights (DepthIO.depth), and keeps the records of the layers behind a fully opaque one too (their zbuf still has
+// a gradient); the image is the plain instantiation's bit for bit.
+template <int NT, bool EP, bool BLOCKS, bool DEPTH = false>
+__device__ __forceinline__ void raster_forward_body(const RasterParams& P, const DepthIO& Dz = DepthIO{}) {
+  static_assert(!DEPTH || !EP, "depth has no loss epilogue");
   static_assert(!BLOCKS || (EP && NT == 128), "the blocks loss pass is a loss-epilogue pass of 128 threads");
   // faces a tile lists at once (more: chunked path)
 #ifndef DBW_LIST_CAP
@@ -1003,6 +1015,7 @@ __device__ __forceinline__ void raster_forward_body(const RasterParams& P) {
   if (live) {
   // ---- shade + blend the sorted fragments front to back (layered_rgb_blend, Appendix B)
   float occ = 1.f, r = 0.f, g = 0.f, bl = 0.f;
+  float dep = 0.f;              // DEPTH: blended depth
   const size_t plane = (size_t)P.H * P.W;
   const size_t pix = (size_t)yi * P.W + xi;
   float ep_e[3] = {0.f, 0.f, 0.f}, ep_t[3] = {0.f, 0.f, 0.f};
@@ -1021,7 +1034,10 @@ __device__ __forceinline__ void raster_forward_body(const RasterParams& P) {
     const float d0 = e.z;
     if (!BLOCKS && P.topk) P.topk[((size_t)view * K + k) * plane + pix] = slot;
     if (!BLOCKS && P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = d0;
-    if (occ == 0.f) continue;     // behind a fully opaque fragment (fine phase: alpha = 1 inside a face): contributes exactly 0
+    if (DEPTH && Dz.zbuf) Dz.zbuf[((size_t)view * K + k) * plane + pix] = e.x;
+    // behind a fully opaque fragment (fine phase: alpha = 1 inside a face): contributes exactly 0 (DEPTH with records: the layer
+    // is still recorded, for the gradient of its zbuf; its weight is 0, so the blend is unchanged)
+    if (occ == 0.f && !(DEPTH && P.frag)) continue;
     n_saved = k + 1;
     const float v = lV[k * NT];
     const int face = slot >= P.F ? slot - P.F : slot;
@@ -1040,12 +1056,15 @@ __device__ __forceinline__ void raster_forward_body(const RasterParams& P) {
     }
     const float w = occ * a;
     r += w * tx.color.x; g += w * tx.color.y; bl += w * tx.color.z;
+    if (DEPTH) dep += w * e.x;
     occ *= (1.f - a);
   }
+  if (DEPTH && Dz.depth) Dz.depth[(size_t)view * plane + pix] = dep;
   if (!BLOCKS && P.nfrag) P.nfrag[(size_t)view * plane + pix] = (unsigned char)n_saved;
   for (int k = n; k < K; ++k) {
     if (!BLOCKS && P.topk) P.topk[((size_t)view * K + k) * plane + pix] = -1;
     if (!BLOCKS && P.out_dists) P.out_dists[((size_t)view * K + k) * plane + pix] = -1.f;
+    if (DEPTH && Dz.zbuf) Dz.zbuf[((size_t)view * K + k) * plane + pix] = -1.f;
   }
   float* o = P.out_rgba + (size_t)view * 4 * plane + pix;
   const float fc[3] = {r + occ * P.bg0, g + occ * P.bg1, bl + occ * P.bg2};
@@ -1099,6 +1118,11 @@ __global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_
   raster_forward_body<NT, EP, false>(P);
 }
 __global__ void __launch_bounds__(128, DBW_FWD_MINB) blocks_loss_kernel(const RasterParams P) { raster_forward_body<128, true, true>(P); }
+// the generic forward with the depth outputs (dbw_render_forward_depth)
+template <int NT>
+__global__ void __launch_bounds__(NT, NT <= 128 ? DBW_FWD_MINB : DBW_FWD_SMALLK_MINB) depth_forward_kernel(const RasterParams P, const DepthIO Dz) {
+  raster_forward_body<NT, false, false, true>(P, Dz);
+}
 
 // ------------------------------------------------------------------------------------------------ hard single-layer forward
 // K = 1, sigma = 0 (the environment pass, src/model/dbw.py:135-138,219; VizMeshRenderer's 4x supersampled renders,
@@ -1200,9 +1224,12 @@ __device__ __forceinline__ HardShade hard_shade_phong(const RasterParams& P, con
 }
 
 // PHONG: the Phong-shaded variants (phong_hard_forward_kernel, phong_resolve_hard_viz_kernel), which shade the winner with
-// hard_shade_phong; the code of the other instantiations is unchanged.
-template <bool VIZ, bool PHONG = false>
-__device__ __forceinline__ void hard_forward_body(const RasterParams& P, const VizOut& Z, const PhongIn& L = PhongIn{}) {
+// hard_shade_phong; the code of the other instantiations is unchanged.  DEPTH (depth_hard_forward_kernel): also the winner's
+// depth (DepthIO.zbuf, -1 where nothing is hit) and its depth times its opacity (DepthIO.depth, 0 where nothing is hit).
+template <bool VIZ, bool PHONG = false, bool DEPTH = false>
+__device__ __forceinline__ void hard_forward_body(const RasterParams& P, const VizOut& Z, const PhongIn& L = PhongIn{},
+                                                  const DepthIO& Dz = DepthIO{}) {
+  static_assert(!DEPTH || (!VIZ && !PHONG), "depth is a plain hard render's");
   __shared__ float4 s_bbox[HARD_CAP];
   __shared__ float4 s_rec[HARD_CAP * 4];
   __shared__ int s_slot[HARD_CAP];
@@ -1302,6 +1329,8 @@ __device__ __forceinline__ void hard_forward_body(const RasterParams& P, const V
     o[0] = P.bg0; o[plane] = P.bg1; o[2 * plane] = P.bg2; o[3 * plane] = 0.f;
     if (P.nfrag) P.nfrag[(size_t)view * plane + pix] = 0;
     if (P.topk) P.topk[(size_t)view * plane + pix] = -1;
+    if (DEPTH && Dz.zbuf) Dz.zbuf[(size_t)view * plane + pix] = -1.f;
+    if (DEPTH && Dz.depth) Dz.depth[(size_t)view * plane + pix] = 0.f;
     return;
   }
   if constexpr (PHONG) {         // no fragment records: a phong render has no backward
@@ -1344,9 +1373,18 @@ __device__ __forceinline__ void hard_forward_body(const RasterParams& P, const V
   const float occ = 1.f - a;
   o[0] = a * tx.color.x + occ * P.bg0; o[plane] = a * tx.color.y + occ * P.bg1; o[2 * plane] = a * tx.color.z + occ * P.bg2;
   o[3 * plane] = a;
+  if (DEPTH) {
+    const float z = __uint_as_float(best_pz);
+    if (Dz.zbuf) Dz.zbuf[(size_t)view * plane + pix] = z;
+    if (Dz.depth) Dz.depth[(size_t)view * plane + pix] = a * z;
+  }
 }
 
 __global__ void __launch_bounds__(HARD_NT, 5) raster_hard_forward_kernel(const RasterParams P) { hard_forward_body<false>(P, VizOut{}); }
+// the hard single-layer forward with the depth outputs (dbw_render_forward_depth)
+__global__ void __launch_bounds__(HARD_NT, 5) depth_hard_forward_kernel(const RasterParams P, const DepthIO Dz) {
+  hard_forward_body<false, false, true>(P, VizOut{}, PhongIn{}, Dz);
+}
 
 // The resolving variant renders the VizMeshRenderer frame (hard render on the 4H x 4W sample grid, avg_pool2d(., 4)) without
 // the sample image: a warp's 8 x 4 samples are the 4 x 4 samples of two frame pixels, which its lanes sum in registers.
@@ -1765,6 +1803,7 @@ __device__ __forceinline__ void epilogue_backward(const RasterParams& P, float4*
 #define DBW_BWD_TILES_KN 1
 
 // K1: faces_per_pixel == 1 (the environment pass): no record prefetch registers, at most one trip through the loops
+// depth_backward_kernel below is a copy of this walk with the depth terms: a fix here belongs there too.
 template <bool DETACH, bool ALPHA, bool K1>
 __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW_BWD_BARY_MINB) raster_backward_kernel(const RasterParams P) {
   extern __shared__ float4 s_dyn[];             // [k][tid] (alpha, cdot, e, occ), [k][tid] record bits, the map table, opacity sums
@@ -1889,6 +1928,176 @@ __global__ void __launch_bounds__(DBW_BWD_NT, DETACH ? DBW_BWD_DETACH_MINB : DBW
     if (P.g_maps4) warp_tex_scatter<K1>(P, tkey, t01, t10, t11, tcells, tg, tw, lane, warp);
     if (!DETACH) {
       if (__ballot_sync(0xffffffffu, key >= 0)) warp_agg_add<9>(P.g_tri + slot_base * 9, 9, key, gv9, lane);
+      if (__ballot_sync(0xffffffffu, ckey >= 0)) warp_agg_add<9>(P.g_conv + slot_base * 9, 9, ckey, gc9, lane);
+    }
+  }
+
+  // pass 2: suffix recurrence on the stored per-fragment scalars
+  suffix_backward(P, s_q, s_bits, DBW_BWD_NT, n, n_warp, p, gr, gg, gb, ga, view, slot_base, want_alpha, alpha_in_smem, s_galpha,
+                  want_dist, lane);
+  }   // tiles of the strip
+  if (alpha_in_smem) {               // one global atomic per (CTA, opacity entry) instead of one per (warp, layer, entry)
+    __syncthreads();
+    for (int i = tid; i < P.n_alpha; i += DBW_BWD_NT) {
+      const float v = s_galpha[i];
+      if (v != 0.f) atomicAdd(&P.g_faces_alpha[(size_t)view * P.alpha_stride + i], v);
+    }
+  }
+  if (K1 && DETACH && P.bary_flags) {
+    if (__syncthreads_or(need_bary) && tid == 0) P.bary_flags[((size_t)view * gridDim.y + blockIdx.y) * gridDim.z + strip] = 1;
+  }
+}
+
+// depth_backward_kernel (dbw_render_backward_depth): raster_backward_kernel with the gradients of the depth outputs too -- a
+// copy of its walk with the DEPTH branches, rather than DEPTH branches in it: routing raster_backward_kernel through a shared
+// body changes its instruction schedule.  d D / d w_k = z_k joins the colour's
+// d RGB / d w_k in cdot, so it takes the same opacity / distance chain through the suffix pass; each fragment's own depth
+// gets g_z = g_D w_k + g_zbuf_k, which depth_frag_backward takes to the slot's vertices -- with DETACH too (only the
+// barycentrics of the colour are detached).  The fragment's geometry is re-derived for its z.  Every recorded layer is visited,
+// also those behind a fully opaque one (the DEPTH forward records them: their zbuf has a gradient, their weight none).
+template <bool DETACH, bool ALPHA, bool K1>
+__global__ void __launch_bounds__(DBW_BWD_NT, DBW_BWD_BARY_MINB) depth_backward_kernel(const RasterParams P, const DepthIO Dz) {
+  constexpr bool DEPTH = true;
+  extern __shared__ float4 s_dyn[];             // [k][tid] (alpha, cdot, e, occ), [k][tid] record bits, the map table, opacity sums
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int view = blockIdx.x;
+  constexpr int DBW_BWD_TILES = K1 ? DBW_BWD_TILES_K1 : DBW_BWD_TILES_KN;
+  const int strip = centre_out(blockIdx.z, gridDim.z);          // DBW_BWD_TILES vertically adjacent 16 x 8 tiles per CTA
+  const int xi = blockIdx.y * TILE_W + (warp & 1) * 8 + (lane & 7);
+  int row_lo = 0, row_hi = P.H;
+  if (P.view_rows) { row_lo = P.view_rows[view * 2]; row_hi = P.view_rows[view * 2 + 1]; }
+  constexpr int TH = DBW_BWD_NT / 16;
+  if (strip * DBW_BWD_TILES * TH >= row_hi || (strip + 1) * DBW_BWD_TILES * TH <= row_lo) return;
+  const size_t plane = (size_t)P.H * P.W;
+  float4* const s_q = s_dyn + tid;
+  int* const s_bits = reinterpret_cast<int*>(s_dyn + (size_t)P.K * DBW_BWD_NT) + tid;
+  int4* const s_desc = reinterpret_cast<int4*>(reinterpret_cast<int*>(s_dyn + (size_t)P.K * DBW_BWD_NT) + (size_t)P.K * DBW_BWD_NT);
+  float* const s_galpha = reinterpret_cast<float*>(s_desc + P.M);
+  const float gs = P.grad_scale ? __ldg(P.grad_scale) : 1.f;
+  stage_map_table(P, s_desc, tid, DBW_BWD_NT);
+  const bool want_alpha = ALPHA && P.g_faces_alpha != nullptr;
+  const bool alpha_in_smem = want_alpha && P.n_alpha <= DBW_ALPHA_SMEM_MAX;       // few opacity entries: hot addresses
+  if (alpha_in_smem) for (int i = tid; i < P.n_alpha; i += DBW_BWD_NT) s_galpha[i] = 0.f;
+  const bool want_dist = P.sigma > 0.f && P.g_tri != nullptr;
+  // d loss / d alpha of the pixel feeds only the suffix pass; without it a zero alpha gradient changes no result (a pixel
+  // whose only non-zero gradient is alpha's contributes zeros), and the plane is not read -- a loss epilogue may not write it
+  const bool want_ga = want_alpha || want_dist;
+  const size_t slot_base = (size_t)view * 2 * P.F;
+  __syncthreads();
+
+  // Every warp walks ITS 8x4 patch of the strip's tiles on its own: no barrier between tiles, and the first-level loads of
+  // the next patch -- gradient pixel, fragment count, first record pair -- are issued before the current patch is processed,
+  // so that their DRAM latency is covered by work instead of by the other (few) resident warps.
+  struct First { float g0, g1, g2, g3; int n; float4 rec, rgb; };
+  auto load_first = [&](int t, First& f) {
+    f.g0 = f.g1 = f.g2 = f.g3 = 0.f; f.n = 0; f.rec = make_float4(0.f, 0.f, 0.f, 0.f); f.rgb = f.rec;
+    const int y = (strip * DBW_BWD_TILES + t) * TH + (warp >> 1) * 4 + (lane >> 3);
+    if (t < DBW_BWD_TILES && xi < P.W && y < P.H && y >= row_lo && y < row_hi) {
+      const size_t px = (size_t)y * P.W + xi;
+      const float* go = P.grad_rgba + (size_t)view * 4 * plane + px;
+      f.g0 = go[0]; f.g1 = go[plane]; f.g2 = go[2 * plane];
+      if (want_ga) f.g3 = go[3 * plane];
+      f.n = (int)P.nfrag[(size_t)view * plane + px];
+      f.rec = P.frag[(size_t)view * P.K * plane + px];          // speculative: a valid workspace address whether or not a
+      if (P.frag_rgb) f.rgb = P.frag_rgb[(size_t)view * P.K * plane + px];      // fragment exists (no colours: see keeps_colours)
+    }
+  };
+  First first_next;
+  load_first(0, first_next);
+  // DEPTH: the pixel's depth gradient, loaded one patch ahead as well
+  auto load_gd = [&](int t) -> float {
+    const int y = (strip * DBW_BWD_TILES + t) * TH + (warp >> 1) * 4 + (lane >> 3);
+    if (!DEPTH || !Dz.g_depth || t >= DBW_BWD_TILES || xi >= P.W || y >= P.H || y < row_lo || y >= row_hi) return 0.f;
+    return Dz.g_depth[(size_t)view * plane + (size_t)y * P.W + xi];
+  };
+  float gd_next = DEPTH ? load_gd(0) : 0.f;
+  bool need_bary = false;       // K1 && DETACH: this thread saw a fragment that raster_bary_backward_kernel must visit
+  for (int t = 0; t < DBW_BWD_TILES; ++t) {
+  const First first = first_next;
+  load_first(t + 1, first_next);
+  const float gd = gd_next * gs;
+  if (DEPTH) gd_next = load_gd(t + 1);
+  const int yi = (strip * DBW_BWD_TILES + t) * TH + (warp >> 1) * 4 + (lane >> 3);
+  const bool live = xi < P.W && yi < P.H && yi >= row_lo && yi < row_hi;
+  const size_t pix = live ? (size_t)yi * P.W + xi : 0;
+  const float4* frag = P.frag + (size_t)view * P.K * plane + pix;
+  const float4* frag_rgb = P.frag_rgb + (size_t)view * P.K * plane + pix;
+  const float gr = first.g0 * gs, gg = first.g1 * gs, gb = first.g2 * gs, ga = first.g3 * gs;
+  const bool any_grad = live && ((gr != 0.f) || (gg != 0.f) || (gb != 0.f) || (ga != 0.f) || (DEPTH && (gd != 0.f || Dz.g_zbuf)));
+  const int n_px = any_grad ? first.n : 0;
+  float4 rec_cur = first.rec, rgb_cur = first.rgb, rec_nxt = make_float4(0.f, 0.f, 0.f, 0.f), rgb_nxt = rec_nxt;
+  if (!K1 && n_px > 1) { rec_nxt = frag[plane]; rgb_nxt = frag_rgb[plane]; }
+  const f2 p = {pix_to_ndc(P.W - 1 - xi, P.W, P.H), pix_to_ndc(P.H - 1 - yi, P.H, P.W)};
+
+  // fragments are walked front to back until every lane of the warp has run out (warp-uniform trip count); the records of
+  // layers k+1 and k+2 are in flight while layer k is processed
+  int n_warp = n_px;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n_warp = max(n_warp, __shfl_xor_sync(0xffffffffu, n_warp, o));
+  int n = 0;
+  float occ = 1.f;
+  for (int k = 0; k < n_warp; ++k) {
+    const float4 fr = rec_cur, fc = rgb_cur;
+    if (!K1) {
+      rec_cur = rec_nxt; rgb_cur = rgb_nxt;
+      if (k + 2 < n_px) { rec_nxt = frag[(size_t)(k + 2) * plane]; rgb_nxt = frag_rgb[(size_t)(k + 2) * plane]; }
+    }
+    // everything behind a fully opaque fragment has zero weight and zero gradient (but for DEPTH, that of its zbuf)
+    const bool have = k < n_px && (DEPTH || occ != 0.f);
+    int key = -1, ckey = -1, tkey = -1, t01 = -1, t10 = -1, t11 = -1;
+    bool tcells = false;
+    float gv9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float gc9[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float tg[3] = {0.f, 0.f, 0.f}, tw[4] = {0.f, 0.f, 0.f, 0.f};      // texture gradient = tg x tw (colour x tap weights)
+    if (have) {
+      n = k + 1;
+      const int bits = __float_as_int(fr.x), slot = bits & DBW_FRAG_SLOT_MASK;
+      const int face = slot >= P.F ? slot - P.F : slot;
+      const float d = fr.w;
+      Texel4 tx;
+      Shade s;
+      const bool bary_path = !DETACH && face >= P.n_static_faces;
+      const int4 desc = s_desc[(unsigned)bits >> DBW_FRAG_MAP_SHIFT];
+      if (bary_path) {              // the gradient through (u, v) needs the four texels and the face's geometry again
+        shade_geometry(P, view, slot, p, s);
+        fetch_color(P, s.u, s.v, desc, tx);
+      } else {                      // texture / opacity / distance gradients: the saved colour and tap addresses suffice
+        if (DEPTH) shade_geometry(P, view, slot, p, s);          // (but not the fragment's depth)
+        tap_only(fr.y, fr.z, desc, tx);
+        tx.color = {fc.x, fc.y, fc.z};
+      }
+      const float e = frag_alpha(d, P.sigma, P.clip_inside);
+      const float fa = ALPHA ? __ldg(&P.faces_alpha[alpha_index(P, view, face)]) : 1.f;
+      const float a = e * fa;
+      float cdot = tx.color.x * gr + tx.color.y * gg + tx.color.z * gb;
+      if (DEPTH) cdot += s.b.pz * gd;          // the depth is a fourth colour channel with background 0
+      s_q[k * DBW_BWD_NT] = make_float4(a, cdot, e, occ);
+      s_bits[k * DBW_BWD_NT] = bits;
+      const float w = occ * a;                 // d RGB / d colour_k
+      if (w != 0.f) {
+        const float gcx = w * gr, gcy = w * gg, gcz = w * gb;
+        if (P.g_maps4) {
+          tkey = tx.tap.i00; t01 = tx.tap.i01; t10 = tx.tap.i10; t11 = tx.tap.i11; tcells = desc.w != 0;
+          tg[0] = gcx; tg[1] = gcy; tg[2] = gcz;
+          tw[0] = tx.tap.w00; tw[1] = tx.tap.w01; tw[2] = tx.tap.w10; tw[3] = tx.tap.w11;
+        }
+        if (bary_path && P.g_tri) {
+          key = slot;
+          if (bary_frag_backward(P, slot_base + slot, p, s, tx, gcx, gcy, gcz, gv9, gc9)) ckey = slot;
+        }
+      }
+      if (DEPTH && P.g_tri && face >= P.n_static_faces) {
+        const float g_pz = gd * w + (Dz.g_zbuf ? Dz.g_zbuf[((size_t)view * P.K + k) * plane + pix] * gs : 0.f);
+        if (g_pz != 0.f) { key = slot; depth_frag_backward(p, s.t, s.b, P.persp, P.clipb, g_pz, gv9); }
+      }
+      if (K1 && DETACH && face >= P.n_static_faces && w != 0.f) need_bary = true;
+      occ *= (1.f - a);
+    }
+    if (P.g_maps4) warp_tex_scatter<K1>(P, tkey, t01, t10, t11, tcells, tg, tw, lane, warp);
+    if (!DETACH || DEPTH) {
+      if (__ballot_sync(0xffffffffu, key >= 0)) warp_agg_add<9>(P.g_tri + slot_base * 9, 9, key, gv9, lane);
+    }
+    if (!DETACH) {
       if (__ballot_sync(0xffffffffu, ckey >= 0)) warp_agg_add<9>(P.g_conv + slot_base * 9, 9, ckey, gc9, lane);
     }
   }
@@ -2174,9 +2383,9 @@ static size_t frag_smem_bytes(int K, int NT, int M, int n_alpha = 0, int alpha_t
          (n_alpha <= DBW_ALPHA_SMEM_MAX ? (size_t)alpha_tables * n_alpha * sizeof(float) : 0);
 }
 
-// BLOCKS: blocks_loss_kernel, whose dispatch guarantees ep_grad and n_alpha <= DBW_ALPHA_SMEM_MAX
-template <int NT, bool BLOCKS = false>
-static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st) {
+// BLOCKS: blocks_loss_kernel, whose dispatch guarantees ep_grad and n_alpha <= DBW_ALPHA_SMEM_MAX; DEPTH: depth_forward_kernel
+template <int NT, bool BLOCKS = false, bool DEPTH = false>
+static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st, const DepthIO* depth = nullptr) {
   static_assert(!BLOCKS || NT == 128, "blocks_loss_kernel runs 128 threads");
   const dim3 grid(P.B, (P.W + TILE_W - 1) / TILE_W, (P.H + NT / 16 - 1) / (NT / 16));       // see centre_out()
   const size_t smem = BLOCKS ? frag_smem_bytes(P.K, NT, P.M, P.faces_alpha ? P.n_alpha : 0, 2)
@@ -2187,6 +2396,11 @@ static cudaError_t launch_forward(const RasterParams& P, cudaStream_t st) {
     return cudaSuccess;
   };
   if (BLOCKS) return go(blocks_loss_kernel);
+  if (DEPTH) {
+    if (smem > 40 * 1024) { cudaError_t e = cudaFuncSetAttribute(depth_forward_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); if (e != cudaSuccess) return e; }
+    depth_forward_kernel<NT><<<grid, NT, smem, st>>>(P, *depth);
+    return cudaSuccess;
+  }
   return P.ep_target ? go(raster_forward_kernel<NT, true>) : go(raster_forward_kernel<NT, false>);
 }
 
@@ -2198,7 +2412,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
                                void* stream, const EpilogueGrad* eg = nullptr, const VizOut* viz = nullptr,
-                               const PhongIn* phong = nullptr);
+                               const PhongIn* phong = nullptr, const DepthIO* depth = nullptr);
 
 extern "C" int dbw_render_forward(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
                                   const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
@@ -2250,7 +2464,8 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids, void* workspace,
                                size_t workspace_bytes, const float* face_shade, float* out_dists, const DbwLossEpilogue* ep,
-                               void* stream, const EpilogueGrad* eg, const VizOut* viz, const PhongIn* phong) {
+                               void* stream, const EpilogueGrad* eg, const VizOut* viz, const PhongIn* phong,
+                               const DepthIO* depth) {
   if (validate(s)) return -1;
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || (!out_rgba && !eg && !viz) || !workspace)
     return fail("dbw_render_forward: null pointer argument");
@@ -2321,6 +2536,7 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
       if (phong && viz) phong_resolve_hard_viz_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *viz, *phong);
       else if (phong) phong_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *phong);
       else if (viz) resolve_hard_viz_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *viz);
+      else if (depth) depth_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P, *depth);
       else raster_hard_forward_kernel<<<grid, HARD_NT, (size_t)P.M * sizeof(int4), st>>>(P);
     } else {
       // the coarse phase's blocks loss pass (K > 4) has a kernel of its own; anything it does not serve takes the generic one
@@ -2330,6 +2546,8 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
       if (blocks_loss) {
         ScopedTimer bl_timer(2, K, st);
         e = launch_forward<128, true>(P, st);
+      } else if (depth) {
+        e = K <= 4 ? launch_forward<DBW_FWD_NT_SMALLK, false, true>(P, st, depth) : launch_forward<DBW_FWD_NT, false, true>(P, st, depth);
       } else {
         e = K <= 4 ? launch_forward<DBW_FWD_NT_SMALLK>(P, st) : launch_forward<DBW_FWD_NT>(P, st);
       }
@@ -2338,6 +2556,27 @@ static int render_forward_impl(const DbwRenderSettings* s, const float* verts, c
   }
   LAUNCH_CK("raster_forward_kernel");
   return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ depth
+// what the depth entry points leave to dbw_render_forward / dbw_render_backward (NULL: nothing)
+static const char* depth_unsupported(const DbwRenderSettings& s) {
+  if (s.view_rows) return "row bands (view_rows) are not supported";
+  return nullptr;
+}
+
+extern "C" int dbw_render_forward_depth(const DbwRenderSettings* s, const float* verts, const int32_t* faces, const float* faces_uvs,
+                                        const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
+                                        const float* T, const float* faces_alpha, float* out_rgba, int32_t* topk_ids,
+                                        void* workspace, size_t workspace_bytes, const float* face_shade, float* out_dists,
+                                        float* out_zbuf, float* out_depth, void* stream) {
+  if (validate(s)) return -1;
+  const char* why = depth_unsupported(*s);
+  if (!why && face_shade) why = "lit renders (face_shade) are not supported";
+  if (why) { char msg[192]; snprintf(msg, sizeof(msg), "dbw_render_forward_depth: %s", why); return fail(msg); }
+  const DepthIO depth = {out_zbuf, out_depth, nullptr, nullptr};
+  return render_forward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, out_rgba, topk_ids,
+                             workspace, workspace_bytes, nullptr, out_dists, nullptr, stream, nullptr, nullptr, nullptr, &depth);
 }
 
 // ------------------------------------------------------------------------------------------------ resolving hard render
@@ -2444,27 +2683,62 @@ static int geometry_backward(const DbwRenderSettings& s, const Workspace& w, con
   return 0;
 }
 
+// g_zbuf / g_depth: the gradients of dbw_render_forward_depth's outputs (both NULL: the plain backward)
+static int render_backward_impl(const DbwRenderSettings* s_in, const float* verts, const int32_t* faces, const float* faces_uvs,
+                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
+                                const float* T, const float* faces_alpha, const void* workspace, size_t workspace_bytes,
+                                const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
+                                float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
+                                void* stream, const float* g_zbuf = nullptr, const float* g_depth = nullptr,
+                                const char* who = "dbw_render_backward");
+
 extern "C" int dbw_render_backward(const DbwRenderSettings* s_in, const float* verts, const int32_t* faces, const float* faces_uvs,
                                    const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
                                    const float* T, const float* faces_alpha, const void* workspace, size_t workspace_bytes,
                                    const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
                                    float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
                                    void* stream) {
+  return render_backward_impl(s_in, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, workspace,
+                              workspace_bytes, grad_rgba, grad_scale, g_verts, g_faces_alpha, g_maps, g_R, g_T, bwd_scratch,
+                              bwd_scratch_bytes, stream);
+}
+
+extern "C" int dbw_render_backward_depth(const DbwRenderSettings* s, const float* verts, const int32_t* faces,
+                                         const float* faces_uvs, const int32_t* face_map, const float* maps,
+                                         const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                                         const void* workspace, size_t workspace_bytes, const float* grad_rgba,
+                                         const float* grad_scale, const float* g_zbuf, const float* g_depth, float* g_verts,
+                                         float* g_faces_alpha, float* g_maps, float* g_R, float* g_T, void* bwd_scratch,
+                                         size_t bwd_scratch_bytes, void* stream) {
+  if (validate(s)) return -1;
+  if (const char* why = depth_unsupported(*s)) { char msg[192]; snprintf(msg, sizeof(msg), "dbw_render_backward_depth: %s", why); return fail(msg); }
+  return render_backward_impl(s, verts, faces, faces_uvs, face_map, maps, map_table, R, T, faces_alpha, workspace,
+                              workspace_bytes, grad_rgba, grad_scale, g_verts, g_faces_alpha, g_maps, g_R, g_T, bwd_scratch,
+                              bwd_scratch_bytes, stream, g_zbuf, g_depth, "dbw_render_backward_depth");
+}
+
+static int render_backward_impl(const DbwRenderSettings* s_in, const float* verts, const int32_t* faces, const float* faces_uvs,
+                                const int32_t* face_map, const float* maps, const DbwMapDesc* map_table, const float* R,
+                                const float* T, const float* faces_alpha, const void* workspace, size_t workspace_bytes,
+                                const float* grad_rgba, const float* grad_scale, float* g_verts, float* g_faces_alpha,
+                                float* g_maps, float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes,
+                                void* stream, const float* g_zbuf, const float* g_depth, const char* who) {
+  char msg[256];                 // error messages name the entry point (`who`)
   if (validate(s_in)) return -1;
   if (!verts || !faces || !faces_uvs || !face_map || !maps || !map_table || !workspace || !grad_rgba || !bwd_scratch)
-    return fail("dbw_render_backward: null pointer argument");
-  if (!s_in->save_fragment_state) return fail("dbw_render_backward: the forward must run with save_fragment_state = 1 or 2");
-  if (s_in->save_fragment_state == 2 && faces_alpha) return fail("dbw_render_backward: save_fragment_state = 2 declares a pass without faces_alpha");
+    { snprintf(msg, sizeof(msg), "%s: null pointer argument", who); return fail(msg); }
+  if (!s_in->save_fragment_state) { snprintf(msg, sizeof(msg), "%s: the forward must run with save_fragment_state = 1 or 2", who); return fail(msg); }
+  if (s_in->save_fragment_state == 2 && faces_alpha) { snprintf(msg, sizeof(msg), "%s: save_fragment_state = 2 declares a pass without faces_alpha", who); return fail(msg); }
   const bool cams = g_R != nullptr || g_T != nullptr;
-  if (cams && s_in->verts_are_ndc) return fail("dbw_render_backward: no camera gradient when verts_are_ndc (R and T are not used)");
-  if ((cams || (g_verts && !s_in->verts_are_ndc)) && (!R || !T)) return fail("dbw_render_backward: R and T are required unless verts_are_ndc");
+  if (cams && s_in->verts_are_ndc) { snprintf(msg, sizeof(msg), "%s: no camera gradient when verts_are_ndc (R and T are not used)", who); return fail(msg); }
+  if ((cams || (g_verts && !s_in->verts_are_ndc)) && (!R || !T)) { snprintf(msg, sizeof(msg), "%s: R and T are required unless verts_are_ndc", who); return fail(msg); }
   // every face moves in the image when the camera moves: a call with camera gradients differentiates the static faces too
   DbwRenderSettings s_local = *s_in;
   if (cams) s_local.n_static_faces = 0;
   const DbwRenderSettings* s = &s_local;
   Workspace w = carve(*s, (void*)workspace);
   BwdScratch g = carve_bwd(*s, bwd_scratch);
-  if (workspace_bytes < w.total || bwd_scratch_bytes < g.total) return fail("dbw_render_backward: workspace too small");
+  if (workspace_bytes < w.total || bwd_scratch_bytes < g.total) { snprintf(msg, sizeof(msg), "%s: workspace too small", who); return fail(msg); }
   cudaStream_t st = (cudaStream_t)stream;
   const bool need_geom = g_verts != nullptr || cams;     // both are reductions of the per-view NDC vertex gradient
   CK(cudaMemsetAsync(bwd_scratch, 0, g.total, st));
@@ -2473,6 +2747,8 @@ extern "C" int dbw_render_backward(const DbwRenderSettings* s_in, const float* v
   P.map_table = map_table;
   P.grad_rgba = grad_rgba; P.grad_scale = grad_scale; P.g_tri = need_geom ? g.g_tri : nullptr; P.g_conv = g.g_conv;
   P.g_faces_alpha = g_faces_alpha; P.g_maps4 = g_maps ? (s->maps_are_texels4 ? (float4*)g_maps : g.g_maps4) : nullptr;
+  const DepthIO dz = {nullptr, nullptr, g_zbuf, g_depth};
+  const bool dep = g_zbuf != nullptr || g_depth != nullptr;
   const int n_entries = s->n_map_floats / 3;
   if (g_maps && s->maps_are_texels4 == 2) { P.g_cells = g.g_cells; P.n_cells = n_entries; }
   const dim3 grid = bwd_grid(*s);        // see centre_out()
@@ -2484,14 +2760,25 @@ extern "C" int dbw_render_backward(const DbwRenderSettings* s_in, const float* v
       kern<<<grid, DBW_BWD_NT, smem, st>>>(P);
       return cudaSuccess;
     };
+    auto launch_depth = [&](auto kern) -> cudaError_t {
+      if (smem > 40 * 1024) { cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); if (e != cudaSuccess) return e; }
+      kern<<<grid, DBW_BWD_NT, smem, st>>>(P, dz);
+      return cudaSuccess;
+    };
     const bool det = s->detach_bary != 0, al = faces_alpha != nullptr, k1 = s->faces_per_pixel == 1;
     // A single-layer pass that is not detached runs as the detached kernel (texture, opacity and distance gradients of
     // every pixel) plus raster_bary_backward_kernel over the strips that hold faces with vertex gradients
     const bool split = k1 && !det && need_geom;
     if (split) P.bary_flags = g.bary_flags;
-    cudaError_t e = k1  ? (al ? launch(raster_backward_kernel<true, true, true>) : launch(raster_backward_kernel<true, false, true>))
-                  : det ? (al ? launch(raster_backward_kernel<true, true, false>) : launch(raster_backward_kernel<true, false, false>))
-                        : (al ? launch(raster_backward_kernel<false, true, false>) : launch(raster_backward_kernel<false, false, false>));
+    cudaError_t e;
+    if (!dep)
+      e = k1  ? (al ? launch(raster_backward_kernel<true, true, true>) : launch(raster_backward_kernel<true, false, true>))
+        : det ? (al ? launch(raster_backward_kernel<true, true, false>) : launch(raster_backward_kernel<true, false, false>))
+              : (al ? launch(raster_backward_kernel<false, true, false>) : launch(raster_backward_kernel<false, false, false>));
+    else        // the same dispatch; the split single-layer pass keeps raster_bary_backward_kernel for the colour's barycentrics
+      e = k1  ? (al ? launch_depth(depth_backward_kernel<true, true, true>) : launch_depth(depth_backward_kernel<true, false, true>))
+        : det ? (al ? launch_depth(depth_backward_kernel<true, true, false>) : launch_depth(depth_backward_kernel<true, false, false>))
+              : (al ? launch_depth(depth_backward_kernel<false, true, false>) : launch_depth(depth_backward_kernel<false, false, false>));
     if (e != cudaSuccess) return fail("raster_backward_kernel attribute", e);
     LAUNCH_CK("raster_backward_kernel");
     if (split) {

@@ -284,8 +284,9 @@ class DifferentiableBlocksWorld(nn.Module):
         fine = not self.is_live('coarse_learning')
         return fine, (filter_transparent or fine), (self.renderer_fine if fine else self.renderer)
 
-    def _render_layers(self, inp, filter_transparent=False):
-        """(environment RGBA, blocks RGBA) in decoupled mode (every shipped config), (whole-scene RGBA, None) otherwise"""
+    def _render_layers(self, inp, filter_transparent=False, depth=False):
+        """(environment RGBA, blocks RGBA) in decoupled mode (every shipped config), (whole-scene RGBA, None) otherwise.
+        depth: each RGBA comes as (RGBA, depth (B,1,H,W)) from the same pass (Renderer.forward(depth=True))"""
         B, R, T, K = len(inp['imgs']), inp['R'], inp['T'], self._view_K(inp)
         self._install_cameras(inp)
         fine, hard_filter, renderer = self._phase(filter_transparent)
@@ -294,20 +295,23 @@ class DifferentiableBlocksWorld(nn.Module):
             alpha = None
             if not hard_filter:
                 alpha = torch.cat([torch.ones(self.env_n_faces, device=R.device), self._alpha.repeat_interleave(self.BNF)])
-            return renderer(scene.extend(B), R=R, T=T, faces_alpha=alpha, K=K), None
+            return renderer(scene.extend(B), R=R, T=T, faces_alpha=alpha, K=K, depth=depth), None
         if self._fused_scene_ok(R):
-            return self._render_decoupled_fused(R, T, hard_filter, renderer, K)
+            return self._render_decoupled_fused(R, T, hard_filter, renderer, K, depth)
         env = join_meshes_as_scene([self.build_bkg(world_coord=True), self.build_ground(world_coord=True)])
-        env_rgba = self.renderer_env(env.extend(B), R=R, T=T, K=K)
+        env_rgba = self.renderer_env(env.extend(B), R=R, T=T, K=K, depth=depth)
         if self.static_topology:
             verts, faces, fvu, fmap, maps, table = self._blocks_static(hard_filter)
             alpha = None if hard_filter else self._alpha.repeat_interleave(self.BNF)
-            return env_rgba, self._raster(renderer, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4=False, K=K)
+            return env_rgba, self._raster(renderer, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4=False, K=K,
+                                          depth=depth)
         blocks = self.build_blocks(filter_transparent=hard_filter, as_scene=True)
         if len(blocks) == 0:
+            if depth:
+                return env_rgba, (torch.zeros_like(env_rgba[0]), torch.zeros_like(env_rgba[1]))
             return env_rgba, torch.zeros_like(env_rgba)
         alpha = None if hard_filter else self._alpha.repeat_interleave(self.BNF)
-        return env_rgba, renderer(blocks.extend(B), R=R, T=T, faces_alpha=alpha, K=K)
+        return env_rgba, renderer(blocks.extend(B), R=R, T=T, faces_alpha=alpha, K=K, depth=depth)
 
     def _fused_scene_ok(self, ref):
         """the fused scene kernels apply: static topology on the GPU, and a box decimation the texture-prep kernel has
@@ -316,12 +320,13 @@ class DifferentiableBlocksWorld(nn.Module):
         return (self.static_topology and self.fused_scene and ref.is_cuda and (not decim_live or self.decim_factor in (1, 8)))
 
     @staticmethod
-    def _raster(r, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4, alpha_group=1, n_static_faces=0, K=None):
+    def _raster(r, verts, faces, fvu, fmap, maps, table, R, T, alpha, texels4, alpha_group=1, n_static_faces=0, K=None,
+                depth=False):
         intr = K if K is not None else r.cameras.intrinsics()          # K (B,4,4): per-view intrinsics (render_scene)
         return render_scene(verts, faces, fvu, fmap, maps, table, R, T, intr, r.img_size, r.sigma,
                             r.faces_per_pixel, r.z_clip, r.detach_bary, r.clip_inside, r.background_color, alpha,
                             r.perspective_correct, blur_radius=r.blur_radius, maps_are_texels4=texels4,
-                            alpha_group=alpha_group, n_static_faces=n_static_faces)
+                            alpha_group=alpha_group, n_static_faces=n_static_faces, return_depth=depth)
 
     @staticmethod
     def _composite(env_rgba, fg_rgba):
@@ -436,14 +441,14 @@ class DifferentiableBlocksWorld(nn.Module):
             alpha = alpha[:, None].expand(-1, self.BNF).reshape(-1)
         return alpha
 
-    def _render_decoupled_fused(self, R, T, hard_filter, renderer, K=None):
-        """environment pass + blocks pass over the fused scene tensors -> (env RGBA, blocks RGBA)"""
+    def _render_decoupled_fused(self, R, T, hard_filter, renderer, K=None, depth=False):
+        """environment pass + blocks pass over the fused scene tensors -> (env RGBA, blocks RGBA) [each with its depth]"""
         st = self._static_arrays()
         (env_verts, env_atlas, env_table), (blk_verts, atlas, table, fmap, alpha) = self._scene_tensors(hard_filter)
         env_rgba = self._raster(self.renderer_env, env_verts, st['faces_e'], st['fvu_e'], st['fmap_e'], env_atlas, env_table,
-                                R, T, None, texels4=True, n_static_faces=self.bkg_n_faces, K=K)
+                                R, T, None, texels4=True, n_static_faces=self.bkg_n_faces, K=K, depth=depth)
         fg_rgba = self._raster(renderer, blk_verts, st['faces_b'], st['fvu_b'], fmap, atlas, table, R, T, alpha, texels4=True,
-                               alpha_group=self.alpha_group_faces or self.BNF, K=K)
+                               alpha_group=self.alpha_group_faces or self.BNF, K=K, depth=depth)
         return env_rgba, fg_rgba
 
     def _fused_loss_ok(self, imgs):
@@ -586,8 +591,22 @@ class DifferentiableBlocksWorld(nn.Module):
         return Meshes(self._to_world(verts[None]), faces[None], scene.textures)
 
     # ------------------------------------------------------------------ prediction / visualisation
-    def predict(self, inp, labels=None, w_edges=False, filter_transparent=False):
-        rec = self._composite(*self._render_layers(inp, filter_transparent))
+    def predict(self, inp, labels=None, w_edges=False, filter_transparent=False, with_depth=False):
+        """the reconstruction (B,3,H,W); with_depth=True: (rec, depth), depth (B,1,H,W) from the same passes, composited the way
+        rec is -- D_fg + (1 - alpha_fg) D_env in decoupled mode, the single pass's in joint mode -- where each pass's D is its
+        fragments' view-space z blended with its colour weights over a background of 0.  Both are differentiable, to the scene
+        parameters, the opacities, the poses and per-view intrinsics."""
+        depth = None
+        if with_depth:
+            env, fg = self._render_layers(inp, filter_transparent, depth=True)
+            if fg is None:
+                rec, depth = env[0][:, :3], env[1]
+            else:
+                cover = fg[0][:, 3:]
+                rec = self._composite(env[0], fg[0])
+                depth = fg[1] + (1 - cover) * env[1]
+        else:
+            rec = self._composite(*self._render_layers(inp, filter_transparent))
         if w_edges:                                   # dbw.py:234-238: coloured face edges drawn over the reconstruction
             B = len(inp['imgs'])
             _, hard_filter, renderer = self._phase(filter_transparent)
@@ -597,7 +616,11 @@ class DifferentiableBlocksWorld(nn.Module):
                 parts.append(blocks)
             colors = self.get_scene_face_colors(filter_transparent=hard_filter).repeat(B, 1)
             rec = renderer.draw_edges(rec, join_meshes_as_scene(parts).extend(B), inp['R'], inp['T'], colors=colors, K=self._view_K(inp))
-        return rec
+        return (rec, depth) if with_depth else rec
+
+    def predict_depth(self, inp, filter_transparent=False):
+        """the composited depth (B,1,H,W) of predict(inp, with_depth=True), differentiable"""
+        return self.predict(inp, filter_transparent=filter_transparent, with_depth=True)[1]
 
     def predict_synthetic(self, inp, labels=None):
         """flat-shaded render of the opaque blocks with one synthetic colour per block (dbw.py:241-248)"""

@@ -131,6 +131,74 @@ class _RenderFn(torch.autograd.Function):
         return g_verts, g_maps, g_fa, g_R, g_T, None, None, None, None, None, None, None, None
 
 
+class _RenderDepthFn(torch.autograd.Function):
+    """autograd seam over dbw_render_forward_depth / dbw_render_backward_depth (include/dbw_render.h): the render of _RenderFn
+    -- the same RGBA bits -- with the blended depth (B,1,H,W) and the per-fragment zbuf (B,K,H,W) as differentiable outputs.
+    Outputs: rgba, then ids (also when only dists are asked, as _RenderFn) and dists (not differentiable), then depth and zbuf."""
+
+    @staticmethod
+    def forward(ctx, verts, maps, faces_alpha, R, T, faces, faces_uvs, face_map, map_table, cfg, want_depth, want_zbuf,
+                want_ids=False, want_dists=False):
+        if not verts.is_cuda:
+            raise DbwError('the CUDA renderer needs CUDA tensors (there is no CPU fallback)')
+        ctx.set_materialize_grads(False)
+        s = cfg
+        B, H, W, K = s.n_views, s.height, s.width, s.faces_per_pixel
+        L = _lib.lib()
+        verts, maps = verts.detach().contiguous().float(), maps.detach().contiguous().float()
+        fa = faces_alpha.detach().contiguous().float() if faces_alpha is not None else None
+        R, T = R.detach().contiguous().float(), T.detach().contiguous().float()
+        fwd, bwd = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        _lib.check(L.dbw_workspace_bytes(ctypes.byref(s), ctypes.byref(fwd), ctypes.byref(bwd)), 'dbw_workspace_bytes')
+        dev = verts.device
+        ws = torch.empty(fwd.value, dtype=torch.uint8, device=dev)
+        out = torch.empty(B, 4, H, W, dtype=torch.float32, device=dev)
+        ids = torch.empty(B, K, H, W, dtype=torch.int32, device=dev) if (want_ids or want_dists) else None
+        dists = torch.empty(B, K, H, W, dtype=torch.float32, device=dev) if want_dists else None
+        depth = torch.empty(B, 1, H, W, dtype=torch.float32, device=dev) if want_depth else None
+        zbuf = torch.empty(B, K, H, W, dtype=torch.float32, device=dev) if want_zbuf else None
+        _lib.check(L.dbw_render_forward_depth(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
+                                              _c(map_table), _c(R), _c(T), _c(fa), _c(out), _c(ids), _c(ws), fwd.value, None,
+                                              _c(dists), _c(zbuf), _c(depth), _stream()), 'dbw_render_forward_depth')
+        ctx.save_for_backward(verts, maps, fa, R, T, faces, faces_uvs, face_map, map_table, ws)
+        ctx.cfg, ctx.bwd_bytes = s, bwd.value
+        extras = [t for t in (ids, dists) if t is not None]           # _RenderFn's layout: ids whenever dists are returned
+        ctx.mark_non_differentiable(*extras)
+        ctx.n_extras, ctx.want_depth = len(extras), want_depth
+        return (out, *extras, *[t for t in (depth, zbuf) if t is not None])
+
+    @staticmethod
+    def backward(ctx, g_out, *grads):
+        verts, maps, fa, R, T, faces, faces_uvs, face_map, map_table, ws = ctx.saved_tensors
+        s = ctx.cfg
+        if not s.save_fragment_state:
+            raise DbwError('this render was made with gradients disabled (no fragment records were kept)')
+        grads = list(grads[ctx.n_extras:])
+        g_depth = grads.pop(0) if ctx.want_depth else None
+        g_zbuf = grads.pop(0) if grads else None
+        L = _lib.lib()
+        dev = verts.device
+        # outputs nothing read have no gradient (None); with neither depth gradient this is dbw_render_backward
+        g_out = torch.zeros(s.n_views, 4, s.height, s.width, device=dev) if g_out is None else g_out.contiguous().float()
+        g_depth = g_depth.contiguous().float() if g_depth is not None else None
+        g_zbuf = g_zbuf.contiguous().float() if g_zbuf is not None else None
+        need = ctx.needs_input_grad
+        g_verts = torch.zeros_like(verts) if need[0] else None
+        g_maps = torch.zeros_like(maps) if need[1] else None
+        g_fa = torch.zeros_like(fa) if need[2] and fa is not None else None
+        g_R = g_T = None
+        if need[3] or need[4]:
+            if s.verts_are_ndc:
+                raise DbwError('R and T are not part of a render from NDC vertices (verts_are_ndc): they have no gradient')
+            g_R, g_T = torch.zeros_like(R) if need[3] else None, torch.zeros_like(T) if need[4] else None
+        scratch = torch.empty(ctx.bwd_bytes, dtype=torch.uint8, device=dev)
+        _lib.check(L.dbw_render_backward_depth(ctypes.byref(s), _c(verts), _c(faces), _c(faces_uvs), _c(face_map), _c(maps),
+                                               _c(map_table), _c(R), _c(T), _c(fa), _c(ws), ws.numel(), _c(g_out), None,
+                                               _c(g_zbuf), _c(g_depth), _c(g_verts), _c(g_fa), _c(g_maps), _c(g_R), _c(g_T),
+                                               _c(scratch), scratch.numel(), _stream()), 'dbw_render_backward_depth')
+        return (g_verts, g_maps, g_fa, g_R, g_T) + (None,) * 9
+
+
 class _ProjectFn(torch.autograd.Function):
     """autograd seam over dbw_camera_project / dbw_camera_project_backward (include/dbw_render.h)."""
 
@@ -284,13 +352,19 @@ def scene_settings(verts, faces, maps, map_table_host, B, intr, image_size, sigm
 def render_scene(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, intr, image_size, sigma, faces_per_pixel,
                  z_clip=None, detach_bary=False, clip_inside=True, background=(0., 0., 0.), faces_alpha=None,
                  perspective_correct=True, verts_are_ndc=False, blur_radius=None, return_ids=False, maps_are_texels4=False,
-                 face_shade=None, return_dists=False, alpha_group=1, n_static_faces=0, view_rows=None):
+                 face_shade=None, return_dists=False, alpha_group=1, n_static_faces=0, view_rows=None, return_depth=False,
+                 return_zbuf=False):
     """Functional form over raw tensors (used by Renderer.forward and by the parity tests).
     verts (V,3) [or (B,V,3) NDC], faces (F,3) int32, faces_uvs (F,3,2), face_map (F) int32, maps flat float buffer,
     map_table_host [(offset,H,W)], R (B,3,3), T (B,3), faces_alpha None | (F,) | (B*F,).
     intr: (fx, fy, px, py) floats shared by every view, or a tensor K (B,4,4) of per-view intrinsics: the world vertices are
     then projected per view on the device (project_verts) and rendered as NDC input; R, T and K receive gradients.
-    maps_are_texels4: `maps` is a float4 (RGB+pad) texel atlas from scene_ops.scene_atlases (offsets stay 3*texel)."""
+    maps_are_texels4: `maps` is a float4 (RGB+pad) texel atlas from scene_ops.scene_atlases (offsets stay 3*texel).
+    return_depth / return_zbuf: also the blended depth (B,1,H,W) -- layered_rgb_blend of the fragments' view-space z with
+    background 0, so depth / alpha is the expected depth of the covered part -- and the per-fragment depth (B,K,H,W)
+    (PyTorch3D's fragments.zbuf, planar like the ids; -1 in empty slots), appended to the outputs in that order.  Both are
+    differentiable, to the same leaves as the image, also with detach_bary; the image is the same bits as without them.
+    Not with face_shade or view_rows."""
     if torch.is_tensor(intr):
         if verts_are_ndc or R is None:
             raise DbwError('per-view intrinsics project world vertices: they need R and T, and verts_are_ndc=False')
@@ -305,9 +379,14 @@ def render_scene(verts, faces, faces_uvs, face_map, maps, map_table_host, R, T, 
     if R is None:
         R = torch.eye(3, device=dev)[None].expand(B, -1, -1)
         T = torch.zeros(B, 3, device=dev)
-    res = _RenderFn.apply(verts, maps, faces_alpha, R, T, faces.to(torch.int32).contiguous(),
-                          faces_uvs.contiguous().float(), face_map.to(torch.int32).contiguous(), map_table, cfg,
-                          face_shade, return_dists, return_ids)
+    args = (verts, maps, faces_alpha, R, T, faces.to(torch.int32).contiguous(), faces_uvs.contiguous().float(),
+            face_map.to(torch.int32).contiguous(), map_table, cfg)
+    if return_depth or return_zbuf:
+        if face_shade is not None:
+            raise NotImplementedError('depth of a lit (flat-shaded) render is not implemented')
+        # (rgba, [slot ids], [signed squared distances], [depth], [zbuf])
+        return _RenderDepthFn.apply(*args, bool(return_depth), bool(return_zbuf), bool(return_ids), bool(return_dists))
+    res = _RenderFn.apply(*args, face_shade, return_dists, return_ids)
     return res                           # rgba | (rgba, slot ids) | (rgba, slot ids, signed squared distances)
 
 
@@ -589,8 +668,12 @@ class Renderer(nn.Module):
                                       'only raw+ambient (training) and flat+directional (renderer_light) are implemented')
         return self._flat_shade(verts, faces, R) if lit else None
 
-    def forward(self, meshes, R, T, viz_purpose=False, **kwargs):
+    def forward(self, meshes, R, T, viz_purpose=False, depth=False, **kwargs):
+        """(B,4,H,W) RGBA; with depth=True (rgba, depth): depth (B,1,H,W) is the fragments' view-space z blended with the colour
+        weights over a background of 0 (depth / alpha: the expected depth of the covered part), differentiable like the image"""
         faces_alpha, K = kwargs.get('faces_alpha'), kwargs.get('K')
+        if depth and (viz_purpose or self.shading_type != 'raw'):
+            raise NotImplementedError('depth=True is a training render: raw shading, viz_purpose=False')
         if self.shading_type == 'phong':
             if viz_purpose:          # VizMeshRenderer's frame, resolved in the kernel: the bits of avg_pool2d(render at 4x, 4)
                 with torch.no_grad():
@@ -612,7 +695,7 @@ class Renderer(nn.Module):
                 return F.avg_pool2d(out, kernel_size=4, stride=4)
         return render_scene(verts, faces, fvu, fmap, maps, table, R, T, intr, (H, W), self.sigma, self.faces_per_pixel,
                             self.z_clip, self.detach_bary, self.clip_inside, self.background_color, faces_alpha,
-                            self.perspective_correct, blur_radius=self.blur_radius, face_shade=shade)
+                            self.perspective_correct, blur_radius=self.blur_radius, face_shade=shade, return_depth=depth)
 
     @torch.no_grad()
     def render_viz(self, meshes, R, T, K=None, bkg=None, frames_u8=False):

@@ -188,6 +188,35 @@ int dbw_render_backward(const DbwRenderSettings* settings, const float* verts, c
                         void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
 
 /*
+ * Depth: dbw_render_forward / dbw_render_backward with PyTorch3D's fragments.zbuf and its layered blend as two more outputs,
+ * differentiable.  Arguments are those of the plain entry points, plus:
+ *   out_zbuf   (B,K,H,W) or NULL: view-space z of each kept fragment's point (= fragments.zbuf): its triangle's vertex depths
+ *              interpolated with the barycentrics the render interpolates with (perspective-corrected when
+ *              perspective_correct, clipped when clip_barycentric); for a z-clipped face, of the clipped triangle; -1 in empty slots
+ *   out_depth  (B,1,H,W) or NULL: layered_rgb_blend of zbuf as a one-channel colour with background 0 -- the weights of the
+ *              RGB channels (occlusion x opacity) times each fragment's z, summed.  depth / alpha is the expected depth of the
+ *              covered part; a hard single layer (sigma = 0, K = 1) gives the winner's z times its opacity
+ *   g_zbuf, g_depth  (backward) gradients of the two outputs (either may be NULL; both NULL = dbw_render_backward), multiplied
+ *              by *grad_scale like grad_rgba.  They reach the weights (opacities, distances) as a fourth colour channel does,
+ *              and each fragment's z reaches its face's vertices through the z interpolation, the z-clip, face setup and
+ *              projection -- g_verts, g_R, g_T -- also with detach_bary (which detaches the colour's barycentrics only)
+ * out_rgba is the image dbw_render_forward writes, bit for bit.  With save_fragment_state the forward also records the layers
+ * behind a fully opaque fragment (their zbuf has a gradient); dbw_render_backward on such a workspace gives the plain gradient.
+ * Refused: view_rows, face_shade (lit renders).  The loss epilogue (dbw_render_forward_loss*) has no depth.
+ */
+int dbw_render_forward_depth(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
+                             const float* faces_uvs, const int32_t* face_map, const float* maps,
+                             const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                             float* out_rgba, int32_t* topk_ids, void* workspace, size_t workspace_bytes,
+                             const float* face_shade, float* out_dists, float* out_zbuf, float* out_depth, void* stream);
+int dbw_render_backward_depth(const DbwRenderSettings* settings, const float* verts, const int32_t* faces,
+                              const float* faces_uvs, const int32_t* face_map, const float* maps,
+                              const DbwMapDesc* map_table, const float* R, const float* T, const float* faces_alpha,
+                              const void* workspace, size_t workspace_bytes, const float* grad_rgba, const float* grad_scale,
+                              const float* g_zbuf, const float* g_depth, float* g_verts, float* g_faces_alpha, float* g_maps,
+                              float* g_R, float* g_T, void* bwd_scratch, size_t bwd_scratch_bytes, void* stream);
+
+/*
  * Phong shading (PyTorch3D phong_shading as the reference's LayeredShader calls it, src/model/renderer.py:187-238; its
  * eye_light views, renderer.py:301-310,343-351).  Forward only: there is no backward of a phong render.
  *
